@@ -3,7 +3,7 @@
     python bench.py [--gpus N] [--steps K] [--warmup W] [--model base|large] [--impl ours|reference]
 
 Workload = the model BASELINE.json's metric names: WavLM-Large, batch 8 x 20 s synthetic 16 kHz waveform per GPU (configs[2]'s
-per-GPU batch; it fits one B200), masking on, fwd + bwd of the whole encoder through the public API (`WavLM.extract_features` +
+per-GPU batch; it fits one 80 GB H100), masking on, fwd + bwd of the whole encoder through the public API (`WavLM.extract_features` +
 probe loss + `backward()`), bf16 kernels, dropout 0 as in BASELINE.md section 3.  At N=1 the line also carries, under `also`,
 WavLM-Base 16 x 15 s (configs[1]) and the same Large workload with the reference's default dropouts (0.1 / 0.1).
 N>1 (launched with torch.distributed.run): same per-GPU batch (weak scaling), plus the gradient average of the flat fp32
@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import argparse
 import json
+import random
 import os
 import subprocess
 import sys
@@ -29,6 +30,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 SR = 16000
@@ -42,7 +44,7 @@ def model_config(name: str):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index, self.rows, self.proc = index, [], None
@@ -279,7 +281,8 @@ class Workload:
             return self.pretrain_step(wav, e2e, collective)
         self._mark("start")
         nvtx.range_push("forward")
-        x, _ = model.extract_features(wav, padding_mask=self.pad_host, mask=True)
+        x, fpm = model.extract_features(wav, padding_mask=self.pad_host, mask=True)
+        self.last_x, self.last_fpm = x, fpm
         loss = (x.float() * self.R).sum()
         nvtx.range_pop()
         self._mark("forward")
@@ -295,6 +298,7 @@ class Workload:
         self._mark("reduce-grads")
         if e2e:
             self.loss_host.copy_(loss.detach().reshape(1), non_blocking=True)
+        self.last_loss = loss
         return loss
 
     def pretrain_step(self, wav, e2e: bool, collective: bool):
@@ -305,6 +309,7 @@ class Workload:
         self._mark("start")
         nvtx.range_push("forward")
         out = model(wav, target_list=self.labels, padding_mask=self.pad_host, mask=True)
+        self.last_x = self.last_fpm = None
         lw = [10.0, 10.0, 0.0, 0.1] if self.sat else [10.0]   # features_pen, loss_spk_m, loss_spk_u, diversity (prob_perplexity)
         loss, sample_size, _ = model.criterion(out, pred_masked_weight=1.0, pred_nomask_weight=0.0, loss_weights=lw)
         nvtx.range_pop()
@@ -332,7 +337,38 @@ class Workload:
         self._mark("optimizer")
         if e2e:
             self.loss_host.copy_(loss.detach().reshape(1), non_blocking=True)
+        self.last_loss = loss
         return loss
+
+    def dump_outputs(self, out_dir: str, max_bytes: int = 64 << 20):
+        """Write what the last step handed its caller as float32 .npy files: the loss, the encoder output (fwd+bwd workloads)
+        and, per parameter, its gradient (fwd+bwd) or its updated value (optimisation step: the step consumes the gradients).
+        The encoder output holds the VALID frames only (padded frames are unspecified, finite).  Arrays larger than their share of
+        `max_bytes` are replaced by a fixed, seeded sample of their elements."""
+        os.makedirs(out_dir, exist_ok=True)
+        per_param = 4096
+
+        def sample(t, k, seed):
+            flat = t.detach().reshape(-1)
+            if flat.numel() <= k:
+                return flat.float().cpu()
+            g = torch.Generator(device="cpu").manual_seed(seed)
+            idx = torch.randint(0, flat.numel(), (k,), generator=g).sort().values
+            return flat[idx.to(flat.device)].float().cpu()
+
+        arrays = {"loss": self.last_loss.detach().float().reshape(1).cpu()}
+        params = [(n, p) for n, p in self.model.named_parameters()]
+        vals = []
+        for i, (n, p) in enumerate(params):
+            src = p if self.pretrain else p.grad
+            vals.append(sample(src, per_param, 1000 + i) if src is not None else torch.zeros(0))
+        arrays["params_after_step_sample" if self.pretrain else "grads_sample"] = torch.cat(vals)
+        if self.last_x is not None:
+            room = max_bytes - sum(a.numel() * 4 for a in arrays.values())
+            x = self.last_x if self.last_fpm is None else self.last_x[~self.last_fpm]
+            arrays["features"] = sample(x, max(1, room // 4), 7)
+        for name, a in arrays.items():
+            np.save(os.path.join(out_dir, f"{name}.npy"), a.numpy().astype(np.float32))
 
     def timed(self, n_steps: int, e2e: bool) -> float:
         """Milliseconds for exactly n_steps: barrier + synchronize on both sides, CUDA events, max over ranks."""
@@ -541,6 +577,8 @@ def main():
     ap.add_argument("--ncu-step", action="store_true", help="profile exactly one step (cudaProfilerStart/Stop) and exit")
     ap.add_argument("--phases", action="store_true", help="add `phases_ms` (device time between the NVTX phase boundaries of a step, "
                     "rank 0, mean of 3 extra steps) to the line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="after the timed steps, write what the last timed step "
+                    "computed (loss, encoder output, gradients; seeded samples of large arrays) as DIR/<name>.npy, float32")
     ap.add_argument("--graph-probe", action="store_true", help="(internal) measure the whole step as one CUDA graph "
                     "(unispeech_b200/graphed.py) and print a small JSON object; the default run calls this in a child process")
     args = ap.parse_args()
@@ -562,7 +600,7 @@ def main():
     if world > 1:
         from unispeech_b200.parallel import configure_overlap
         _lib.check_device()
-        nccl_ctas = configure_overlap(int(os.environ.get("B200S_NCCL_CTAS", "0")))   # optional: NCCL_MAX_CTAS + SMs the persistent GEMMs leave free
+        nccl_ctas = configure_overlap(int(os.environ.get("B200S_NCCL_CTAS", "0")))   # optional: bound NCCL to that many CTAs (NCCL_MAX_CTAS)
         # the host side of a step (span-mask sampling, instance draws) is torch / numpy CPU work: torchrun pins every rank to ONE
         # OpenMP thread unless told otherwise
         if os.environ.get("OMP_NUM_THREADS", "1") == "1":
@@ -570,6 +608,10 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
     assert world == args.gpus, f"--gpus {args.gpus} but WORLD_SIZE={world}"
 
+    # host-side randomness of a step (span masks, negatives, utterance mixing) is seeded: the same arguments give the same inputs
+    random.seed(0)
+    np.random.seed(0)
+    torch.manual_seed(0)
     w = Workload(args.model, dev, rank, world, dropout=args.dropout, ragged=args.ragged, pretrain=args.pretrain, sat=args.sat)
     cfg, B, secs, T = w.cfg, w.B, w.secs, w.T
 
@@ -592,6 +634,9 @@ def main():
     ms = w.timed(args.steps, False)
     launches = lc0() - n0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        torch.cuda.synchronize()
+        w.dump_outputs(args.dump_outputs)
     for _ in range(2):
         w.step(True)
     ms_e2e = w.timed(args.steps, True)
@@ -622,7 +667,7 @@ def main():
     value = audio_s / (ms * 1e-3)
     e2e_value = audio_s / (ms_e2e * 1e-3)
 
-    # ---- roofline of the dominant kernel family (tcgen05 GEMM): per-op CUDA-event timing in one extra profiled step
+    # ---- roofline of the dominant kernel family (wgmma GEMM): per-op CUDA-event timing in one extra profiled step
     roofline, breakdown = None, None
     if rank == 0 and not args.no_profile:
         prof = ops.Profiler()
@@ -636,24 +681,18 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak = peaks.get("bf16_tflops_sustained", 989.0)   # H100 SXM data sheet, dense bf16
         is_gemm = lambda k: k.startswith("gemm") or k.startswith("posconv_gemm") or k.startswith("posconv_wgrad")
         gemm_ms = sum(v["ms"] for k, v in breakdown.items() if is_gemm(k))
         gemm_flops = sum(v["flops"] for k, v in breakdown.items() if is_gemm(k))
         achieved = gemm_flops / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else 0.0
         n_gemm = sum(v["calls"] for k, v in breakdown.items() if is_gemm(k))
-        traffic, traffic_src = None, None
-        try:  # DRAM bytes of the same launches from the committed ncu capture of one step (profiles/, same workload)
-            tj = json.load(open(os.path.join(ROOT, "profiles", f"gemm_traffic_{args.model}.json")))
-            traffic, traffic_src = tj["dram_bytes_per_launch"], tj["source"]
-        except Exception:
-            pass
-        roofline = {"bound": "tensor", "kernel": "gemm_bf16_pair_kernel / gemm_bf16_kernel (all tcgen05 GEMM launches of one step, "
+        roofline = {"bound": "tensor", "kernel": "gemm_bf16_kernel / posconv_window_kernel (all wgmma GEMM launches of one step, "
                                                  "per-launch averages)",
                     "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                    "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1400",
+                    "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "H100 SXM data sheet (989, dense bf16)",
                     "flop_per_launch": gemm_flops / max(n_gemm, 1), "launches_per_step": n_gemm,
-                    "us_per_launch": gemm_ms * 1e3 / max(n_gemm, 1), "traffic": traffic, "traffic_source": traffic_src,
+                    "us_per_launch": gemm_ms * 1e3 / max(n_gemm, 1),
                     "gemm_ms_per_step": gemm_ms, "gemm_share_of_step": gemm_ms / (ms / args.steps)}
         # the other kernel families of the same profiled step, each against its own bound (algorithmic work / CUDA-event time)
         fam = {}
@@ -663,7 +702,7 @@ def main():
                 tf = v["flops"] / (v["ms"] * 1e-3) / 1e12
                 fam[k] = {"bound": "tensor (+ SFU: one exp2 per score)", "achieved": tf, "unit": "TFLOP/s (algorithmic)",
                           "frac": tf / peak, "ms_per_step": v["ms"], "launches": v["calls"]}
-        hbm_peak = peaks.get("hbm_gbs", 6650.0)
+        hbm_peak = peaks.get("hbm_gbs", 3350.0)   # H100 SXM data sheet, HBM3
         for k in ("layer_norm_fwd", "layer_norm_gate_fwd", "layer_norm_bwd", "colsum"):
             v = breakdown.get(k)
             if v and v["ms"] > 0 and v["bytes"] > 0:
@@ -740,7 +779,7 @@ def main():
             "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": w.describe() + (f"; gradient exchange: bucketed NCCL all-reduce (AVG, fp32) overlapped with backward, "
-                                                   + (f"NCCL_MAX_CTAS={nccl_ctas}, the persistent GEMMs leave that many SMs free" if nccl_ctas else "NCCL defaults")
+                                                   + (f"NCCL_MAX_CTAS={nccl_ctas}" if nccl_ctas else "NCCL defaults")
                                                    if world > 1 else ""),
                        "global_batch": world * B,
                        "frames": T, "parallelism": f"dp{world}", "l2": "inputs larger than L2 (no flush needed)", 

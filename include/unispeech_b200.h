@@ -1,10 +1,10 @@
 /*
- * unispeech_b200 -- C ABI of the B200-native WavLM / UniSpeech-SAT encoder hot path.
+ * unispeech_b200 -- C ABI of the H100 (sm_90a) WavLM / UniSpeech-SAT encoder hot path.
  *
- * Every entry point enqueues hand-written sm_100a kernels on the given CUDA stream and returns without
+ * Every entry point enqueues hand-written sm_90a kernels on the given CUDA stream and returns without
  * synchronising.  All pointers are DEVICE pointers owned by the caller (PyTorch tensors); the library never
  * allocates or frees caller memory on the hot path.  Return value: 0 on success, negative on error (message via
- * b200s_last_error(), thread-local).  There is no CPU fallback: on a device that is not compute capability 10.x
+ * b200s_last_error(), thread-local).  There is no CPU fallback: on a device that is not compute capability 9.0
  * b200s_check_device() fails and so does every kernel launch.
  *
  * The reference (microsoft/UniSpeech) has no FFI for this path: it is plain PyTorch module code.  Each function
@@ -28,7 +28,7 @@ typedef void* b200s_stream; /* cudaStream_t */
 
 int b200s_version(void);
 const char* b200s_last_error(void);
-/* 0 if the current device can run the kernels (sm_100), negative otherwise */
+/* 0 if the current device can run the kernels (sm_90), negative otherwise */
 int b200s_check_device(void);
 /* number of kernels launched by this library so far (bench.py reports the per-step count) */
 long long b200s_launch_count(void);
@@ -52,9 +52,9 @@ typedef struct {
   int dgelu;
 } b200s_epilogue;
 
-/* ============================ tcgen05 GEMM family (csrc/gemm.cuh, gemm.cu) ============================ */
+/* ============================ wgmma GEMM family (csrc/gemm.cuh, gemm.cu) ============================== */
 
-/* out[b, r, 0:N] = epilogue( A[b, r, 0:K] . W[N,K]^T ),  bf16 in / bf16 out, fp32 accumulate in TMEM.
+/* out[b, r, 0:N] = epilogue( A[b, r, 0:K] . W[N,K]^T ),  bf16 in / bf16 out, fp32 accumulate.
  * A rows live at a + b*a_bs + r*a_rs and may OVERLAP (a_rs < K): this is how the strided Conv1d layers 1-6 of
  * ConvFeatureExtractionModel (WavLM/WavLM.py:400-403,485-504) and their input gradients become GEMMs on
  * channels-last [B,T,C] activations (row = k*C window, row stride = stride*C).  Also every nn.Linear forward /
@@ -65,7 +65,7 @@ int b200s_gemm_rows(const void* a, long long a_bs, long long a_rs, int rows, int
                     const b200s_epilogue* epi, b200s_stream stream);
 
 /* dW[n, k] (+=) sum_{b,r} Y[b,r,n] * X[b,r,k]   (fp32, row stride dw_ld): the weight gradient of the GEMMs above
- * (autograd of nn.Linear / nn.Conv1d).  Both operands are read MN-major by tcgen05.mma; X rows may overlap
+ * (autograd of nn.Linear / nn.Conv1d).  Both operands are read MN-major by wgmma; X rows may overlap
  * (conv im2col view).  Split-K over (batch, row) blocks.  N % 8 == 0, K % 8 == 0. */
 int b200s_gemm_wgrad(const void* y, long long y_bs, long long y_rs, const void* x, long long x_bs,
                      long long x_rs, int rows, int batches, int N, int K, float* dw, long long dw_ld,
@@ -99,24 +99,26 @@ int b200s_posconv_gemm(const void* xpad, long long xpad_bs, int T, int B, int D,
 int b200s_posconv_wgrad(const void* dy, long long dy_bs, long long dy_rs, const void* xpad, long long xpad_bs,
                         int T, int B, int D, int G, int taps, float* dwp, b200s_stream stream);
 
-/* ============================ attention (csrc/attn_fwd.cu, attn_bwd.cu) ============================ */
+/* ============================ attention (csrc/attn_fwd.cu, attn_bwd2.cu) =========================== */
 
 /* out[b,t,h*64+d] = sum_j softmax_j(scale q_i.k_j + gate[b,h,i]*tab[h,j-i+T-1], -inf at padded keys) v_j
  * Replaces compute_bias + gate multiply + F.multi_head_attention_forward (WavLM/modules.py:417-455,504-563); the
  * [B*H,T,T] bias is never materialised (it is Toeplitz).  qkv: bf16 [B,T,3D] fused projection output; gate: fp32
  * [B,H,T] or NULL (=1); tab: fp32 [H,2T-1] or NULL (no bias); key_pad: uint8 [B,T] or NULL; out: bf16 [B,T,D];
- * lse: fp32 [B,H,T] log2-domain log-sum-exp (saved for backward).  head_dim = 64, T <= 4096. */
+ * lse: fp32 [B,H,T] log2-domain log-sum-exp (saved for backward).  head_dim = 64; T <= 3840 with the bias table (shared-memory
+ * copies of its slice), T <= 4096 without. */
 int b200s_attn_fwd(const void* qkv, const float* gate, const float* tab, const uint8_t* key_pad, void* out,
                    float* lse, int B, int T, int H, float scale, b200s_stream stream);
 
 /* Backward of b200s_attn_fwd (autograd of the same lines).  delta: fp32 [B,H,T] workspace; dqkv: bf16 [B,T,3D];
- * dgate: fp32 [B,H,T] (written); dtab: fp32 [H,2T-1] (+=, shared by all layers: WavLM/WavLM.py:549,594-599). */
+ * dgate: fp32 [B,H,T] (written); dtab: fp32 [H,2T-1] (+=, shared by all layers: WavLM/WavLM.py:549,594-599).  T <= 4096; runs the
+ * fused kernel below with an fp32 dQ buffer allocated on the stream for the call. */
 int b200s_attn_bwd(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                    const uint8_t* key_pad, const float* lse, float* delta, void* dqkv, float* dgate, float* dtab,
                    int B, int T, int H, float scale, b200s_stream stream);
 
 /* Same contract as b200s_attn_bwd, computed by ONE fused tensor-core kernel (csrc/attn_bwd2.cu: probabilities recomputed
- * once, dK/dV accumulated in TMEM, dQ reduced across key tiles in fp32).  dq_acc: fp32 [B,T,D] workspace that must be ZERO
+ * once, dK/dV accumulated in registers, dQ reduced across key tiles in fp32).  dq_acc: fp32 [B,T,D] workspace that must be ZERO
  * on entry and is zero again on return.  T <= 2048. */
 int b200s_attn_bwd_fused(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                          const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv,
@@ -136,10 +138,8 @@ int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* d
                                  float drop_p, const uint32_t* drop_mask, b200s_stream stream);
 long long b200s_attn_dropout_mask_words(int B, int T, int H);
 
-/* SMs the persistent CTA-pair GEMM kernels leave free (0 = none, the default).  Data-parallel runs overlap the NCCL gradient exchange
- * with the backward pass; its CTAs (bounded by NCCL_MAX_CTAS) then find free SMs instead of displacing clusters of a grid that was
- * sized for the whole chip (legacy_distributed_data_parallel.py:76-165 runs the exchange strictly after backward, so the reference
- * has no counterpart). */
+/* Deprecated, kept for callers of the earlier ABI: validates 0 <= sms < SM count and has no effect.  It reserved SMs of the persistent
+ * GEMM grid for a concurrent collective; the GEMMs now launch one CTA per tile, so NCCL's CTAs take SMs as tiles retire. */
 int b200s_reserve_sms(int sms);
 
 /* ============================ row kernels (csrc/rowops.cu) ============================ */
@@ -312,7 +312,7 @@ int b200s_adam_step(const void* table, int n_tensors, long long total_chunks, fl
 /* ============================ masked-prediction loss head (csrc/nce.cu) ============================ */
 /* final_proj + cosine-similarity NCE logits + sum-reduced cross entropy of the pre-training models
  * (src/fairseq/models/wavlm/wavlm.py:426-438,525-576; src/fairseq/criterions/wavlm_criterion.py:63-87), built around the
- * tcgen05 GEMMs above: z[s,c] = cos(proj_s, E_c)/temp = (proj En^T)[s,c] / (|proj_s| temp), loss = w * sum_s CE(z[s,:], target_s)
+ * wgmma GEMMs above: z[s,c] = cos(proj_s, E_c)/temp = (proj En^T)[s,c] / (|proj_s| temp), loss = w * sum_s CE(z[s,:], target_s)
  * (the reference's {positive} U {negatives != positive} softmax IS the softmax over the C classes). */
 
 /* out[s,:] = x[idx[s],:]  (x[masked_indices], wavlm.py:541,558) and its autograd dx[idx[s],:] += src[s,:] (distinct rows) */

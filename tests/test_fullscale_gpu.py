@@ -10,11 +10,8 @@ with depth (|h| up to ~25 at layer 24 with these weights) the bound is stated RE
     max-abs diff  <=  MAX_REL  * max|h_layer|        (MAX_REL  = 0.03)
     mean-abs diff <=  MEAN_REL * mean|h_layer|       (MEAN_REL = 0.015; bf16 has 2^-8 = 0.4 % relative spacing per rounding)
 and for the post-LN WavLM-Base (|h| <= ~6 everywhere) additionally the absolute max-abs < 0.12 of the small-model tests.
-Measured (profiles/r02_parity_fullscale_*.json): the relative error does NOT grow with depth -- 0.8-1.0 % of mean|h| right
-after the conv stack / pos_conv (layer 0) and 0.8-1.15 % at layer 24; max-abs 0.044-0.076 on WavLM-Base (below the reference's own
-bf16 drift), <= 2.6 % of max|h| on WavLM-Large.
 Every layer's numbers are printed as a table (pytest -s) and written to gpurun_out/parity_fullscale.json when that directory
-is writable; the committed copy lives in profiles/.
+is writable.
 """
 import json
 import os

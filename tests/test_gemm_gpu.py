@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05 GEMM family against a plain PyTorch fp32 reference of the same op."""
+"""GPU parity tests of the wgmma GEMM family against a plain PyTorch fp32 reference of the same op."""
 import ctypes as C
 
 import pytest

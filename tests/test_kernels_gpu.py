@@ -302,7 +302,8 @@ def _attn_ref(qkv, gate, tab, pad, B, T, H, scale):
 
 
 @pytest.mark.parametrize("B,T,H,bias,padded", [(2, 100, 2, True, True), (1, 128, 2, True, False), (2, 333, 3, True, True),
-                                               (1, 749, 12, True, False), (2, 257, 2, False, True), (1, 1499, 2, True, True)])
+                                               (1, 749, 12, True, False), (2, 257, 2, False, True), (1, 1499, 2, True, True),
+                                               (2, 3072, 1, True, True)])
 def test_attn_fwd(cuda_device, B, T, H, bias, padded):
     from unispeech_b200 import ops
     dev = cuda_device
@@ -322,7 +323,7 @@ def test_attn_fwd(cuda_device, B, T, H, bias, padded):
     ref = _attn_ref(qkv, gate, tab, pad, B, T, H, 0.125)
     assert torch.isfinite(out.float()).all()
     d = (out.float() - ref).abs()
-    if padded:  # rows of padded QUERY frames are unspecified-but-finite (zeros where a whole 256-row block is padded): the
+    if padded:  # rows of padded QUERY frames are unspecified-but-finite (zeros where a whole 128-row block is padded): the
         d = d[pad == 0]  # reference's values there never reach a valid frame (padded keys are masked)
     err = d.max().item()
     assert err < 0.03, err
@@ -400,6 +401,12 @@ def test_attn_bwd(cuda_device, B, T, H, bias, padded, fused):
         assert e1 < 0.03 * max(1.0, gr.grad.abs().max().item()), e1
         e2 = (dtab - tr.grad).abs().max().item()
         assert e2 < 0.03 * max(1.0, tr.grad.abs().max().item()), (e2, tr.grad.abs().max().item())
+
+
+def test_attn_bwd_long_sequence(cuda_device):
+    """The longest utterance the bias path takes (T = 3072 frames, about 61 s), ragged: b200s_attn_bwd (the entry point used beyond
+    the fused API's T <= 2048) against autograd of the reference."""
+    test_attn_bwd(cuda_device, 2, 3072, 1, True, True, False)
 
 
 def test_prep_linear_batched_shapes(cuda_device):

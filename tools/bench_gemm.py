@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM family on the shapes of the WavLM-Base 16 x 15 s step (run on the GPU box).
+"""Micro-benchmark of the wgmma GEMM family on the shapes of the WavLM-Base 16 x 15 s step (needs an H100).
 
     python tools/bench_gemm.py [--reps 20] [--only NAME]
 Prints one line per shape: time, TFLOP/s, fraction of the measured bf16 peak.

@@ -1,3 +1,3 @@
-"""unispeech_b200 -- B200-native WavLM / UniSpeech-SAT encoder hot path (hand-written sm_100a kernels behind a C ABI)."""
+"""unispeech_b200 -- WavLM / UniSpeech-SAT encoder hot path for the H100 (hand-written sm_90a kernels behind a C ABI)."""
 
 __version__ = "0.1.0"

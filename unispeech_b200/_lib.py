@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI library (include/unispeech_b200.h).
 
 The product path has no CPU / PyTorch fallback: if the shared library is missing, or the device is not
-sm_100, calls raise.  Functions take torch CUDA tensors and pass raw device pointers + the current stream.
+sm_90, calls raise.  Functions take torch CUDA tensors and pass raw device pointers + the current stream.
 """
 from __future__ import annotations
 
@@ -58,9 +58,7 @@ _RESTYPES = {"int": C.c_int, "long long": C.c_longlong, "uint32_t": C.c_uint32, 
 def _bind_prototypes(lib):
     """Declare `argtypes` / `restype` of every entry point ONCE, from the prototypes of include/unispeech_b200.h.  The wrappers
     then pass plain Python ints / floats (raw device pointers, strides, sizes) instead of one ctypes object per argument
-    (15-20 arguments per call, ~6400 calls per WavLM-Large step).  Measured on the B200 box: the step's host time did not move
-    (24.4 -> 24.4 ms) -- the launch path itself (cudaLaunchKernelEx, tensor-map encodes, torch's allocator and autograd glue)
-    dominates, not the marshalling; the whole-step CUDA graph (graphed.py) is what takes the host off the path."""
+    (15-20 arguments per call, ~6400 calls per WavLM-Large step)."""
     import re
     hdr = Path(__file__).resolve().parent.parent / "include" / "unispeech_b200.h"
     src = hdr.read_text()

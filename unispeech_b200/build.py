@@ -1,7 +1,7 @@
-"""In-tree build of the C-ABI library (nvcc, sm_100a only).
+"""In-tree build of the C-ABI library (nvcc, sm_90a only).
 
 `python -m unispeech_b200.build` compiles every `csrc/*.cu` into `unispeech_b200/lib/libunispeech_b200.so`.
-nvcc cross-compiles without a GPU; the resulting .so travels to the GPU box with the repo snapshot.
+nvcc cross-compiles without a GPU.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ BUILD = PKG.parent / "build"
 LIB = LIBDIR / "libunispeech_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

@@ -1,29 +1,28 @@
 // Fused attention backward with the gated relative-position bias (autograd of WavLM/modules.py:521-563): ONE tensor-core
-// kernel produces dQ, dK, dV, d gate and d tab, so the probabilities are recomputed once.
+// kernel produces dQ, dK, dV, d gate and d tab, so the probabilities are recomputed once.  wgmma + TMA (sm_90a).
 //
-// CTA = 128 keys of one (batch, head); it walks over the 128-row query tiles.  Orientation: THREAD = QUERY ROW (TMEM lane),
-// as in the forward kernel, so everything that is per query -- lse, Delta, the gate -- is a register, d gate is a thread-local
-// sum, and the Toeplitz bias entries a thread needs are consecutive table words (64-bit loads from two shifted copies).
-// Per query tile i (two 64-key halves so that S / dP of the next tile are produced under the exponentials of this one):
-//   S_hf  = Q_i K_hf^T        128x64x64   -> TMEM stage hf, columns [0,64)
-//   dP_hf = dO_i V_hf^T       128x64x64   -> TMEM stage hf, columns [64,128)
-//   P  = exp2(S*scale*log2e + gate_i*log2e*tab[j-i] + keymask_j - lse_i);   dS = P o (dP - Delta_i) * scale
-//   P, dS -> shared memory once, bf16 [128 queries][128 keys] operand tiles (two 64-key blocks)
-//   dV += P^T dO_i           A = P tile read MN-major (M = keys), accumulates in TMEM over the whole loop
-//   dK += dS^T Q_i           same with the dS tile
-//   dQ_i = dS K              A = dS tile read K-major; read back from TMEM and added to an fp32 [B,T,D] buffer with vector
-//                            reductions (one writer CTA per key tile)
-//   d gate_i += sum_j dS_ij tab[j-i]        thread-local FMA, one global atomic per thread and tile
-//   d tab[d]  = sum_i gate_i dS_{i,i+d}     diagonal sums of a staged bf16 tile gate*dS (one per half), per-CTA accumulators
-// Warp roles: warps 0-15 = CUDA-core warps: warpgroup g = (key half g>>1, 32-column group g&1), thread = query row;
-// warp 16 = producer (its lane 0 issues every TMA load and MMA).  All hand-offs are mbarriers (+ one 256-thread named barrier per half that
-// recycles the diagonal staging tile).
+// CTA = 128 keys of one (batch, head); it walks over the 128-row query tiles.  Two consumer warpgroups (WG w = 0, 1) and one TMA
+// warp.  Per query tile i, WG w owns query rows 64 w .. 64 w + 63 for the scores and key rows 64 w .. 64 w + 63 for the dK / dV
+// accumulators (registers, across the whole loop).  Everything element-wise is done on the wgmma accumulator fragments:
+//   for each 64-key half hf:
+//     S  = Q_i K_hf^T,  dP = dO_i V_hf^T                     wgmma m64n64k16 (64 query rows of this WG)
+//     P  = exp2(S*scale*log2e + gate_i*log2e*tab[j-i] + keymask_j - lse_i);   dS = P o (dP - Delta_i) * scale
+//     P, dS -> shared memory, bf16 [128 queries][128 keys] operand tiles (two 64-key blocks); gate*dS/scale -> a bf16 staging
+//     tile for the d tab diagonal sums (one tile: the first half's sums are taken before the second half is staged);
+//     d gate_i += sum_j dS_ij tab[j-i] (quad shuffles, one atomic per row)
+//   (all 256 threads) barrier, then
+//   dV += P^T dO_i, dK += dS^T Q_i     A = P / dS tile read MN-major (M = this WG's 64 keys), B = dO / Q MN-major
+//   dQ_i = dS K                        A = dS read K-major (this WG's 64 queries), added to an fp32 [B,T,D] buffer with vector
+//                                      reductions (one writer CTA per key tile and query element)
+//   d tab[d] = sum_i gate_i dS_{i,i+d}  diagonal sums of the staged tiles, per-CTA accumulators, flushed with atomics at the end
+// Dropout: the keep bit of (query i, key j) is bit i & 31 of word drop_mask[block(i), j], written by the forward kernel.
 // Padding: a CTA whose 128 keys are all padded writes zero dK / dV rows and exits; query tiles that are fully padded at the end
 // of the utterance are not visited (their probabilities are zero: the forward leaves lse = +inf there).
 #include "../../include/unispeech_b200.h"
 #include "attn_common.cuh"
 #include "common.h"
-#include <type_traits>
+
+#include <algorithm>
 
 namespace b200 {
 
@@ -34,20 +33,8 @@ __device__ __forceinline__ float ex2f(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void mbar_arrive_cta(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.release.cta.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ uint32_t bit_transpose32(uint32_t x, int lane) {  // see warp_bit_transpose in attn_fwd.cu
-#pragma unroll
-  for (int s = 16; s >= 1; s >>= 1) {
-    const uint32_t m = (s == 16) ? 0x0000FFFFu : (s == 8) ? 0x00FF00FFu : (s == 4) ? 0x0F0F0F0Fu : (s == 2) ? 0x33333333u : 0x55555555u;
-    const uint32_t y = __shfl_xor_sync(0xffffffffu, x, s);
-    x = (lane & s) ? ((x & ~m) | ((y >> s) & m)) : ((x & m) | ((y << s) & ~m));
-  }
-  return x;
+__device__ __forceinline__ void red_add_v2(float* dst, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(a), "f"(b) : "memory");
 }
 
 // shared-memory map (bytes from the 1024-aligned base)
@@ -57,21 +44,20 @@ constexpr int kFQ = 32768;         // Q tiles, 2 stages x 16 KB
 constexpr int kFDO = 65536;        // dO tiles, 2 stages x 16 KB
 constexpr int kFP = 98304;         // P  : [128 queries][128 keys] as two 64-key blocks, 32 KB
 constexpr int kFDS = 131072;       // dS : same layout, 32 KB
-constexpr int kFW = 163840;        // gate*dS staging for the diagonal sums: one [128 queries][66] bf16 tile per key half
+constexpr int kFW = 163840;        // gate*dS staging for the diagonal sums: one [128 queries][66] bf16 tile
 constexpr int kWStride2 = 66;      // bf16 per staged row (33 words: conflict-free row writes and diagonal reads)
 constexpr int kFWBytes = 128 * kWStride2 * 2;   // 16896
-constexpr int kFTab = kFW + 2 * kFWBytes;        // 197632: tab copies [2][tab_stride], dtab_acc[(N+1)*128]
-constexpr int kCudaThreads = 512;             // 16 CUDA-core warps: four per scheduler hide the TMEM / SFU / LDS latencies
-constexpr int kFThreads = kCudaThreads + 32;  // + 1 producer warp (only its first lane works): 17 warps x 120 registers
-constexpr int kProdWarp = kCudaThreads / 32;
-
-// floats of ONE copy of the bias-table slice: (N + 1) * 128 entries + 16, so that the second copy (shifted by one element)
-// starts 16 banks further.  Lane 0 of every warp starts on an ODD table index (j0 - r + N*128 - 1 with j0, r multiples of 32), so
-// within a half warp the 8 odd lanes read 16 consecutive words of copy 1 and the 8 even lanes the SAME 16 word offsets of copy 0:
-// with the copies 16 banks apart the 64-bit loads touch 32 distinct banks (measured: 2 wavefronts per load instead of 4)
-__host__ __device__ constexpr int bwd_tab_stride(int N) { return (N + 1) * kAttnTile + 16; }
+constexpr int kFTab = kFW + kFWBytes;            // 180736: tab slice [(N+1)*128], dtab_acc[(N+1)*128]
+constexpr int kConsumers = 256;                  // two warpgroups
+constexpr int kFThreads = kConsumers + 32;       // + the TMA warp
+constexpr int kProdWarp = kConsumers / 32;
 
 }  // namespace
+
+// shared memory of the fused backward for N key tiles (with or without the relative-position bias)
+static inline int attn_bwd_smem_bytes(int N, bool bias) {
+  return kFTab + static_cast<int>(sizeof(float)) * ((bias ? (N + 1) * kAttnTile : 0) + (N + 1) * kAttnTile) + 1024;
+}
 
 template <bool HAS_BIAS, bool DROP>
 __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tm_qkv,
@@ -91,12 +77,10 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
   uint8_t* sDO = smem + kFDO;
   uint8_t* sP = smem + kFP;
   uint8_t* sDS = smem + kFDS;
-  float* tab_s = reinterpret_cast<float*>(smem + kFTab);  // [2][tab_stride]: copy c holds slice[l + c]
-  const int tab_stride = bwd_tab_stride(N);
-  float* dtab_acc = tab_s + (HAS_BIAS ? 2 * tab_stride : 0);  // [(N+1)*128]
+  float* tab_s = reinterpret_cast<float*>(smem + kFTab);  // slice[l] = tab[h, l + tab_base]
+  float* dtab_acc = tab_s + (HAS_BIAS ? (N + 1) * kAttnTile : 0);  // [(N+1)*128]
 
-  __shared__ uint64_t kv_full, qdo_full[2], qdo_free[2], st_full[2], ready[2], mma_done, dq_full, acc_done;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t kv_full, qdo_full[2], qdo_free[2];
   __shared__ uint32_t key_mask_s[4];  // bit j of word j>>5: key k0 + j is padded / beyond T
 
   // ---- padding: which of this CTA's keys are masked, and how many query tiles hold a valid query.  ONE pass over the
@@ -145,13 +129,8 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     mbar_init(&kv_full, 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&qdo_full[i], 1);
-      mbar_init(&qdo_free[i], 1);
-      mbar_init(&st_full[i], 1);
-      mbar_init(&ready[i], kCudaThreads / 2);
+      mbar_init(&qdo_free[i], kConsumers / 32);  // one arrival per consumer warp once its MMAs reading the stage have retired
     }
-    mbar_init(&mma_done, 1);
-    mbar_init(&dq_full, 1);
-    mbar_init(&acc_done, 1);
     fence_mbar_init();
     mbar_expect_tx(&kv_full, 32768);
     tma_load_4d(sK, &tm_qkv, &kv_full, D + h * kHeadDim, k0, b, 0);
@@ -162,153 +141,49 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       tma_load_4d(sDO + qi * 16384, &tm_do, &qdo_full[qi], h * kHeadDim, qi * kAttnTile, b, 0);
     }
   }
-  __syncwarp();
-  if (warp == 0) tmem_alloc(&tmem_base_s, 512);
 
   // per-CTA tables: slice[l] = tab[h, l + base], base = k0 - (N*128-1) + (T-1); element (query i, key k0 + j) -> l = j - i + N*128-1
   const int tab_base = k0 - (N * kAttnTile - 1) + (T - 1);
   if (HAS_BIAS) {
     const int len = (N + 1) * kAttnTile;
     const float* tab_h = p.tab + static_cast<long long>(h) * (2 * T - 1);
-    for (int l = tid; l < 2 * len; l += kFThreads) {
-      const int c = l / len, k = l - c * len;
-      const int gi = k + c + tab_base;
-      tab_s[c * tab_stride + k] = (gi >= 0 && gi < 2 * T - 1) ? tab_h[gi] : 0.f;
+    for (int l = tid; l < len; l += kFThreads) {
+      const int gi = l + tab_base;
+      tab_s[l] = (gi >= 0 && gi < 2 * T - 1) ? tab_h[gi] : 0.f;
+      dtab_acc[l] = 0.f;
     }
-    for (int l = tid; l < len; l += kFThreads) dtab_acc[l] = 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
-  // TMEM columns: stage hf at hf*128: S [0,64), dP [64,128); dV 256; dK 320; dQ 384
-  constexpr uint32_t kColDV = 256, kColDK = 320, kColDQ = 384;
 
-  if (warp >= kProdWarp) {
-    if (warp == kProdWarp && lane == 0) {
-      // ================================================================== TMA producer + MMA issuer
-      constexpr uint32_t idesc_st = make_idesc_bf16(128, 64, 0, 0);   // K-major A (Q / dO), K-major B (K / V half)
-      constexpr uint32_t idesc_acc = make_idesc_bf16(128, 64, 1, 1);  // MN-major A (P / dS read transposed), MN-major B (dO / Q)
-      constexpr uint32_t idesc_dq = make_idesc_bf16(128, 64, 0, 1);   // K-major A (dS), MN-major B (K)
-      auto load_qdo = [&](int qi) {
+  if (warp == kProdWarp) {
+    // ================================================================== TMA producer: Q / dO stage refills
+    if (lane == 0) {
+      for (int qi = 2; qi < NQ; ++qi) {
         const int s = qi & 1;
+        mbar_wait(&qdo_free[s], ((qi - 2) >> 1) & 1);  // the MMAs of tile qi-2 have retired
         mbar_expect_tx(&qdo_full[s], 32768);
         tma_load_4d(sQ + s * 16384, &tm_qkv, &qdo_full[s], h * kHeadDim, qi * kAttnTile, b, 0);
         tma_load_4d(sDO + s * 16384, &tm_do, &qdo_full[s], h * kHeadDim, qi * kAttnTile, b, 0);
-      };
-      auto issue_st = [&](int qi, int hf) {  // S and dP of (query tile qi, key half hf) into TMEM stage hf
-        const uint32_t aq = smem_u32(sQ + (qi & 1) * 16384), ad = smem_u32(sDO + (qi & 1) * 16384);
-        const uint32_t bk = smem_u32(sK + hf * 8192), bv = smem_u32(sV + hf * 8192);
-        const uint32_t d0 = tmem + hf * 128;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(d0, make_smem_desc_sw128(aq + k * 32, 16, 1024), make_smem_desc_sw128(bk + k * 32, 16, 1024), idesc_st,
-                    k > 0 ? 1u : 0u);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(d0 + 64, make_smem_desc_sw128(ad + k * 32, 16, 1024), make_smem_desc_sw128(bv + k * 32, 16, 1024),
-                    idesc_st, k > 0 ? 1u : 0u);
-        umma_commit(&st_full[hf]);
-      };
-
-      mbar_wait(&kv_full, 0);  // (K, V and the first two Q / dO tiles were issued in the prologue)
-      mbar_wait(&qdo_full[0], 0);
-      tc_fence_after();
-      issue_st(0, 0);
-      issue_st(0, 1);
-
-      for (int qi = 0; qi < NQ; ++qi) {
-        const int st = qi & 1;
-#pragma unroll 1
-        for (int hf = 0; hf < 2; ++hf) {
-          mbar_wait(&ready[hf], qi & 1);  // P / dS / W of this half are staged; TMEM stage hf has been read
-          tc_fence_after();
-          if (qi + 1 < NQ) {
-            if (hf == 0) {
-              mbar_wait(&qdo_full[(qi + 1) & 1], ((qi + 1) >> 1) & 1);
-              tc_fence_after();
-            }
-            issue_st(qi + 1, hf);  // next tile's scores first: the CUDA-core warps never wait for the accumulation MMAs
-          }
-        }
-        const uint32_t ap = smem_u32(sP), ads = smem_u32(sDS);
-        const uint32_t bdo = smem_u32(sDO + st * 16384), bq = smem_u32(sQ + st * 16384), bk = smem_u32(sK);
-#pragma unroll
-        for (int k = 0; k < 8; ++k)  // dV += P^T dO   (K = 128 queries, 16 per step)
-          umma_bf16(tmem + kColDV, make_smem_desc_sw128(ap + k * 2048, 16384, 1024),
-                    make_smem_desc_sw128(bdo + k * 2048, 8192, 1024), idesc_acc, (qi > 0 || k > 0) ? 1u : 0u);
-#pragma unroll
-        for (int k = 0; k < 8; ++k)  // dK += dS^T Q
-          umma_bf16(tmem + kColDK, make_smem_desc_sw128(ads + k * 2048, 16384, 1024),
-                    make_smem_desc_sw128(bq + k * 2048, 8192, 1024), idesc_acc, (qi > 0 || k > 0) ? 1u : 0u);
-#pragma unroll
-        for (int k = 0; k < 8; ++k)  // dQ_i = dS K    (K = 128 keys: two 64-key blocks, 16 per step)
-          umma_bf16(tmem + kColDQ, make_smem_desc_sw128(ads + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
-                    make_smem_desc_sw128(bk + k * 2048, 8192, 1024), idesc_dq, k > 0 ? 1u : 0u);
-        umma_commit(&dq_full);
-        umma_commit(&mma_done);
-        umma_commit(&qdo_free[st]);
-        if (qi + 1 == NQ) umma_commit(&acc_done);
-        if (qi + 2 < NQ) {  // refill this Q/dO stage once its readers have retired
-          mbar_wait(&qdo_free[st], (qi >> 1) & 1);
-          load_qdo(qi + 2);
-        }
       }
     }
   } else {
-    // ==================================================================== CUDA-core warps
-    const int g = warp >> 2;              // warpgroup 0..3
-    const int hf = g >> 1;                // key half of this warpgroup
-    const int j0 = hf * 64 + (g & 1) * 32;  // first of this thread's 32 key columns (inside the 128-key tile)
-    const int r = (warp & 3) * 32 + lane;  // query row inside the tile == TMEM lane
-    const int ht = tid & 255;             // thread index inside the half (diagonal-sum tasks)
+    // ==================================================================== consumer warpgroups
+    const int w = warp >> 2;                 // warpgroup: query rows 64 w.. of each tile, key rows 64 w.. of dK / dV
+    const int wq = warp & 3;
+    const int fr = 64 * w + 16 * wq + (lane >> 2);   // first of this thread's two fragment rows (the other is fr + 8)
+    const int fc = 2 * (lane & 3);                    // column of fragment element 0 inside each 8-column group
     const float sc = p.scale * kLog2e;
-    const uint32_t lane_addr = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const uint32_t kmask = key_mask_s[j0 >> 5];  // bit jj: key column j0 + jj is masked
+    const float inv_scale = 1.0f / p.scale;
     const bool any_masked = (key_mask_s[0] | key_mask_s[1] | key_mask_s[2] | key_mask_s[3]) != 0u;  // uniform over the CTA
-    // bias entries of (row r, keys j0 + jj) in query tile qi: slice[tstart - qi*128 + jj]
-    const int tstart = j0 - r + N * kAttnTile - 1;
-    const float* tab_row = tab_s + (tstart & 1) * tab_stride + (tstart & ~1);  // 8-byte aligned in the copy of matching parity
-    uint32_t* wtile = reinterpret_cast<uint32_t*>(smem + kFW + hf * kFWBytes);
     const long long bh = static_cast<long long>(b) * p.H + h;
 
-    // per-row scalars of query tile qi: the RAW values are loaded one tile ahead (no arithmetic on them until the next tile starts,
-    // so the loads stay in flight under a whole tile of work); lse = +inf marks out-of-range queries (p = exp2(-inf) = 0)
-    float r_lse = INFINITY, r_delta = 0.f, r_gate = 0.f;
-    auto load_row = [&](int qi, float& a_lse, float& a_delta, float& a_gate) {
-      const int i = qi * kAttnTile + r;
-      a_lse = INFINITY; a_delta = 0.f; a_gate = 0.f;
-      if (i < T) {
-        a_lse = p.lse[bh * T + i];
-        a_delta = p.delta[bh * T + i];
-        if (HAS_BIAS) a_gate = (p.gate != nullptr) ? p.gate[bh * T + i] : 1.0f;
-      }
-    };
-    load_row(0, r_lse, r_delta, r_gate);
-    const float inv_scale = 1.0f / p.scale;
+    float dv_acc[32], dk_acc[32];  // written by the first tile's MMAs (scale_d = 0)
 
-    // dQ tile of query tile qi: TMEM -> fp32 reductions into dq_acc[b, q, h*64 + g*16 ..]  (thread = query row, 16 columns)
-    auto flush_dq = [&](int qi) {
-      mbar_wait(&dq_full, qi & 1);
-      tc_fence_after();
-      uint32_t t0[16];
-      tmem_ld_32x32b_x16(tmem + lane_addr + kColDQ + g * 16, t0);
-      tmem_ld_wait();
-      const int q = qi * kAttnTile + r;
-      if (q < T) {
-        float* dst = dq_acc + (static_cast<long long>(b) * T + q) * D + h * kHeadDim + g * 16;
-#pragma unroll
-        for (int v = 0; v < 4; ++v)
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + v * 4), "f"(__uint_as_float(t0[v * 4 + 0])),
-                       "f"(__uint_as_float(t0[v * 4 + 1])), "f"(__uint_as_float(t0[v * 4 + 2])),
-                       "f"(__uint_as_float(t0[v * 4 + 3]))
-                       : "memory");  // the staged dS already carries the softmax scale
-      }
-    };
-    // diagonal sums of the staged gate*dS tile of (query tile qi, this half).  Task (e, s): elements (i = (jj - e) & 127, jj)
+    // diagonal sums of the staged gate*dS tile of (query tile qi, key half hf).  Task (e, s): elements (i = (jj - e) & 127, jj)
     // for jj = 16 s .. 16 s + 15: diagonal jj - i = e (not wrapped, jj >= e) or e - 128 (wrapped).  The wrap point is a per-task
     // constant, so every load is base + immediate.
-    auto diag_task = [&](int qi, int e, int s) {
+    auto diag_task = [&](int qi, int hf, int e, int s) {
+      const uint32_t* wtile = reinterpret_cast<const uint32_t*>(smem + kFW);
       const int w0 = e - 16 * s;  // columns jj = 16 s + c with c < w0 are on the wrapped diagonal
       const uint32_t base_nw = smem_u32(wtile) + static_cast<uint32_t>((16 * s - e) * kWStride2 + 16 * s) * 2u;
       const uint32_t base_w = base_nw + static_cast<uint32_t>(kAttnTile * kWStride2 * 2);
@@ -328,130 +203,164 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     };
 
     for (int qi = 0; qi < NQ; ++qi) {
-      mbar_wait(&st_full[hf], qi & 1);
-      tc_fence_after();
-      const float lse2 = r_lse, dsc = r_delta * p.scale, gl = r_gate * kLog2e, gos = r_gate * inv_scale;
-      // next tile's row scalars: in flight under this tile's arithmetic
-      float n_lse = INFINITY, n_delta = 0.f, n_gate = 0.f;
-      if (qi + 1 < NQ) load_row(qi + 1, n_lse, n_delta, n_gate);
-      uint32_t keep_bits = 0xffffffffu;
-      if (DROP) {  // word (32-query block, key column) holds the bits of this warp's 32 rows: transpose to one word per row
-        const long long blk = bh * (4 * N) + ((qi * kAttnTile + r) >> 5);
-        const uint32_t wcol = p.drop_mask[blk * (N * kAttnTile) + k0 + j0 + lane];
-        keep_bits = bit_transpose32(wcol, lane);
+      const int st = qi & 1;
+      // per-row scalars of this thread's two fragment rows; lse = +inf marks out-of-range queries (p = exp2(-inf) = 0)
+      float r_lse[2], r_dsc[2], r_gl[2], r_gos[2];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int i = qi * kAttnTile + fr + 8 * rr;
+        float lse = INFINITY, delta = 0.f, gate = 0.f;
+        if (i < T) {
+          lse = p.lse[bh * T + i];
+          delta = p.delta[bh * T + i];
+          if (HAS_BIAS) gate = (p.gate != nullptr) ? p.gate[bh * T + i] : 1.0f;
+        }
+        r_lse[rr] = lse;
+        r_dsc[rr] = delta * p.scale;
+        r_gl[rr] = gate * kLog2e;
+        r_gos[rr] = gate * inv_scale;
       }
-      float dg = 0.f;
-      const float* trow = tab_row - qi * kAttnTile;
-      uint32_t* wrow = wtile + r * (kWStride2 / 2) + (g & 1) * 16;
+      float dg[2] = {0.f, 0.f};
+      mbar_wait(&kv_full, 0);
+      mbar_wait(&qdo_full[st], (qi >> 1) & 1);
+      const uint32_t aq = smem_u32(sQ + st * 16384) + w * 8192, ad = smem_u32(sDO + st * 16384) + w * 8192;
 
-      // 16 key columns at a time: probabilities / dS / gate*dS packed to bf16 in registers, then staged.  The first stores of a
-      // tile wait for the accumulation MMAs of the previous tile (which read the P / dS tiles); by then half of this tile's
-      // arithmetic is done.
-      auto body = [&](auto MSK) {
-        constexpr bool kMsk = decltype(MSK)::value;
+#pragma unroll 1
+      for (int hf = 0; hf < 2; ++hf) {
+        float s_acc[32], d_acc[32];
+        const uint32_t bk = smem_u32(sK) + hf * 8192, bv = smem_u32(sV) + hf * 8192;
+        wgmma_fence();
 #pragma unroll
-        for (int sub = 0; sub < 2; ++sub) {
-          uint32_t su[16], du[16];
-          tmem_ld_32x32b_x16(tmem + lane_addr + hf * 128 + (g & 1) * 32 + sub * 16, su);
-          tmem_ld_32x32b_x16(tmem + lane_addr + hf * 128 + 64 + (g & 1) * 32 + sub * 16, du);
-          tmem_ld_wait();
-          uint32_t pw[8], dw[8], ww[8];
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n64k16<0, 0>(s_acc, make_smem_desc_sw128(aq + k * 32, 16, 1024), make_smem_desc_sw128(bk + k * 32, 16, 1024),
+                                k > 0 ? 1u : 0u);
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            float2 tb = make_float2(0.f, 0.f);
-            if (HAS_BIAS) tb = *reinterpret_cast<const float2*>(trow + sub * 16 + 2 * q);
-            const float tbv[2] = {tb.x, tb.y};
-            float pr2[2], ds2[2], w2[2] = {0.f, 0.f};
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n64k16<0, 0>(d_acc, make_smem_desc_sw128(ad + k * 32, 16, 1024), make_smem_desc_sw128(bv + k * 32, 16, 1024),
+                                k > 0 ? 1u : 0u);
+        wgmma_commit();
+        // dropout keep words of this thread's key columns (bit = query row & 31; both fragment rows are in one 32-row block)
+        const uint32_t* mrow = nullptr;
+        if (DROP) mrow = p.drop_mask + (bh * (4 * N) + ((qi * kAttnTile + fr) >> 5)) * (N * kAttnTile) + k0 + hf * 64 + fc;
+        wgmma_wait<0>();
+        uint32_t* wtile = reinterpret_cast<uint32_t*>(smem + kFW);
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {        // 8-column group
+          uint2 kw = make_uint2(0u, 0u);     // keep words of columns fc, fc + 1 of the group
+          if (DROP) kw = *reinterpret_cast<const uint2*>(mrow + 8 * g);
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {   // fragment row
+            const int r = fr + 8 * rr;
+            const int i = qi * kAttnTile + r;
+            float pr2[2], ds2[2], w2[2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              const int jj = sub * 16 + 2 * q + e;
-              float x = fmaf(__uint_as_float(su[2 * q + e]), sc, -lse2);
-              if (HAS_BIAS) x = fmaf(gl, tbv[e], x);
+              const int idx = 4 * g + 2 * rr + e;
+              const int jj = hf * 64 + 8 * g + fc + e;   // key column inside the tile
+              float tb = 0.f;
+              if (HAS_BIAS) tb = tab_s[jj - r + N * kAttnTile - 1 - qi * kAttnTile];
+              float x = fmaf(s_acc[idx], sc, -r_lse[rr]);
+              if (HAS_BIAS) x = fmaf(r_gl[rr], tb, x);
               float pr = ex2f(x);
-              if (kMsk) pr = ((kmask >> jj) & 1u) ? 0.f : pr;
-              float dpv = __uint_as_float(du[2 * q + e]);
+              if (any_masked) pr = ((key_mask_s[jj >> 5] >> (jj & 31)) & 1u) ? 0.f : pr;
+              float dpv = d_acc[idx];
               bool keep = true;
               if (DROP) {  // O = (P o M) V / (1-p):  dP = M o (dO V^T) / (1-p);  dV takes the dropped probabilities (scaled at the end)
-                keep = ((keep_bits >> jj) & 1u) != 0u;
+                keep = (((e ? kw.y : kw.x) >> (i & 31)) & 1u) != 0u;
                 dpv = keep ? dpv * p.drop_rp : 0.f;
               }
-              const float ds = pr * fmaf(dpv, p.scale, -dsc);  // dS * scale
+              const float ds = pr * fmaf(dpv, p.scale, -r_dsc[rr]);  // dS * scale
               pr2[e] = keep ? pr : 0.f;
               ds2[e] = ds;
+              w2[e] = 0.f;
               if (HAS_BIAS) {
-                dg = fmaf(ds, tbv[e], dg);
-                w2[e] = gos * ds;
+                dg[rr] = fmaf(ds, tb, dg[rr]);
+                w2[e] = r_gos[rr] * ds;
               }
             }
-            pw[q] = pack_bf16x2(pr2[0], pr2[1]);
-            dw[q] = pack_bf16x2(ds2[0], ds2[1]);
-            if (HAS_BIAS) ww[q] = pack_bf16x2(w2[0], w2[1]);
-          }
-          if (sub == 0 && qi >= 1) {
-            // the accumulation MMAs of the previous tile have retired: the P / dS tiles may be overwritten, and its dQ is complete
-            mbar_wait(&mma_done, (qi - 1) & 1);
-            flush_dq(qi - 1);
-          }
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            store_sw128_chunk(sP, r, (j0 >> 3) + sub * 2 + c, make_uint4(pw[c * 4], pw[c * 4 + 1], pw[c * 4 + 2], pw[c * 4 + 3]));
-            store_sw128_chunk(sDS, r, (j0 >> 3) + sub * 2 + c, make_uint4(dw[c * 4], dw[c * 4 + 1], dw[c * 4 + 2], dw[c * 4 + 3]));
-          }
-          if (HAS_BIAS) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) wrow[sub * 8 + j] = ww[j];
+            // bf16 pairs into the operand tiles (K-major SWIZZLE_128B, block hf) and the diagonal staging tile
+            const int c = 8 * g + fc;  // column inside the 64-key block
+            const uint32_t off = static_cast<uint32_t>(hf * 16384 + r * 128 + ((g ^ (r & 7)) << 4) + (c & 7) * 2);
+            *reinterpret_cast<uint32_t*>(sP + off) = pack_bf16x2(pr2[0], pr2[1]);
+            *reinterpret_cast<uint32_t*>(sDS + off) = pack_bf16x2(ds2[0], ds2[1]);
+            if (HAS_BIAS) wtile[r * (kWStride2 / 2) + (c >> 1)] = pack_bf16x2(w2[0], w2[1]);
           }
         }
-      };
-      if (any_masked) body(std::true_type{}); else body(std::false_type{});
-
+        if (HAS_BIAS && hf == 0) {  // the first half's diagonal sums, then the staging tile is free for the second half
+          named_bar_sync(1, kConsumers);
+          diag_task(qi, 0, tid & 127, tid >> 7);
+          diag_task(qi, 0, tid & 127, (tid >> 7) + 2);
+          named_bar_sync(1, kConsumers);
+        }
+      }
       if (HAS_BIAS && p.dgate != nullptr) {
-        const int i = qi * kAttnTile + r;
-        if (i < T) atomicAdd(p.dgate + bh * T + i, dg * inv_scale);
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          float v = dg[rr];
+          v += __shfl_xor_sync(0xffffffffu, v, 1);
+          v += __shfl_xor_sync(0xffffffffu, v, 2);
+          const int i = qi * kAttnTile + fr + 8 * rr;
+          if ((lane & 3) == 0 && i < T) atomicAdd(p.dgate + bh * T + i, v * inv_scale);
+        }
       }
       fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      tc_fence_before();
-      mbar_arrive_cta(&ready[hf]);
-      r_lse = n_lse; r_delta = n_delta; r_gate = n_gate;
-      if (HAS_BIAS) {
-        mbar_wait(&ready[hf], qi & 1);  // all 256 threads of this half have staged their rows
-        diag_task(qi, ht & 127, ht >> 7);
-        diag_task(qi, ht & 127, (ht >> 7) + 2);
-        named_bar_sync(1 + hf, kCudaThreads / 2);  // the staging tile of this half may be overwritten
+      named_bar_sync(1, kConsumers);
+
+      // ---- dV += P^T dO, dK += dS^T Q (this WG's 64 keys), dQ = dS K (this WG's 64 queries)
+      {
+        const uint32_t ap = smem_u32(sP) + w * 16384, ads = smem_u32(sDS) + w * 16384;
+        const uint32_t bdo = smem_u32(sDO + st * 16384), bq = smem_u32(sQ + st * 16384);
+        const uint32_t adq = smem_u32(sDS) + w * 8192, bk = smem_u32(sK);
+        float dq[32];
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 8; ++k)  // K = 128 queries, 16 per step
+          wgmma_m64n64k16<1, 1>(dv_acc, make_smem_desc_sw128(ap + k * 2048, 16384, 1024),
+                                make_smem_desc_sw128(bdo + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          wgmma_m64n64k16<1, 1>(dk_acc, make_smem_desc_sw128(ads + k * 2048, 16384, 1024),
+                                make_smem_desc_sw128(bq + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+#pragma unroll
+        for (int k = 0; k < 8; ++k)  // K = 128 keys: two 64-key blocks, 16 per step
+          wgmma_m64n64k16<0, 1>(dq, make_smem_desc_sw128(adq + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
+                                make_smem_desc_sw128(bk + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+        wgmma_commit();
+        if (HAS_BIAS) {  // the second half's diagonal sums while the MMAs run (256 threads, 2 tasks each)
+          diag_task(qi, 1, tid & 127, tid >> 7);
+          diag_task(qi, 1, tid & 127, (tid >> 7) + 2);
+        }
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&qdo_free[st]);
+        // dQ rows of this WG -> fp32 reductions into dq_acc[b, q, h*64 + col]  (the staged dS already carries the softmax scale)
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int q = qi * kAttnTile + fr + 8 * rr;
+          if (q < T) {
+            float* dst = dq_acc + (static_cast<long long>(b) * T + q) * D + h * kHeadDim + fc;
+#pragma unroll
+            for (int g = 0; g < 8; ++g) red_add_v2(dst + 8 * g, dq[4 * g + 2 * rr], dq[4 * g + 2 * rr + 1]);
+          }
+        }
       }
+      named_bar_sync(1, kConsumers);  // P / dS / staging tiles may be overwritten by the next tile
     }
-    // ---- tail: last dQ tile, then the dK / dV accumulators
-    flush_dq(NQ - 1);
-    mbar_wait(&acc_done, 0);
-    tc_fence_after();
-    {
-      // 128 key rows x (64 dV + 64 dK) columns over 512 threads: g 0,1 -> dV columns 32*(g&1).., g 2,3 -> dK
-      uint32_t t0[32];
-      const uint32_t col = ((g < 2) ? kColDV : kColDK) + (g & 1) * 32;
-      tmem_ld_32x32b_x32(tmem + lane_addr + col, t0);
-      tmem_ld_wait();
-      if (DROP && g < 2) {  // dV = (P o M)^T dO / (1-p)
+    // ---- dK / dV rows of this WG (keys k0 + 64 w ..): bf16 pairs straight from the fragments
 #pragma unroll
-        for (int i = 0; i < 32; ++i) t0[i] = __float_as_uint(__uint_as_float(t0[i]) * p.drop_rp);
-      }
-      const int key = k0 + r;
+    for (int rr = 0; rr < 2; ++rr) {
+      const int key = k0 + fr + 8 * rr;
       if (key < T) {
-        __nv_bfloat16* dst = p.dqkv + (static_cast<long long>(b) * T + key) * (3 * D) + ((g < 2) ? 2 * D : D) + h * kHeadDim +
-                             (g & 1) * 32;
+        __nv_bfloat16* dst = p.dqkv + (static_cast<long long>(b) * T + key) * (3 * D) + h * kHeadDim + fc;
 #pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          uint4 w;
-          w.x = pack_bf16x2(__uint_as_float(t0[v * 8 + 0]), __uint_as_float(t0[v * 8 + 1]));
-          w.y = pack_bf16x2(__uint_as_float(t0[v * 8 + 2]), __uint_as_float(t0[v * 8 + 3]));
-          w.z = pack_bf16x2(__uint_as_float(t0[v * 8 + 4]), __uint_as_float(t0[v * 8 + 5]));
-          w.w = pack_bf16x2(__uint_as_float(t0[v * 8 + 6]), __uint_as_float(t0[v * 8 + 7]));
-          *reinterpret_cast<uint4*>(dst + v * 8) = w;
+        for (int g = 0; g < 8; ++g) {
+          const float rp = DROP ? p.drop_rp : 1.0f;   // dV = (P o M)^T dO / (1-p)
+          *reinterpret_cast<uint32_t*>(dst + 2 * D + 8 * g) = pack_bf16x2(dv_acc[4 * g + 2 * rr] * rp, dv_acc[4 * g + 2 * rr + 1] * rp);
+          *reinterpret_cast<uint32_t*>(dst + D + 8 * g) = pack_bf16x2(dk_acc[4 * g + 2 * rr], dk_acc[4 * g + 2 * rr + 1]);
         }
       }
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   if (HAS_BIAS) {
     // per-CTA accumulators -> global (the relative-position table is shared by all layers: atomics)
@@ -462,10 +371,6 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
         if (gi >= 0 && gi < 2 * T - 1 && v != 0.f) atomicAdd(p.dtab + static_cast<long long>(h) * (2 * T - 1) + gi, v);
       }
     }
-  }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_dealloc(tmem, 512);
   }
 }
 
@@ -513,27 +418,15 @@ __global__ void __launch_bounds__(256) attn_dq_convert_kernel(float* __restrict_
 
 int make_qkv_tmap(CUtensorMap* out, const void* qkv, int T, int B, int D3, int box_rows);
 
-}  // namespace b200
 
-using namespace b200;
-
-extern "C" {
-
-// Fused backward of b200s_attn_fwd.  Same contract as b200s_attn_bwd plus dq_acc: fp32 [B,T,D] workspace that must be ZERO
-// on entry and is zero again on return (the q gradient is reduced there across key tiles before it is rounded to bf16).
-int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
-                                 const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv,
-                                 float* dgate, float* dtab, int B, int T, int H, float scale, float drop_p,
-                                 const uint32_t* drop_mask, b200s_stream stream) {
-  B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv && dq_acc, "attn_bwd_fused: null pointer");
-  B200_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f, "attn_bwd_fused: dropout p=%f out of range [0,1)", static_cast<double>(drop_p));
-  B200_CHECK_ARG(drop_p == 0.f || drop_mask != nullptr, "attn_bwd_fused: dropout needs the mask written by b200s_attn_fwd_dropout");
-  B200_CHECK_ARG(T >= 1 && T <= 2048, "attn_bwd_fused: T=%d out of range (1..2048)", T);
-  B200_CHECK_ARG(!tab || (dgate && dtab), "attn_bwd_fused: bias given but dgate/dtab missing");
+// Delta pre-kernel, the fused kernel and the dQ conversion on one stream (see the entry points below for the contract).
+static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
+                           const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv, float* dgate,
+                           float* dtab, int B, int T, int H, float scale, float drop_p, const uint32_t* drop_mask,
+                           cudaStream_t st) {
   const int D = H * kHeadDim;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long rows = static_cast<long long>(B) * T;
-  B200_CHECK_CUDA(launch_pdl(attn_delta2_kernel, dim3(static_cast<unsigned>(ceil_div_ll(rows * 32, 256))), dim3(256), 0, st, 
+  B200_CHECK_CUDA(launch_pdl(attn_delta2_kernel, dim3(static_cast<unsigned>(ceil_div_ll(rows * 32, 256))), dim3(256), 0, st,
       static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), B, T, H, delta,
       tab != nullptr ? dgate : nullptr));
   B200_CHECK_LAUNCH();
@@ -557,8 +450,8 @@ int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* d
   p.drop_mask = const_cast<uint32_t*>(drop_mask);
   p.drop_rp = 1.0f / (1.0f - drop_p);
   const int N = p.n_tiles;
-  const int smem = kFTab + sizeof(float) * ((tab != nullptr ? 2 * bwd_tab_stride(N) : 0) + (N + 1) * kAttnTile) + 1024;
-  B200_CHECK_ARG(smem <= 232448 - 512, "attn_bwd_fused: T=%d needs %d bytes of shared memory", T, smem);
+  const int smem = attn_bwd_smem_bytes(N, tab != nullptr);
+  B200_CHECK_ARG(smem <= 232448 - 512, "attn_bwd: T=%d needs %d bytes of shared memory", T, smem);
   dim3 grid(N, H, B);
   void (*kern)(const CUtensorMap, const CUtensorMap, const AttnParams, float*) =
       tab != nullptr ? (drop ? attn_bwd_fused_kernel<true, true> : attn_bwd_fused_kernel<true, false>)
@@ -567,10 +460,52 @@ int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* d
   B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFThreads), smem, st, tm_qkv, tm_do, p, dq_acc));
   B200_CHECK_LAUNCH();
   const long long nvec = rows * (D / 8);
-  const int blocks = static_cast<int>(std::min<long long>(ceil_div_ll(nvec, 256), 148 * 16));
+  const int blocks = static_cast<int>(std::min<long long>(ceil_div_ll(nvec, 256), static_cast<long long>(sm_count()) * 16));
   B200_CHECK_CUDA(launch_pdl(attn_dq_convert_kernel, dim3(blocks), dim3(256), 0, st, dq_acc, static_cast<__nv_bfloat16*>(dqkv), rows, D));
   B200_CHECK_LAUNCH();
   return 0;
+}
+
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+// Backward of b200s_attn_fwd.  out/dout: bf16 [B,T,D]; lse from the forward; delta: fp32 [B,H,T] workspace;
+// dqkv: bf16 [B,T,3D] (fully written for valid rows); dgate: fp32 [B,H,T] (written); dtab: fp32 [H,2T-1] (ACCUMULATED with
+// atomics -- the caller zeroes it once per step, the table is shared by all layers).  gate/tab/dgate/dtab NULL = no bias.
+// The fp32 dQ reduction buffer is allocated on the stream for the call (b200s_attn_bwd_fused takes it from the caller).
+int b200s_attn_bwd(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
+                   const uint8_t* key_pad, const float* lse, float* delta, void* dqkv, float* dgate, float* dtab, int B,
+                   int T, int H, float scale, b200s_stream stream) {
+  B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv, "attn_bwd: null pointer");
+  B200_CHECK_ARG(T >= 1 && T <= 4096, "attn_bwd: T=%d out of range (1..4096)", T);
+  B200_CHECK_ARG(!tab || (dgate && dtab), "attn_bwd: bias given but dgate/dtab missing");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t bytes = sizeof(float) * static_cast<size_t>(B) * T * H * kHeadDim;
+  void* dq_acc = nullptr;
+  B200_CHECK_CUDA(cudaMallocAsync(&dq_acc, bytes, st));
+  B200_CHECK_CUDA(cudaMemsetAsync(dq_acc, 0, bytes, st));
+  const int rc = attn_bwd_launch(qkv, out, dout, gate, tab, key_pad, lse, delta, static_cast<float*>(dq_acc), dqkv, dgate, dtab, B,
+                                 T, H, scale, 0.f, nullptr, st);
+  B200_CHECK_CUDA(cudaFreeAsync(dq_acc, st));
+  return rc;
+}
+
+// Fused backward of b200s_attn_fwd.  Same contract as b200s_attn_bwd plus dq_acc: fp32 [B,T,D] workspace that must be ZERO
+// on entry and is zero again on return (the q gradient is reduced there across key tiles before it is rounded to bf16).
+int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
+                                 const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv,
+                                 float* dgate, float* dtab, int B, int T, int H, float scale, float drop_p,
+                                 const uint32_t* drop_mask, b200s_stream stream) {
+  B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv && dq_acc, "attn_bwd_fused: null pointer");
+  B200_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f, "attn_bwd_fused: dropout p=%f out of range [0,1)", static_cast<double>(drop_p));
+  B200_CHECK_ARG(drop_p == 0.f || drop_mask != nullptr, "attn_bwd_fused: dropout needs the mask written by b200s_attn_fwd_dropout");
+  B200_CHECK_ARG(T >= 1 && T <= 2048, "attn_bwd_fused: T=%d out of range (1..2048)", T);
+  B200_CHECK_ARG(!tab || (dgate && dtab), "attn_bwd_fused: bias given but dgate/dtab missing");
+  return attn_bwd_launch(qkv, out, dout, gate, tab, key_pad, lse, delta, dq_acc, dqkv, dgate, dtab, B, T, H, scale, drop_p,
+                         drop_mask, static_cast<cudaStream_t>(stream));
 }
 
 int b200s_attn_bwd_fused(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,

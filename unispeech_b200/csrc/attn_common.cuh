@@ -46,30 +46,8 @@ static inline long long attn_drop_mask_words(int B, int H, int T) {
   return static_cast<long long>(B) * H * (4 * n) * (kAttnTile * n);
 }
 
-// fill the shared-memory slice of the bias table used by query tile q0: tab_s[idx] = tab[h, idx + T-1-(q0+127)]
-__device__ __forceinline__ void load_tab_slice(float* tab_s, const float* tab, int h, int T, int q0, int n_tiles) {
-  const int len = n_tiles * kAttnTile + kAttnTile;
-  const int base = (T - 1) - (q0 + kAttnTile - 1);
-  for (int i = threadIdx.x; i < len; i += blockDim.x) {
-    const int gi = i + base;
-    tab_s[i] = (tab != nullptr && gi >= 0 && gi < 2 * T - 1) ? tab[static_cast<long long>(h) * (2 * T - 1) + gi] : 0.f;
-  }
-}
-
-// additive key mask (0 / -inf) for all key positions of the padded key range, plus per-tile "has masked key" flags
-__device__ __forceinline__ void load_key_mask(float* kbias, int* tile_flags, const uint8_t* key_pad, int b, int T,
-                                              int n_tiles) {
-  for (int i = threadIdx.x; i < n_tiles; i += blockDim.x) tile_flags[i] = 0;
-  __syncthreads();
-  for (int j = threadIdx.x; j < n_tiles * kAttnTile; j += blockDim.x) {
-    const bool masked = (j >= T) || (key_pad != nullptr && key_pad[static_cast<long long>(b) * T + j] != 0);
-    kbias[j] = masked ? -INFINITY : 0.f;
-    if (masked) tile_flags[j / kAttnTile] = 1;
-  }
-}
-
 // write 8 consecutive bf16 of row r, 16-byte chunk index `chunk` (0..15 over 128 columns) into a K-major SWIZZLE_128B tile
-// made of two [128 rows][64 cols] blocks (the layout tcgen05.mma expects for a K-major operand, and -- read as
+// made of two [128 rows][64 cols] blocks (the layout of a K-major wgmma operand, and -- read as
 // MN-major -- for the transposed use).
 __device__ __forceinline__ void store_sw128_chunk(uint8_t* tile, int r, int chunk, uint4 v) {
   const int kb = chunk >> 3;       // which 64-column block

@@ -1,15 +1,13 @@
-// Host side of the tcgen05 GEMM family: TMA tensor-map construction, tile mapping and launch.
+// Host side of the wgmma GEMM family: TMA tensor-map construction, tile mapping and launch.
 #include <stdarg.h>
 #include <stdlib.h>
 
 #include <algorithm>
-#include <atomic>
 #include <mutex>
 
 #include "../../include/unispeech_b200.h"
 #include "common.h"
 #include "gemm.cuh"
-#include "gemm2.cuh"
 
 namespace b200 {
 
@@ -37,7 +35,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -135,137 +133,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmP
   return 0;
 }
 
-// persistent CTA-pair kernel (gemm2.cuh): cluster (2,1,1), one pair per two SMs
-// how many CTA pairs share (multicast) the B operand: 2 when B200S_GEMM_CLUSTER4=1 and the problem has >= 2 M tiles
-// (experimental, off by default: measured SLOWER than independent pairs on B200 -- a 4-CTA cluster only gets 132 of the 148
-// SMs and the multicast does not raise the L2 -> SM throughput at this cluster size; kept for the A/B numbers in DESIGN.md)
-static int cluster_pairs_for(int m_tiles_total) {
-  const char* e = getenv("B200S_GEMM_CLUSTER4");
-  return (e && e[0] == '1' && m_tiles_total >= 2) ? 2 : 1;
-}
-
-static std::atomic<int> g_reserved_sms{0};
-
-// opt the kernel into its shared-memory size (once) and report how many clusters can be resident at once (a 4-CTA cluster
-// does not fit every GPC remainder, so fewer than sm_count / 4 are)
-template <bool A_MN, bool B_MN, int KIND, int NPAIR>
-static cudaError_t pair_kernel_setup(int* units) {
-  using Cfg = Gemm2Cfg<KIND>;
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  static int max_units = 0;
-  std::call_once(once, [] {
-    attr_err = cudaFuncSetAttribute(gemm_bf16_pair_kernel<A_MN, B_MN, KIND, NPAIR>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
-    max_units = sm_count() / (2 * NPAIR);
-    if (attr_err == cudaSuccess && NPAIR > 1) {
-      cudaLaunchConfig_t q;
-      memset(&q, 0, sizeof(q));
-      q.gridDim = dim3(2 * NPAIR * max_units, 1, 1);
-      q.blockDim = dim3(Cfg::kThreads, 1, 1);
-      q.dynamicSmemBytes = Cfg::kSmemBytes;
-      cudaLaunchAttribute qa[1];
-      qa[0].id = cudaLaunchAttributeClusterDimension;
-      qa[0].val.clusterDim.x = 2 * NPAIR;
-      qa[0].val.clusterDim.y = 1;
-      qa[0].val.clusterDim.z = 1;
-      q.attrs = qa;
-      q.numAttrs = 1;
-      int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, gemm_bf16_pair_kernel<A_MN, B_MN, KIND, NPAIR>, &q) == cudaSuccess && n > 0)
-        max_units = std::min(max_units, n);
-    }
-  });
-  *units = max_units;
-  // SMs set aside for a concurrent collective (b200s_reserve_sms): a persistent kernel that asks for every SM while NCCL holds a
-  // few would leave its last clusters waiting for the others to finish -- up to twice the kernel's time for a statically
-  // scheduled grid
-  const int keep = g_reserved_sms.load(std::memory_order_relaxed);
-  if (keep > 0) *units = std::max(1, std::min(max_units, (sm_count() - keep) / (2 * NPAIR)));
-  return attr_err;
-}
-
-// output tensor maps of the staged epilogue: one SWIZZLE_128B box = 32 rows x 64 bf16 columns of [batches][rows][N]
-static int make_out_tmap(CUtensorMap* tm, const EpiTensor& t, int N, int rows, int batches) {
-  ViewSpec v{t.p, {N, rows, batches, 1}, {t.ld, batches > 1 ? t.bs : 0, 0}, {64, 32, 1, 1}};
-  return make_tmap(tm, v);
-}
-
-template <bool A_MN, bool B_MN, int KIND, int NPAIR>
-static int launch_gemm_pair_n(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<KIND>;
-  CUtensorMap to, to2;
-  if (KIND != EK_F32) {
-    const int batches = p.tiles_total / (p.m_tiles_per_batch * p.n_tiles);
-    if (make_out_tmap(&to, p.out, p.n_total, p.m_rows, batches)) return -3;
-    to2 = to;
-    if (p.out2.p != nullptr && make_out_tmap(&to2, p.out2, p.n_total, p.m_rows, batches)) return -3;
-  } else {
-    to = ta;  // unused by the fp32 kind
-    to2 = ta;
-  }
-  int max_units = 0;
-  B200_CHECK_CUDA((pair_kernel_setup<A_MN, B_MN, KIND, NPAIR>(&max_units)));
-  const int m_tiles_total = p.tiles_total / p.n_tiles;
-  const int items = ceil_div(m_tiles_total, NPAIR) * p.n_tiles * p.splits;
-  const int pairs = p.stream_k ? std::max(1, max_units) : std::max(1, std::min(items, max_units));  // stream-K: every pair has a range
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(2 * NPAIR * pairs, 1, 1);
-  cfg.blockDim = dim3(Cfg::kThreads, 1, 1);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2 * NPAIR;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_pair_kernel<A_MN, B_MN, KIND, NPAIR>, ta, tb, to, to2, p));
-  B200_CHECK_LAUNCH();
-  return 0;
-}
-template <bool A_MN, bool B_MN, int KIND>
-static int launch_gemm_pair(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int npair,
-                            cudaStream_t stream) {
-  return npair == 2 ? launch_gemm_pair_n<A_MN, B_MN, KIND, 2>(ta, tb, p, stream)
-                    : launch_gemm_pair_n<A_MN, B_MN, KIND, 1>(ta, tb, p, stream);
-}
-
-// stream-K schedule of the weight-gradient GEMMs (B200S_WGRAD_STREAMK=0: whole (split, tile) items, the round-1 schedule)
-static bool wgrad_stream_k() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200S_WGRAD_STREAMK");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-// 0/1 switch for the CTA-pair kernel (B200S_GEMM_PAIR=0 forces the single-CTA kernel; used by the A/B micro-benchmarks)
-static bool pair_kernel_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200S_GEMM_PAIR");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-static int gemm_debug_flags() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200S_GEMM_DEBUG");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-
 static void fill_epilogue(GemmParams& p, const b200s_epilogue* e) {
-  p.debug = gemm_debug_flags();
   p.bias = nullptr;
   p.colsum = nullptr;
   p.out2 = {nullptr, 0, 0};
@@ -288,20 +156,6 @@ static void fill_epilogue(GemmParams& p, const b200s_epilogue* e) {
   }
   p.res1 = {const_cast<void*>(e->res1), e->res1_bs, e->res1_ld};
   p.res2 = {const_cast<void*>(e->res2), e->res2_bs, e->res2_ld};
-  // compacted input list of the pair kernel's staged epilogue
-  if (e->dgelu) p.in[p.n_in++] = p.aux;
-  if (e->res1) p.in[p.n_in++] = p.res1;
-  if (e->res2) p.in[p.n_in++] = p.res2;
-}
-
-// all row strides / batch strides / base pointers of the bf16 epilogue tensors 16-byte aligned (the staged epilogue moves
-// 16-byte chunks); otherwise the single-CTA kernel (element-wise tail) is used
-static bool epilogue_aligned(const GemmParams& p) {
-  auto ok = [](const EpiTensor& t) {
-    return t.p == nullptr || ((reinterpret_cast<uintptr_t>(t.p) & 15) == 0 && t.ld % 8 == 0 && t.bs % 8 == 0);
-  };
-  return ok(p.out) && ok(p.out2) && ok(p.aux) && ok(p.res1) && ok(p.res2) &&
-         (p.bias == nullptr || (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0);
 }
 
 static int check_epilogue(const b200s_epilogue* e) {
@@ -336,7 +190,7 @@ int b200s_check_device(void) {
   int major = 0, minor = 0;
   B200_CHECK_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   B200_CHECK_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  B200_CHECK_ARG(major == 10, "unispeech_b200 needs an sm_100 device (B200); found sm_%d%d", major, minor);
+  B200_CHECK_ARG(major == 9 && minor == 0, "unispeech_b200 needs an sm_90 device (H100); found sm_%d%d", major, minor);
   return 0;
 }
 
@@ -359,36 +213,6 @@ static int gemm_rows_impl(const void* a, long long a_bs, long long a_rs, int row
   memset(&p, 0, sizeof(p));
   fill_epilogue(p, epi);
   p.out = {out, out_bs, out_ld};
-  const bool pair_epi_ok = epilogue_aligned(p) && !((p.flags & EPI_GELU) && p.n_in > 1);
-  if (pair_kernel_enabled() && pair_epi_ok && N >= 256 && rows >= 256 && static_cast<long long>(rows) * batches >= 2048) {
-    // persistent CTA-pair kernel: 256 x 256 tiles, each CTA stages 128 A rows and 128 of the 256 B rows (loaded as one box,
-    // or as 64-row quarters multicast between two pairs)
-    const int npair = m_valid != nullptr ? 1 : cluster_pairs_for(ceil_div(rows, 256) * batches);
-    // ragged batch: tiles beyond a batch's valid rows are zero-filled instead of computed (too many batches for the kernel's
-    // prefix table: computed densely, which is what the padded path has always done)
-    p.m_valid = (batches <= kMaxRagBatches && ceil_div(rows, 256) * batches < 65536) ? m_valid : nullptr;
-    ViewSpec vb2{w, {K, N, 1, 1}, {K, 0, 0}, {64, npair == 2 ? 64 : 128, 1, 1}};
-    if (make_tmap(&tb, vb2)) return -3;
-    p.m_rows = rows;
-    p.m_tile_stride = 256;
-    p.m_tile_valid = 256;
-    p.m_tiles_per_batch = ceil_div(rows, 256);
-    p.n_total = N;
-    p.n_out_stride = 256;
-    p.n_tile_valid = 256;
-    p.n_tiles = ceil_div(N, 256);
-    p.tiles_total = p.m_tiles_per_batch * batches * p.n_tiles;
-    p.splits = 1;
-    p.k_blocks = K / 64;
-    p.k_blocks_per_batch = 0;
-    p.k_blocks_per_split = p.k_blocks;
-    // A coords: (k0, m0 [+128*rank, added by the kernel], mb, 0)   B coords: (k0, n_tile*256 + sub(=128*rank), 0, 0)
-    p.ca[0][4] = 1; p.ca[1][1] = 1; p.ca[2][2] = 1;
-    p.cb[0][4] = 1; p.cb[1][3] = 256; p.cb[1][7] = 1;
-    if (p.flags & EPI_GELU) return launch_gemm_pair<false, false, EK_GELU>(ta, tb, p, npair, st);
-    if (p.flags & EPI_DGELU) return launch_gemm_pair<false, false, EK_DGELU>(ta, tb, p, npair, st);
-    return launch_gemm_pair<false, false, EK_LINEAR>(ta, tb, p, npair, st);
-  }
   const int block_n = (N >= 128) ? 128 : 64;
   ViewSpec vb{w, {K, N, 1, 1}, {K, 0, 0}, {64, block_n, 1, 1}};
   if (make_tmap(&tb, vb)) return -3;
@@ -406,17 +230,17 @@ static int gemm_rows_impl(const void* a, long long a_bs, long long a_rs, int row
   // A coords: (k0, m0, mb, 0)   B coords: (k0, n_tile*block_n, 0, 0)
   p.ca[0][4] = 1; p.ca[1][1] = 1; p.ca[2][2] = 1;
   p.cb[0][4] = 1; p.cb[1][3] = block_n;
+  // ragged batch: tiles beyond a batch's valid rows are zero-filled instead of computed
+  p.m_valid = m_valid;
   dim3 grid(ceil_div(N, block_n), p.m_tiles_per_batch * batches, 1);
   B200_CHECK_ARG(grid.y <= 65535, "gemm_rows: too many M tiles (%u)", grid.y);
   return block_n == 128 ? launch_gemm<128, false, false>(ta, tb, p, grid, st)
                         : launch_gemm<64, false, false>(ta, tb, p, grid, st);
 }
 
-/* SMs the persistent GEMM kernels leave free for a concurrently running collective (data-parallel runs: NCCL's CTAs, bounded by
- * NCCL_MAX_CTAS).  0 = use every SM (default). */
+/* Deprecated (see the header): range check only. */
 int b200s_reserve_sms(int sms) {
   B200_CHECK_ARG(sms >= 0 && sms < sm_count(), "reserve_sms: %d out of range", sms);
-  g_reserved_sms.store(sms, std::memory_order_relaxed);
   return 0;
 }
 
@@ -445,58 +269,6 @@ static int gemm_wgrad_impl(const void* y, long long y_bs, long long y_rs, const 
   ViewSpec vb{x, {K, rows, batches, 1}, {x_rs, batches > 1 ? x_bs : 0, 0}, {64, 64, 1, 1}};
   if (make_tmap(&tb, vb)) return -3;
 
-  if (pair_kernel_enabled() && N >= 256 && K >= 256 && static_cast<long long>(rows) * batches >= 1024) {
-    // persistent CTA-pair kernel, both operands MN-major; work items = (K split, tile)
-    GemmParams p;
-    memset(&p, 0, sizeof(p));
-    p.m_rows = N;
-    p.m_tile_stride = 256;
-    p.m_tile_valid = 256;
-    p.m_tiles_per_batch = ceil_div(N, 256);
-    p.n_total = K;
-    p.n_out_stride = 256;
-    p.n_tile_valid = 256;
-    p.n_tiles = ceil_div(K, 256);
-    p.tiles_total = p.m_tiles_per_batch * p.n_tiles;
-    p.k_blocks_per_batch = ceil_div(rows, 64);
-    p.k_blocks = p.k_blocks_per_batch * batches;
-    // ragged batch: row blocks beyond a batch's valid rows are neither loaded nor multiplied
-    p.k_valid = (batches <= kMaxRagBatches && p.k_blocks < 65536) ? k_valid : nullptr;
-    // multicast pays only when the M (output-feature) tile count pairs up without much waste
-    const int npair = (p.m_tiles_per_batch % 2 == 0 || p.m_tiles_per_batch >= 8) ? cluster_pairs_for(p.m_tiles_per_batch) : 1;
-    int units = 0;
-    if (npair == 2) B200_CHECK_CUDA((pair_kernel_setup<true, true, EK_F32, 2>(&units)));
-    else B200_CHECK_CUDA((pair_kernel_setup<true, true, EK_F32, 1>(&units)));
-    // about one work item per cluster: the fp32 reduction epilogue of a split is the expensive part, the main loop is cheap
-    const int pairs = std::max(1, units);
-    int splits = std::max(1, pairs / (ceil_div(p.m_tiles_per_batch, npair) * p.n_tiles));
-    if (const char* e = getenv("B200S_WGRAD_SPLITS")) {  // micro-benchmark knob
-      if (atoi(e) > 0) splits = atoi(e);
-    }
-    if (splits > p.k_blocks) splits = p.k_blocks;
-    p.k_blocks_per_split = ceil_div(p.k_blocks, splits);
-    p.splits = ceil_div(p.k_blocks, p.k_blocks_per_split);
-    const int tiles = p.m_tiles_per_batch * p.n_tiles;
-    // (few tiles, e.g. the 1024 x 1024 out_proj gradient with 16: whole (split, tile) items already balance and a range per pair
-    // only adds partial-tile epilogues -- measured 23.6 vs 22.9 us; from ~half a wave of tiles on, stream-K wins: 47 vs 64 us for
-    // the 3072 x 1024 qkv gradient, 60 vs 64 us for the FFN ones, profiles/r02_microbench_gemm_large.txt)
-    if (npair == 1 && wgrad_stream_k() && 2 * tiles >= pairs && tiles * p.k_blocks >= 2 * pairs) {
-      // stream-K: equal K-block ranges per pair; a range of `per` blocks touches at most ceil(per / kbt) + 1 tiles (kbt = K blocks
-      // per tile; for a ragged batch only the live ones count, which makes `per` smaller, never larger)
-      const int per = ceil_div(tiles * p.k_blocks, pairs);
-      p.stream_k = 1;
-      p.splits = std::min(tiles, ceil_div(per, std::max(1, p.k_blocks)) + 1);
-      if (p.k_valid != nullptr) p.splits = std::min(tiles, p.splits + 1);  // live blocks per tile unknown on the host: one spare segment
-    }
-    // A coords: (m0 [+128*rank] + sub, k0, kbatch, 0)   B coords: (n_tile*256 + sub (=128*rank + 64*i), k0, kbatch, 0)
-    p.ca[0][1] = 1; p.ca[0][7] = 1; p.ca[1][4] = 1; p.ca[2][5] = 1;
-    p.cb[0][3] = 256; p.cb[0][7] = 1; p.cb[1][4] = 1; p.cb[2][5] = 1;
-    p.flags = EPI_OUT_F32 | (p.splits > 1 ? EPI_ATOMIC : EPI_ACCUM);
-    fill_epilogue(p, nullptr);
-    p.out = {dw, 0, dw_ld};
-    return launch_gemm_pair<true, true, EK_F32>(ta, tb, p, npair, static_cast<cudaStream_t>(stream));
-  }
-
   GemmParams p;
   memset(&p, 0, sizeof(p));
   p.m_rows = N;
@@ -520,6 +292,8 @@ static int gemm_wgrad_impl(const void* y, long long y_bs, long long y_rs, const 
   p.flags = EPI_OUT_F32 | EPI_ATOMIC;
   fill_epilogue(p, nullptr);
   p.out = {dw, 0, dw_ld};
+  // ragged batch: row blocks beyond a batch's valid rows are neither loaded nor multiplied
+  p.k_valid = k_valid;
   dim3 grid(ceil_div(K, block_n), p.m_tiles_per_batch, splits);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   return block_n == 128 ? launch_gemm<128, true, true>(ta, tb, p, grid, st)
@@ -545,6 +319,7 @@ int b200s_posconv_gemm(const void* xpad, long long xpad_bs, int T, int B, int D,
   const int Cg = D / G;
   B200_CHECK_ARG(Cg <= 64 && Cg % 8 == 0, "posconv_gemm: channels per group %d must be <=64 and a multiple of 8", Cg);
   B200_CHECK_ARG(D % 8 == 0, "posconv_gemm: D must be a multiple of 8");
+  B200_CHECK_ARG(taps >= 1, "posconv_gemm: taps=%d must be positive", taps);
   if (check_epilogue(epi)) return -1;
 
   CUtensorMap ta, tb;
@@ -569,7 +344,7 @@ int b200s_posconv_gemm(const void* xpad, long long xpad_bs, int T, int B, int D,
   dim3 grid(G, p.m_tiles_per_batch * B, 1);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
-  if (taps <= 129 && !(p.debug & 16)) {
+  if (taps <= 129) {
     // windowed kernel: the A operand (256 input rows of this group's channels) is loaded once per tile, every tap reads it
     // shifted by one row; rows past T + taps - 1 (end of this utterance's zero padding) are zero-filled by the tensor map
     ViewSpec vw{xpad, {D, T + taps - 1, B, 1}, {D, B > 1 ? xpad_bs : 0, 0}, {64, 256, 1, 1}};

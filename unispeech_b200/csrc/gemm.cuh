@@ -1,10 +1,11 @@
-// Generic bf16 tcgen05 GEMM for sm_100a:  D[M,N] (+)= A[M,K] * B[N,K]^T, fp32 accumulation in TMEM.
+// Generic bf16 wgmma GEMM for sm_90a:  D[M,N] (+)= A[M,K] * B[N,K]^T, fp32 accumulation in registers.
 //
 // One CTA computes one 128 x BLOCK_N output tile (optionally one K-split of it).  Warp roles:
-//   warp 0 : TMA producer (one elected lane)   global -> 128B-swizzled shared memory ring
-//   warp 1 : TMEM allocator + MMA issuer (one elected lane, tcgen05.mma cta_group::1 kind::f16)
-//   warps 2-5 : epilogue (tcgen05.ld 32x32b, one accumulator row per thread) with a fused
-//               bias / GELU / GELU' / residual / fp32-atomic (split-K) tail.
+//   warpgroups 0-1 : consumers, 64 accumulator rows each (wgmma m64nNk16, one K block in flight while the next is issued)
+//   warp 8 : TMA producer (one elected lane)   global -> 128B-swizzled shared memory ring
+//   After the main loop the consumers stage the fp32 tile in the (then idle) operand ring and run the fused
+//   bias / GELU / GELU' / residual / fp32-atomic (split-K) tail on it, one accumulator row per thread.  Two CTAs share an SM
+//   (shared memory and registers are sized for it), so one CTA's epilogue runs under the other's main loop.
 // Operands may be K-major (reduction dim contiguous) or MN-major (reduction dim strided; used by the
 // weight-gradient GEMMs), selected per operand.  All the "view" tricks of the WavLM path (strided
 // Conv1d as an overlapping-row view, grouped pos_conv taps, per-batch tiles) are expressed on the host
@@ -34,9 +35,6 @@ enum : int {
 // variables the coordinate matrices multiply: {1, m0, mb, n_tile, k0, kbatch, kb, sub}
 constexpr int kCoordVars = 8;
 
-// ragged batches: at most this many batches per launch take the live-unit schedule (the per-batch prefix lives in shared memory)
-constexpr int kMaxRagBatches = 255;
-
 struct GemmParams {
   int m_rows;            // valid rows per batch
   int m_tiles_per_batch; // ceil over m_tile_stride
@@ -54,22 +52,12 @@ struct GemmParams {
   const float* bias;     // [n] fp32 or null
   float* colsum;         // [n] fp32 or null (EPI_COLSUM)
   EpiTensor out, out2, aux, res1, res2;
-  // persistent CTA-pair kernel only (gemm2.cuh): work items = (split, m_tile, n_tile), n fastest
-  int n_tiles, tiles_total, splits;
-  // bf16 epilogue inputs in application order, compacted on the host: in[0] is the GELU' argument when EPI_DGELU is set,
-  // the others are added (res1, res2)
-  EpiTensor in[3];
-  int n_in;
-  int debug;  // diagnostics only (B200S_GEMM_DEBUG): 1 = no epilogue global traffic, 2 = no MMAs, 4 = no TMA loads
-  // ragged batches (CTA-pair kernel only; null = every row counts).  m_valid[b]: rows of batch b that hold real frames -- an M
-  // tile that starts at or beyond it is not computed, its output rows are written as zeros.  k_valid[b] (weight gradients, K
-  // iterates over (batch, row block)): row blocks that start at or beyond it are not loaded / multiplied (their gradient rows
-  // are zero by construction: nothing downstream of a padded frame reaches the loss).
+  // ragged batches (null = every row counts).  m_valid[b]: rows of batch b that hold real frames -- an M tile that starts at or
+  // beyond it is not computed, its output rows are written as zeros.  k_valid[b] (weight gradients, K iterates over (batch, row
+  // block)): row blocks that start at or beyond it are not loaded / multiplied (their gradient rows are zero by construction:
+  // nothing downstream of a padded frame reaches the loss).
   const int* m_valid;
   const int* k_valid;
-  // weight gradients (fp32 kind, one pair per cluster): the (tile, K block) space is cut into one contiguous range per CTA pair
-  // (stream-K) instead of whole (split, tile) items; `splits` then holds the largest number of tiles a range can touch
-  int stream_k;
 };
 
 template <int BLOCK_N>
@@ -78,8 +66,11 @@ struct GemmCfg {
   static constexpr int kABytes = 128 * 128;          // 128 rows x 64 bf16
   static constexpr int kBBytes = BLOCK_N * 128;
   static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kAccPitch = BLOCK_N + 8;      // fp32 staging row (floats): conflict-free fragment stores
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024;
-  static constexpr int kThreads = 192;
+  static constexpr int kThreads = 288;
+  static_assert(128 * kAccPitch * 4 <= kStages * kStageBytes, "accumulator staging must fit in the operand ring");
+  static_assert(2 * (kSmemBytes + 1024) <= 233472, "two CTAs per SM");
 };
 
 __device__ __forceinline__ int coord_dot(const int* row, const int* v) {
@@ -126,14 +117,16 @@ __device__ __forceinline__ uint4 pack_bf16x8(const float* a8) {
   return w;
 }
 
-// One 32-column chunk of the fused epilogue for this thread's accumulator row (taddr = TMEM address of the chunk).
-__device__ __forceinline__ void epilogue_chunk32(const GemmParams& p, const EpiRow& e, uint32_t taddr, int c0, int n_valid,
+// One 32-column chunk of the fused epilogue for this thread's accumulator row (src = the chunk in the fp32 staging tile).
+__device__ __forceinline__ void epilogue_chunk32(const GemmParams& p, const EpiRow& e, const float* src, int c0, int n_valid,
                                                  int col_base, bool row_ok, int lane) {
   const int flags = p.flags;
-  uint32_t acc_u[32];
-  tmem_ld_32x32b_x32(taddr, acc_u);
-  tmem_ld_wait();
-  float* acc = reinterpret_cast<float*>(acc_u);
+  float acc[32];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 v = reinterpret_cast<const float4*>(src)[j];
+    acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.z; acc[4 * j + 3] = v.w;
+  }
   const bool full = (c0 + 32 <= n_valid);  // warp-uniform
   if (p.bias != nullptr) {
     const float* bp = p.bias + col_base + c0;
@@ -218,10 +211,51 @@ __device__ __forceinline__ void epilogue_chunk32(const GemmParams& p, const EpiR
   }
 }
 
+
+template <int N, bool TA, bool TB>
+__device__ __forceinline__ void wgmma_tile(float* acc, uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (N == 64) wgmma_m64n64k16<TA ? 1 : 0, TB ? 1 : 0>(acc, da, db, scale_d);
+  else wgmma_m64n128k16<TA ? 1 : 0, TB ? 1 : 0>(acc, da, db, scale_d);
+}
+
+// Consumer tail shared by the GEMM kernels: the two consumer warpgroups (threads 0..255) stage their fp32 accumulators in
+// shared memory (rows [64 c, 64 c + 64) of a 128 x BLOCK_N tile) and run the fused epilogue on it.  Warp ew = 0..7 owns rows
+// 32 (ew & 3) .. + 31 (one per lane) and the column half ew >> 2.  Every consumer MMA must have completed before the call
+// (the staging tile overlaps the operand ring).
+template <int BLOCK_N>
+__device__ __forceinline__ void gemm_consumer_tail(const GemmParams& p, const float* acc, float* acc_s, int mb, int m0,
+                                                   int col_base, int n_valid, int m_valid) {
+  constexpr int kPitch = BLOCK_N + 8;
+  const int ew = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  named_bar_sync(1, 256);
+  acc_to_smem<BLOCK_N>(acc, acc_s, kPitch, 64 * (ew >> 2));
+  named_bar_sync(1, 256);
+  const int r = (ew & 3) * 32 + lane;
+  const EpiRow erow = make_epi_row(p, mb, static_cast<long long>(m0) + r);
+#pragma unroll 1
+  for (int c0 = (ew >> 2) * (BLOCK_N / 2); c0 < ((ew >> 2) + 1) * (BLOCK_N / 2); c0 += 32) {
+    if (c0 >= n_valid) break;  // warp-uniform
+    epilogue_chunk32(p, erow, acc_s + r * kPitch + c0, c0, n_valid, col_base, r < m_valid, lane);
+  }
+}
+
+// Output rows of an M tile that holds only padded frames (ragged batch): zeros, so that padded frames stay FINITE (a NaN in a
+// padded key row would survive the -inf mask as NaN * 0 in the probabilities x V product).  bf16 outputs only.
+__device__ __forceinline__ void zero_dead_tile(const GemmParams& p, int mb, int m0, int col_base, int n_valid) {
+  const int rows = min(p.m_tile_valid, p.m_rows - m0), c8 = n_valid / 8;
+  for (int i = threadIdx.x; i < rows * c8; i += blockDim.x) {
+    const long long row = static_cast<long long>(m0) + i / c8;
+    const int col = col_base + (i % c8) * 8;
+    *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(p.out.p) + mb * p.out.bs + row * p.out.ld + col) = make_uint4(0u, 0u, 0u, 0u);
+    if (p.out2.p != nullptr)
+      *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(p.out2.p) + mb * p.out2.bs + row * p.out2.ld + col) = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
+
 template <int BLOCK_N, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(192) gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                        const __grid_constant__ CUtensorMap tmB,
-                                                        const __grid_constant__ GemmParams p) {
+__global__ void __launch_bounds__(288, 2) gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                           const __grid_constant__ CUtensorMap tmB,
+                                                           const __grid_constant__ GemmParams p) {
   pdl_launch_dependents();
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int kStages = Cfg::kStages;
@@ -234,41 +268,49 @@ __global__ void __launch_bounds__(192) gemm_bf16_kernel(const __grid_constant__ 
   const int kb_begin = blockIdx.z * p.k_blocks_per_split;
   const int kb_end = min(kb_begin + p.k_blocks_per_split, p.k_blocks);
   if (kb_begin >= kb_end) return;  // uniform per CTA
+  const int col_base = n_tile * p.n_out_stride;
+  const int n_valid = min(p.n_tile_valid, p.n_total - col_base);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, still a __shared__ pointer (LDS/STS, not generic)
   __shared__ uint64_t full_bar[kStages];
   __shared__ uint64_t empty_bar[kStages];
-  __shared__ uint64_t tmem_full_bar;
-  __shared__ uint32_t tmem_base_smem;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
 #pragma unroll
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
     }
-    mbar_init(&tmem_full_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, BLOCK_N);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   pdl_wait();  // prologue overlapped the previous kernel's tail; global memory is touched only from here on
 
-  if (warp == 0) {
+  if (p.m_valid != nullptr && m0 >= p.m_valid[mb]) {
+    zero_dead_tile(p, mb, m0, col_base, n_valid);
+    return;
+  }
+  // ragged weight gradients: a 64-row K block at or beyond its batch's valid rows is neither loaded nor multiplied
+  auto kb_live = [&](int kb) {
+    if (p.k_valid == nullptr) return true;
+    const int kbatch = kb / p.k_blocks_per_batch;
+    return (kb - kbatch * p.k_blocks_per_batch) * 64 < p.k_valid[kbatch];
+  };
+
+  if (warp == 8) {
     if (lane == 0) {
       // ------------------------------------------------------------ TMA producer
       int v[kCoordVars];
       v[0] = 1; v[1] = m0; v[2] = mb; v[3] = n_tile;
       int it = 0;
-      for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
+      for (int kb = kb_begin; kb < kb_end; ++kb) {
+        if (!kb_live(kb)) continue;
         const int s = it % kStages;
         const uint32_t ph = (it / kStages) & 1;
+        ++it;
         mbar_wait(&empty_bar[s], ph ^ 1);
         if (p.k_blocks_per_batch > 0) {
           v[5] = kb / p.k_blocks_per_batch;
@@ -307,80 +349,58 @@ __global__ void __launch_bounds__(192) gemm_bf16_kernel(const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------------------------------------ MMA issuer
-      constexpr uint32_t idesc = make_idesc_bf16(128, BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0);
-      int it = 0;
-      for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
-        const int s = it % kStages;
-        const uint32_t ph = (it / kStages) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes);
-        const uint32_t sb = sa + Cfg::kABytes;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          // K-major: advance 16 elements (32 B) inside the 128B swizzle row; SBO = 8 rows * 128 B.
-          // MN-major: advance 16 K-rows (2048 B); LBO = stride between 64-wide MN atoms (8192 B), SBO = 1024 B.
-          const uint64_t da = A_MN ? make_smem_desc_sw128(sa + k * 2048, 8192, 1024)
-                                   : make_smem_desc_sw128(sa + k * 32, 16, 1024);
-          const uint64_t db = B_MN ? make_smem_desc_sw128(sb + k * 2048, 8192, 1024)
-                                   : make_smem_desc_sw128(sb + k * 32, 16, 1024);
-          umma_bf16(tmem_base, da, db, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[s]);  // frees the smem slot once these MMAs retire
-      }
-      umma_commit(&tmem_full_bar);
-    }
   } else {
-    // -------------------------------------------------------------- epilogue
-    const int q = warp & 3;             // TMEM lane quadrant this warp may access
-    const int r = q * 32 + lane;        // row inside the tile
-    const int m_valid = min(p.m_tile_valid, p.m_rows - m0);
-    const bool row_ok = r < m_valid;
-    const int col_base = n_tile * p.n_out_stride;
-    const int n_valid = min(p.n_tile_valid, p.n_total - col_base);
-    const long long row = static_cast<long long>(m0) + r;
-
-    const EpiRow erow = make_epi_row(p, mb, row);
-    mbar_wait(&tmem_full_bar, 0);
-    tc_fence_after();
-
-#pragma unroll 1
-    for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-      if (c0 >= n_valid) break;  // warp-uniform
-      epilogue_chunk32(p, erow, tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c0, c0, n_valid, col_base, row_ok, lane);
+    // -------------------------------------------------------------- consumers: warpgroup c owns rows 64 c .. 64 c + 63
+    const int c = warp >> 2;
+    float acc[BLOCK_N / 2];  // written by the first MMA (scale_d = 0)
+    int it = 0;
+    for (int kb = kb_begin; kb < kb_end; ++kb) {
+      if (!kb_live(kb)) continue;
+      const int s = it % kStages;
+      mbar_wait(&full_bar[s], (it / kStages) & 1);
+      // rows 64 c.. of A: 64 rows x 128 B (K-major) or the second 64-row MN block (MN-major) -- 8 KB either way
+      const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes) + c * 8192;
+      const uint32_t sb = smem_u32(smem + s * Cfg::kStageBytes + Cfg::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t da = A_MN ? make_smem_desc_sw128(sa + k * 2048, 8192, 1024) : make_smem_desc_sw128(sa + k * 32, 16, 1024);
+        const uint64_t db = B_MN ? make_smem_desc_sw128(sb + k * 2048, 8192, 1024) : make_smem_desc_sw128(sb + k * 32, 16, 1024);
+        wgmma_tile<BLOCK_N, A_MN, B_MN>(acc, da, db, (it > 0 || k > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous K block's MMAs have retired: its stage goes back to the producer
+      if (it > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
+      ++it;
     }
-  }
-
-  // teardown: everyone done with TMEM before the allocating warp frees it
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, BLOCK_N);
+    wgmma_wait<0>();
+    if (it == 0) {  // no live K block (ragged weight gradient): the split contributes zeros
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+    }
+    gemm_consumer_tail<BLOCK_N>(p, acc, reinterpret_cast<float*>(smem), mb, m0, col_base, n_valid,
+                                min(p.m_tile_valid, p.m_rows - m0));
   }
 }
 
 // ---------------------------------------------------------------------------------------------- pos_conv, windowed
 // Grouped Conv1d(k = taps, padding = taps/2) as an implicit GEMM whose A operand is loaded ONCE per tile: the 128 frames of a
 // tile need input rows m0 .. m0+127+taps-1 of the zero-padded activation, and tap j multiplies rows m0+j .. m0+j+127 -- the same
-// shared-memory tile, shifted by j rows.  One 256-row TMA box brings the window in; every tap is four tcgen05.mma whose A
-// descriptor starts j rows (j * 128 bytes) into the tile (the swizzle follows the absolute address, see the MMA loop).  Only the per-tap weight tile (8 KB) streams through the TMA ring, so the kernel
-// reads ~1/3 of the bytes of the box-per-tap formulation (which was bound by the L2 -> SM fabric).
-// grid (groups, m_tiles * batches); block 192 (TMA warp, MMA warp, 4 epilogue warps); fused tail = epilogue_chunk32.
+// shared-memory tile, shifted by j rows.  One 256-row TMA box brings the window in; every tap is four wgmma per consumer
+// warpgroup whose A descriptor starts j rows (j * 128 bytes) into the tile.  Only the per-tap weight tile (8 KB) streams through
+// the TMA ring, so the kernel reads ~1/3 of the bytes of the box-per-tap formulation.
+// grid (groups, m_tiles * batches); block 288 (two consumer warpgroups, TMA warp); fused tail = epilogue_chunk32.
 struct PosconvCfg {
   static constexpr int kStages = 6;
   static constexpr int kABytes = 256 * 128;  // 256 rows x 64 bf16
   static constexpr int kBBytes = 64 * 128;   // 64 output channels x 64 input channels of one tap
   static constexpr int kSmemBytes = kABytes + kStages * kBBytes + 1024;
-  static constexpr int kThreads = 192;
+  static constexpr int kThreads = 288;
 };
 
-__global__ void __launch_bounds__(192) posconv_window_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                             const __grid_constant__ CUtensorMap tmB,
-                                                             const __grid_constant__ GemmParams p, int taps, int cg) {
+__global__ void __launch_bounds__(288, 2) posconv_window_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                const __grid_constant__ CUtensorMap tmB,
+                                                                const __grid_constant__ GemmParams p, int taps, int cg) {
   pdl_launch_dependents();
   using Cfg = PosconvCfg;
   constexpr int kStages = Cfg::kStages;
@@ -394,29 +414,23 @@ __global__ void __launch_bounds__(192) posconv_window_kernel(const __grid_consta
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
   uint8_t* sB = smem + Cfg::kABytes;
-  __shared__ uint64_t a_full, full_bar[kStages], empty_bar[kStages], tmem_full_bar;
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ uint64_t a_full, full_bar[kStages], empty_bar[kStages];
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     mbar_init(&a_full, 1);
 #pragma unroll
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);
     }
-    mbar_init(&tmem_full_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, 64);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(&a_full, Cfg::kABytes);
       tma_load_4d(sA, &tmA, &a_full, g * cg, m0, mb, 0);  // rows m0 .. m0+255 of this group's channels (zero-filled past the end)
@@ -427,48 +441,26 @@ __global__ void __launch_bounds__(192) posconv_window_kernel(const __grid_consta
         tma_load_4d(sB + s * Cfg::kBBytes, &tmB, &full_bar[s], j * 64, g * 64, 0, 0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(128, 64, 0, 0);
-      mbar_wait(&a_full, 0);
-      for (int j = 0; j < taps; ++j) {
-        const int s = j % kStages;
-        mbar_wait(&full_bar[s], (j / kStages) & 1);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(sA) + j * 128;  // the window shifted by j rows
-        const uint32_t sb = smem_u32(sB + s * Cfg::kBBytes);
-        // base offset 0: measured on B200, the tensor core applies the 128-byte swizzle to the ABSOLUTE shared-memory address
-        // bits (as TMA does when it writes the tile), so a row-shifted start needs no correction (B200S_GEMM_DEBUG=8 sets the
-        // "(start >> 7) & 7" value the descriptor format documents for unaligned starts: it produces wrong results here)
-        const uint32_t bo = (p.debug & 8) ? static_cast<uint32_t>(j & 7) : 0u;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(tmem_base, make_smem_desc_sw128_bo(sa + k * 32, 16, 1024, bo), make_smem_desc_sw128(sb + k * 32, 16, 1024),
-                    idesc, (j > 0 || k > 0) ? 1u : 0u);
-        umma_commit(&empty_bar[s]);
-      }
-      umma_commit(&tmem_full_bar);
-    }
   } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    const int m_valid = min(128, p.m_rows - m0);
-    const bool row_ok = r < m_valid;
-    const int col_base = g * cg;
-    const EpiRow erow = make_epi_row(p, mb, static_cast<long long>(m0) + r);
-    mbar_wait(&tmem_full_bar, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c0 = 0; c0 < 64; c0 += 32) {
-      if (c0 >= cg) break;
-      epilogue_chunk32(p, erow, tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c0, c0, cg, col_base, row_ok, lane);
+    const int c = warp >> 2;
+    float acc[32];  // written by the first tap's MMAs (scale_d = 0)
+    mbar_wait(&a_full, 0);
+    for (int j = 0; j < taps; ++j) {
+      const int s = j % kStages;
+      mbar_wait(&full_bar[s], (j / kStages) & 1);
+      const uint32_t sa = smem_u32(sA) + (64 * c + j) * 128;  // this warpgroup's 64 rows of the window, shifted by j rows
+      const uint32_t sb = smem_u32(sB + s * Cfg::kBBytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_tile<64, false, false>(acc, make_smem_desc_sw128(sa + k * 32, 16, 1024), make_smem_desc_sw128(sb + k * 32, 16, 1024),
+                                     (j > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (j > 0 && lane == 0) mbar_arrive(&empty_bar[(j - 1) % kStages]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, 64);
+    wgmma_wait<0>();
+    gemm_consumer_tail<64>(p, acc, reinterpret_cast<float*>(smem), mb, m0, g * cg, cg, min(128, p.m_rows - m0));
   }
 }
 

@@ -1,4 +1,4 @@
-// Masked-prediction head of the WavLM / HuBERT-style pre-training loss (SURVEY.md section 8f row 1), fused around the tcgen05
+// Masked-prediction head of the WavLM / HuBERT-style pre-training loss (SURVEY.md section 8f row 1), fused around the wgmma
 // GEMMs of gemm.cu.  Reference: src/fairseq/models/wavlm/wavlm.py:525-576 (final_proj, compute_pred), :426-438 (compute_nce:
 // cosine similarity against the positive + every label embedding, / logit_temp, -inf where a negative equals the positive)
 // and src/fairseq/criterions/wavlm_criterion.py:63-87 (sum-reduced cross entropy with the positive at index 0).

@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), proxy fences.
-// Written for CUDA 12.9 / PTX ISA 8.8, target sm_100a only.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA), proxy fences, named barriers.
+// Written for CUDA 12.x / PTX ISA 8.x, target sm_90a only.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -59,11 +59,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+// barrier over `count` threads (a multiple of 32) of the CTA on hardware barrier `id` (0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -107,168 +105,76 @@ __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.
 // all bulk groups of this thread are complete (writes performed)
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---------------------------------------------------------------- TMEM alloc
-// Must be executed by one full warp. ncols: power of two >= 32.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor (SM100 format, cute/arch/mma_sm100_desc.hpp field layout):
-//   [0,14) start address >> 4, [16,30) leading byte offset >> 4, [32,46) stride byte offset >> 4,
-//   [46,48) version = 1, [61,64) layout type (2 = SWIZZLE_128B).
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
+// Shared-memory matrix descriptor (sm_90 format, cute/arch/mma_sm90_desc.hpp field layout):
+//   [0,14) start address >> 4, [16,30) leading byte offset >> 4, [32,46) stride byte offset >> 4, [62,64) layout (1 = SWIZZLE_128B).
+// K-major operand (rows of 64 bf16 = one 128-byte swizzle row): SBO = 1024 (8-row groups), LBO unused; the K step of 16
+// elements advances the start address by 32 bytes.  MN-major operand: LBO = stride between 64-wide MN blocks, SBO = 1024
+// (8 K-rows), the K step advances by 16 rows = 2048 bytes.  The swizzle is a function of the absolute shared-memory address
+// (as for the TMA writes), so a start address shifted by whole rows needs no base-offset correction.
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Same with the 3-bit base offset (bits [49,52)): needed when the matrix does not start on the 1024-byte repeat of the 128-byte
-// swizzle, e.g. a K-major tile read from row j of a larger TMA-written tile: base_offset = (start_address >> 7) & 7.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128_bo(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                            uint32_t base_offset) {
-  return make_smem_desc_sw128(smem_addr, lbo_bytes, sbo_bytes) | (static_cast<uint64_t>(base_offset & 7u) << 49);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// Instruction descriptor for kind::f16 with bf16 A/B, fp32 accumulate.
-//   c_format [4,6)=1 (F32); a_format [7,10)=1 (BF16); b_format [10,13)=1; a_major bit15; b_major bit16 (1 = MN-major);
-//   n_dim [17,23) = N>>3; m_dim [24,29) = M>>4.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands in shared memory, fp32 accumulators in registers; executed by all 128
+// threads of a warpgroup.  TA / TB: 0 = K-major, 1 = MN-major operand.  scale_d = 0 overwrites D.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB)
       : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
 }
 
-// ---------------------------------------------------------------- TMEM -> registers
-// 32 lanes x 32 consecutive fp32 columns; thread i of the warp gets lane (lane_base + i).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- CTA pair (cta_group::2) variants
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// executed by the same warp index in BOTH CTAs of the pair
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load into THIS CTA's shared memory whose completion bytes are signalled on the LEADER CTA's mbarrier (same smem offset;
-// clearing bit 24 of the shared::cluster address selects CTA rank 0 of the pair)
-__device__ __forceinline__ void tma_load_4d_2cta(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                 int c3) {
-  const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_leader), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// Same, multicast: the box is written at the same shared-memory offset of every CTA in `cta_mask`, and each destination
-// signals the full barrier at that offset of ITS OWN pair leader (the barrier address is CTA-relative, peer bit cleared).
-__device__ __forceinline__ void tma_load_4d_2cta_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                    int c3, uint16_t cta_mask) {
-  const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], "
-      "[%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_leader), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(cta_mask)
-      : "memory");
-}
-// D[tmem, both CTAs] (+)= A * B with M = 256 split over the pair; issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_bf16_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                               uint32_t accumulate) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB)
       : "memory");
 }
-// commit: arrive (once) on the mbarrier at the same smem offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
+
+
+// Accumulator fragment of a 64 x N wgmma (thread t of the warpgroup, warp w = t / 32, lane l):
+//   d[i] is row 16 w + l / 4 + 8 ((i / 2) & 1), column 8 (i / 4) + 2 (l & 3) + (i & 1).
+// Rows [row0, row0 + 64) of a row-major fp32 shared-memory tile (pitch in floats, even) <-> the fragment.
+template <int N>
+__device__ __forceinline__ void acc_to_smem(const float* d, float* tile, int pitch, int row0) {
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  float* base = tile + (row0 + 16 * w + (l >> 2)) * pitch + 2 * (l & 3);
+#pragma unroll
+  for (int i = 0; i < N / 2; i += 2)
+    *reinterpret_cast<float2*>(base + 8 * ((i >> 1) & 1) * pitch + 8 * (i >> 2)) = make_float2(d[i], d[i + 1]);
 }
-// arrive on the mbarrier at the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(rank)
-      : "memory");
-}
-// wait with cluster-scope acquire (pairs with remote arrives)
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0, done = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (!done && ++spins > (1u << 28)) __trap();
+template <int N>
+__device__ __forceinline__ void smem_to_acc(float* d, const float* tile, int pitch, int row0) {
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  const float* base = tile + (row0 + 16 * w + (l >> 2)) * pitch + 2 * (l & 3);
+#pragma unroll
+  for (int i = 0; i < N / 2; i += 2) {
+    const float2 v = *reinterpret_cast<const float2*>(base + 8 * ((i >> 1) & 1) * pitch + 8 * (i >> 2));
+    d[i] = v.x;
+    d[i + 1] = v.y;
   }
 }
 

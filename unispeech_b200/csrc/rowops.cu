@@ -764,10 +764,9 @@ static int dispatch_width(int D, F&& f) {
   }
 }
 
-// Which LayerNorm kernels run at the wide widths (512 / 768 / 1024).  Measured on B200 (tools/bench_rowops.py --norms, WavLM-Large
-// shapes, profiles/r02_microbench_norms.txt): the block-per-row-group kernels win only for the gate-fused forward (14.7 vs 17.5 us);
-// the plain forward ties (9.6 us) and the backward LOSES (21 vs 15-18 us; conv-stack shape 315 vs 230 us) -- one block barrier per
-// row group stalls all of a block's warps on the same loads, while 16 independent warp-per-row chains per SM overlap better.
+// Which LayerNorm kernels run at the wide widths (512 / 768 / 1024): the block-per-row-group kernels for the gate-fused forward only;
+// elsewhere the warp-per-row kernels -- one block barrier per row group stalls all of a block's warps on the same loads, while
+// independent warp-per-row chains overlap better (tools/bench_rowops.py --norms compares the two).
 // B200S_LN_WIDE=0 / 1 forces the warp-per-row / wide kernels everywhere (A/B runs).
 static int ln_wide_mode() {
   static int v = -1;

@@ -1,4 +1,4 @@
-// UniSpeech-SAT utterance-contrastive head (BASELINE config #4; SURVEY.md section 8f row 1, second half) around the tcgen05 GEMMs:
+// UniSpeech-SAT utterance-contrastive head (BASELINE config #4; SURVEY.md section 8f row 1, second half) around the wgmma GEMMs:
 //   src/fairseq/models/unispeech_sat/unispeech_sat.py:699-758 (forward tail / compute_pred_spk), :545-557 (compute_nce with
 //   replace_inf=False), :487-543 (sample_instances: index tensors drawn on the HOST with the reference's torch.randint call order),
 //   src/fairseq/modules/gumbel_vector_quantizer.py:141-201 (GumbelVectorQuantizer.forward, hard codes).

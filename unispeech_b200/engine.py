@@ -1,6 +1,6 @@
 """Host-side orchestration of the WavLM hot path over the C-ABI kernels (forward and backward).
 
-Everything numerical runs in the hand-written sm_100a kernels (`ops.*`); this file only owns buffers, parameter
+Everything numerical runs in the hand-written sm_90a kernels (`ops.*`); this file only owns buffers, parameter
 preparation, the order of launches and the autograd glue.  PyTorch is used for device memory and streams.
 
 Layouts

@@ -10,7 +10,7 @@
 Both keep the reference's freeze logic (`freeze_finetune_updates`: the encoder runs under no_grad until that many updates) and
 `apply_mask` (span masking only in training).  They are host glue around `unispeech_b200.wavlm.WavLM`: every tensor they return is a
 view of the kernels' output.  `final_dropout` and the output projection `proj` (CTC vocabulary / decoder width,
-hubert_asr.py:299-312,330-340) run on the same kernels as the encoder (`b200s_dropout_rows`, the tcgen05 GEMMs); `proj` keeps the
+hubert_asr.py:299-312,330-340) run on the same kernels as the encoder (`b200s_dropout_rows`, the wgmma GEMMs); `proj` keeps the
 reference's parameter names (`proj.weight [V, D]`, `proj.bias`) and initialiser (xavier_uniform / zeros, `Linear()` of
 hubert_asr.py:367-372).
 """
@@ -33,7 +33,7 @@ _SITE_FINAL = 0x7F000001  # dropout site of `final_dropout` (distinct from every
 
 class _OutputProjFn(torch.autograd.Function):
     """y = proj(final_dropout(x)):  x bf16 [R, D] (R = T*B rows, any order), W fp32 [V, D], b fp32 [V].  Forward: counter-based
-    dropout rows kernel + tcgen05 GEMM with the bias in its epilogue (the N dimension is padded to a multiple of 64 for the
+    dropout rows kernel + wgmma GEMM with the bias in its epilogue (the N dimension is padded to a multiple of 64 for the
     operand tiles, the padding columns are never returned).  Backward: column sum (bias), weight-gradient GEMM, input-gradient
     GEMM, the same dropout mask regenerated from its key."""
 

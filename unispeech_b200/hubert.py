@@ -22,7 +22,7 @@ class HubertConfig(WavLMPretrainConfig):
 
 class HubertModel(WavLMForPretraining):
     """`HubertModel.forward(source, target_list, padding_mask, mask, features_only, output_layer)` and the masked-prediction
-    criterion (src/fairseq/criterions/hubert_criterion.py has the same get_loss as wavlm_criterion.py) on the B200 kernels."""
+    criterion (src/fairseq/criterions/hubert_criterion.py has the same get_loss as wavlm_criterion.py) on the project's kernels."""
 
     def __init__(self, cfg: HubertConfig, num_classes: List[int]):
         if getattr(cfg, "relative_position_embedding", False) or getattr(cfg, "gru_rel_pos", False):

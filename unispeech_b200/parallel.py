@@ -39,12 +39,8 @@ def all_reduce_grads(flat: torch.Tensor, group=None) -> torch.Tensor:
 
 def configure_overlap(nccl_ctas: int = 0):
     """Optional knob for the overlapped exchange: bound NCCL to `nccl_ctas` CTAs (NCCL_MAX_CTAS, read when the communicator is created:
-    call this BEFORE `init_process_group`; an explicit setting in the environment wins) and make the persistent GEMM kernels leave
-    that many SMs free (`b200s_reserve_sms`), so that NCCL's CTAs never displace clusters of a grid sized for the whole chip.
-    Measured at N = 2 on B200 (WavLM-Large, profiles/r02_bench_*_n2*.json): no gain -- backward 23.9 -> 25.2 ms with 4 reserved SMs
-    against 23.2 -> 24.7 ms without, and the last bucket finishes later with four CTAs (0.97 vs 0.43 ms exposed) -- so the
-    slowdown of the overlapped backward pass is HBM / power contention rather than displaced clusters, and the default (0) leaves
-    NCCL alone.  Kept for larger node counts and other interconnects."""
+    call this BEFORE `init_process_group`; an explicit setting in the environment wins) and record that many SMs as reserved
+    (`b200s_reserve_sms`; the GEMMs launch one CTA per tile, so no grid is sized around them).  The default (0) leaves NCCL alone."""
     import os
     from . import ops
     if int(nccl_ctas) <= 0:

@@ -1,4 +1,4 @@
-"""Pre-training surface of the fairseq WavLM model: encoder + masked-prediction head + criterion on the B200 kernels.
+"""Pre-training surface of the fairseq WavLM model: encoder + masked-prediction head + criterion on the project's kernels.
 
 Mirrors (SURVEY.md section 8b B2 / 8f row 1):
   * `WavLMModel.forward(source, target_list, padding_mask, mask, features_only, output_layer)`
@@ -6,7 +6,7 @@ Mirrors (SURVEY.md section 8b B2 / 8f row 1):
   * `WavLMCriterion.get_loss`  -- src/fairseq/criterions/wavlm_criterion.py:52-138: sum-reduced cross entropy over the masked
     (x pred_masked_weight) and unmasked (x pred_nomask_weight) frames, `sample_size`, `features_pen` extra loss, accuracy counts.
 The reference materialises `[C+1, S, final_dim]` expanded targets and `[S, C+1]` logits per label set; here the logits are one
-tcgen05 GEMM against the row-normalised label embeddings and the softmax / cross entropy / backward operand come from one
+wgmma GEMM against the row-normalised label embeddings and the softmax / cross entropy / backward operand come from one
 row kernel (csrc/nce.cu), so the loss is a scalar produced on the device with no host synchronisation.
 """
 from __future__ import annotations

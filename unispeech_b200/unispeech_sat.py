@@ -1,6 +1,6 @@
 """UniSpeech-SAT pre-training model (BASELINE.json configs[3]): the WavLM-style encoder + masked-prediction head of
 `pretrain.WavLMForPretraining` plus the UTTERANCE-CONTRASTIVE loss on the output of an intermediate layer and the Gumbel vector
-quantizer of its targets, on the B200 kernels (csrc/sat.cu + the tcgen05 GEMMs).
+quantizer of its targets, on the project's kernels (csrc/sat.cu + the wgmma GEMMs).
 
 Mirrors src/fairseq/models/unispeech_sat/unispeech_sat.py: constructor tail :383-412 (state_dict keys `spk_proj.*`, `project_q.*`,
 `quantizer.vars`, `quantizer.weight_proj.*`, `encoder.layer_norm_for_extract.*`), `forward` :585-760 (result keys `loss_spk_m`,

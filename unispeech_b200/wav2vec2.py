@@ -7,7 +7,7 @@ MASKED frames, quantised and projected; negatives drawn from them; x = `final_pr
 `sample_negatives` :474-531 (host `torch.randint`, same calls in the same order), `compute_preds` :533-553 (cosine logits / temp,
 a negative that equals the positive gets -inf), `get_extra_losses` :752-767, and `Wav2vecCriterion.get_loss` with `infonce`
 (src/fairseq/criterions/wav2vec_criterion.py:44-118).
-Kernels: `b200s_gather_rows`, tcgen05 GEMMs (final_proj, quantizer logits, project_q), `b200s_vq_hard` (eval arg-max / training
+Kernels: `b200s_gather_rows`, wgmma GEMMs (final_proj, quantizer logits, project_q), `b200s_vq_hard` (eval arg-max / training
 Gumbel hard sample with the counter-based noise), `b200s_w2v_nce_fwd` (logits + -inf masking + cross entropy + accuracy in one pass;
 nothing of size [N+1, S, Dp] exists), `b200s_sat_nce_bwd`, `b200s_vq_logits_bwd`, `b200s_vq_dvars`.  The gradient of the quantizer
 branch reaches the conv stack through the LayerNorm output (`_ProjFn`'s third output).

@@ -1,4 +1,4 @@
-"""B200-native WavLM / UniSpeech-SAT encoder with the reference's public surface.
+"""H100 (sm_90a) WavLM / UniSpeech-SAT encoder with the reference's public surface.
 
 Mirrors (names, arguments, return values, module tree and state_dict keys):
   * `WavLMConfig`, `WavLM.extract_features(source, padding_mask, mask, ret_conv, output_layer, ret_layer_results)`
@@ -7,7 +7,7 @@ Mirrors (names, arguments, return values, module tree and state_dict keys):
     returning `(x[B,T,C], layer_results)` -- the contract downstream heads hook (SURVEY.md section 8b, B3)
   * `WavLM.forward(source, padding_mask, mask, features_only, output_layer)` returning the fairseq-style dict
     (`x`, `padding_mask`, `features`, `layer_results`) -- src/fairseq/models/wavlm/wavlm.py:465-597 (encoder part).
-The numerical work is done by hand-written sm_100a kernels through the C ABI (`engine.py`, `ops.py`); these modules only hold
+The numerical work is done by hand-written sm_90a kernels through the C ABI (`engine.py`, `ops.py`); these modules only hold
 the fp32 master parameters (so released checkpoints load with `load_state_dict`) and sequence the launches.
 There is no CPU / PyTorch fallback: calling the model on a non-CUDA tensor raises.
 """
@@ -488,7 +488,7 @@ class WavLM(nn.Module):
         super().__init__()
         bad = _check_supported(cfg)
         if bad:
-            raise NotImplementedError("unsupported configuration for the B200 hot path: " + "; ".join(bad))
+            raise NotImplementedError("unsupported configuration for the CUDA hot path: " + "; ".join(bad))
         self.cfg = cfg
         self.conv_cfg = eval(cfg.conv_feature_layers)
         self.embed = self.conv_cfg[-1][0]
@@ -524,7 +524,7 @@ class WavLM(nn.Module):
     # ---- engine plumbing
     def _engine_for(self, device) -> Engine:
         if device.type != "cuda":
-            raise RuntimeError("unispeech_b200 runs on a B200 (sm_100) only: there is no CPU fallback for the hot path")
+            raise RuntimeError("unispeech_b200 runs on an H100 (sm_90) only: there is no CPU fallback for the hot path")
         if self._engine is None:
             self._engine = Engine(self)
         self._engine._ensure_device(device)
@@ -532,7 +532,7 @@ class WavLM(nn.Module):
 
     def _begin(self, device) -> Engine:
         if device.type != "cuda":
-            raise RuntimeError("the B200 hot path runs on a CUDA device (there is no CPU fallback)")
+            raise RuntimeError("the hot path runs on a CUDA device (there is no CPU fallback)")
         if device.index is not None and device.index != torch.cuda.current_device():
             # kernels are launched on the CURRENT device's current stream (_lib.stream_ptr)
             raise RuntimeError(f"make cuda:{device.index} the current device (torch.cuda.set_device) before calling the model")
