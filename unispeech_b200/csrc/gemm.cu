@@ -213,25 +213,46 @@ static int gemm_rows_impl(const void* a, long long a_bs, long long a_rs, int row
   memset(&p, 0, sizeof(p));
   fill_epilogue(p, epi);
   p.out = {out, out_bs, out_ld};
-  const int block_n = (N >= 128) ? 128 : 64;
-  ViewSpec vb{w, {K, N, 1, 1}, {K, 0, 0}, {64, block_n, 1, 1}};
-  if (make_tmap(&tb, vb)) return -3;
-
   p.m_rows = rows;
   p.m_tile_stride = 128;
   p.m_tile_valid = 128;
   p.m_tiles_per_batch = ceil_div(rows, 128);
+  p.m_tiles = p.m_tiles_per_batch * batches;
   p.n_total = N;
+  p.k_blocks = K / 64;
+  // ragged batch: tiles beyond a batch's valid rows are zero-filled instead of computed
+  p.m_valid = m_valid;
+
+  if (N >= 256 && m_valid == nullptr) {
+    // persistent 128 x 256 kernel.  Narrower outputs keep the 128 x 64 / 128 x 128 tiles, which compute no padded columns;
+    // ragged batches keep them too: their dead tiles end a CTA at once and the hardware hands its SM the next live tile, which
+    // a static persistent walk cannot match (measured ~1 ms per WavLM-Large ragged step slower even with live tiles first)
+    ViewSpec vb{w, {K, N, 1, 1}, {K, 0, 0}, {64, 256, 1, 1}};
+    if (make_tmap(&tb, vb)) return -3;
+    static std::once_flag once;
+    static cudaError_t attr_err = cudaSuccess;
+    std::call_once(once, [] {
+      attr_err = cudaFuncSetAttribute(gemm_ws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WsCfg::kSmemBytes);
+    });
+    B200_CHECK_CUDA(attr_err);
+    const int tiles = p.m_tiles * ceil_div(N, 256);
+    B200_CHECK_CUDA(launch_pdl(gemm_ws_kernel, dim3(std::min(tiles, sm_count())), dim3(WsCfg::kThreads), WsCfg::kSmemBytes, st,
+                               ta, tb, p));
+    B200_CHECK_LAUNCH();
+    return 0;
+  }
+
+  const int block_n = (N >= 128) ? 128 : 64;
+  ViewSpec vb{w, {K, N, 1, 1}, {K, 0, 0}, {64, block_n, 1, 1}};
+  if (make_tmap(&tb, vb)) return -3;
+
   p.n_out_stride = block_n;
   p.n_tile_valid = block_n;
-  p.k_blocks = K / 64;
   p.k_blocks_per_batch = 0;
   p.k_blocks_per_split = p.k_blocks;
   // A coords: (k0, m0, mb, 0)   B coords: (k0, n_tile*block_n, 0, 0)
   p.ca[0][4] = 1; p.ca[1][1] = 1; p.ca[2][2] = 1;
   p.cb[0][4] = 1; p.cb[1][3] = block_n;
-  // ragged batch: tiles beyond a batch's valid rows are zero-filled instead of computed
-  p.m_valid = m_valid;
   dim3 grid(ceil_div(N, block_n), p.m_tiles_per_batch * batches, 1);
   B200_CHECK_ARG(grid.y <= 65535, "gemm_rows: too many M tiles (%u)", grid.y);
   return block_n == 128 ? launch_gemm<128, false, false>(ta, tb, p, grid, st)

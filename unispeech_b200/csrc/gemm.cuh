@@ -10,6 +10,7 @@
 // weight-gradient GEMMs), selected per operand.  All the "view" tricks of the WavLM path (strided
 // Conv1d as an overlapping-row view, grouped pos_conv taps, per-batch tiles) are expressed on the host
 // as <=4-D TMA tensor maps plus a small integer matrix that maps tile indices to TMA coordinates.
+// Row GEMMs (K-major, bf16 out) with N >= 256 run the persistent 128 x 256 gemm_ws_kernel further down instead.
 #pragma once
 #include "ptx.cuh"
 
@@ -40,6 +41,7 @@ struct GemmParams {
   int m_tiles_per_batch; // ceil over m_tile_stride
   int m_tile_stride;     // rows between consecutive M tiles (128 normally)
   int m_tile_valid;      // max valid rows per tile (128 normally; Cg for grouped wgrad)
+  int m_tiles;           // M tiles over all batches (persistent kernel)
   int n_total;           // valid output columns
   int n_out_stride;      // output column stride per N tile
   int n_tile_valid;      // max valid columns per tile
@@ -380,6 +382,212 @@ __global__ void __launch_bounds__(288, 2) gemm_bf16_kernel(const __grid_constant
     }
     gemm_consumer_tail<BLOCK_N>(p, acc, reinterpret_cast<float*>(smem), mb, m0, col_base, n_valid,
                                 min(p.m_tile_valid, p.m_rows - m0));
+  }
+}
+
+// ------------------------------------------------------------------------------- persistent 128 x 256 row GEMM
+// D[M, N] = A[M, K] * B[N, K]^T with K-major operands and a bf16 output (b200s_gemm_rows: the layer, conv and projection GEMMs).
+// One CTA per SM walks the 128 x 256 output tiles with N fastest inside a 128-row band, so the CTAs resident at any time share
+// their A bands in L2 and A is read from HBM about once.  Warp roles:
+//   warpgroup 0    : TMA producer (one elected lane); it hands its registers to the consumers
+//   warpgroups 1-2 : consumers, 64 rows of the tile each (wgmma m64n256k16, 128 fp32 accumulators per thread)
+// The producer runs ahead into the next tile while the consumers run the epilogue, so the operand ring is never epilogue staging:
+// each consumer warpgroup moves 64 accumulator columns at a time into its own 16 KB buffer and applies the fused epilogue
+// (epilogue_chunk32's semantics, bf16 output) row-wise, 16 lanes per 64-column row segment, so every global load and store of a
+// warp covers two whole 128-byte lines.
+// The epilogue's bf16 inputs (GELU' aux, residuals) are fetched with per-thread asynchronous copies into a per-warpgroup buffer
+// one 64-column chunk ahead -- chunk 0 while the tile's main loop runs -- so their latency is never paid row by row.
+struct WsCfg {
+  static constexpr int kStages = 3;
+  static constexpr int kABytes = 128 * 128;  // 128 rows x 64 bf16
+  static constexpr int kBBytes = 256 * 128;  // 256 rows x 64 bf16
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kEpiBytes = 64 * 64 * 4;  // one consumer warpgroup's 64 x 64 fp32 staging chunk
+  static constexpr int kPfBytes = 3 * 8 * 128 * 8;  // one consumer warpgroup's prefetched inputs: {aux, res1, res2} x 8 rows x 128 threads x 4 bf16
+  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kEpiBytes + 2 * kPfBytes + 1024;
+  static constexpr int kThreads = 384;
+  static_assert(kSmemBytes + 1024 <= 232448, "one CTA per SM");
+};
+
+__device__ __forceinline__ void add_bf16x4(float* v, uint2 w) {
+  const float2 f0 = unpack_bf16x2(w.x), f1 = unpack_bf16x2(w.y);
+  v[0] += f0.x; v[1] += f0.y; v[2] += f1.x; v[3] += f1.y;
+}
+__device__ __forceinline__ uint2 pack_bf16x4(const float* v) { return make_uint2(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3])); }
+
+__global__ void __launch_bounds__(384, 1) gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                         const __grid_constant__ CUtensorMap tmB,
+                                                         const __grid_constant__ GemmParams p) {
+  pdl_launch_dependents();
+  using Cfg = WsCfg;
+  constexpr int kStages = Cfg::kStages;
+  const int wg = threadIdx.x >> 7;
+  const int lane = threadIdx.x & 31;
+  const int n_tiles = (p.n_total + 255) / 256;
+  const int num_tiles = p.m_tiles * n_tiles;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  __shared__ uint64_t full_bar[kStages];
+  __shared__ uint64_t empty_bar[kStages];
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+#pragma unroll
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (wg == 0) {
+    // ------------------------------------------------------------ TMA producer
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int mt = tile / n_tiles, n_tile = tile - mt * n_tiles;
+        const int mb = mt / p.m_tiles_per_batch, m0 = (mt - mb * p.m_tiles_per_batch) * 128;
+        for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
+          const int s = it % kStages;
+          mbar_wait(&empty_bar[s], ((it / kStages) & 1) ^ 1);
+          uint8_t* sa = smem + s * Cfg::kStageBytes;
+          mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
+          tma_load_4d(sa, &tmA, &full_bar[s], kb * 64, m0, mb, 0);
+          tma_load_4d(sa + Cfg::kABytes, &tmB, &full_bar[s], kb * 64, n_tile * 256, 0, 0);
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------- consumers: warpgroup c owns rows 64 c .. 64 c + 63
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;
+  const int t = threadIdx.x & 127, w = t >> 5;
+  float* stage = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes + c * Cfg::kEpiBytes);
+  uint2* pf = reinterpret_cast<uint2*>(smem + kStages * Cfg::kStageBytes + 2 * Cfg::kEpiBytes + c * Cfg::kPfBytes);
+  const int cq = 4 * (lane & 15);  // epilogue: this lane's 4 columns of a 64-column chunk
+  const EpiTensor* const pf_src[3] = {&p.aux, &p.res1, &p.res2};
+  float acc[128];                  // written by each tile's first MMA (scale_d = 0)
+  int it = 0;
+  for (int tile = blockIdx.x; tile < p.m_tiles * n_tiles; tile += gridDim.x) {
+    const int mt = tile / n_tiles, n_tile = tile - mt * n_tiles;
+    const int mb = mt / p.m_tiles_per_batch, m0 = (mt - mb * p.m_tiles_per_batch) * 128;
+    const int col_base = n_tile * 256;
+    const int n_valid = min(256, p.n_total - col_base);
+    const int rows_here = min(128, p.m_rows - m0) - 64 * c;  // valid rows of this warpgroup's half (may be <= 0)
+    // the 4 columns x 8 rows of chunk j's epilogue inputs that this thread reads are copied into its own slots pf[(q, i), t]
+    auto prefetch = [&](int j) {
+      const int cl = 64 * j + cq;
+      if (cl < n_valid) {
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+          const EpiTensor& e = *pf_src[q];
+          if (e.p == nullptr) continue;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int r = 16 * w + 2 * i + (lane >> 4);
+            if (r < rows_here)
+              cp_async_8(pf + (q * 8 + i) * 128 + t, static_cast<const __nv_bfloat16*>(e.p) + mb * e.bs +
+                                                         (static_cast<long long>(m0) + 64 * c + r) * e.ld + col_base + cl);
+          }
+        }
+      }
+      cp_async_commit();
+    };
+    prefetch(0);
+    for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
+      const int s = it % kStages;
+      mbar_wait(&full_bar[s], (it / kStages) & 1);
+      const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes) + c * 8192;  // rows 64 c .. of A: 64 rows x 128 B
+      const uint32_t sb = smem_u32(smem + s * Cfg::kStageBytes + Cfg::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n256k16<0, 0>(acc, make_smem_desc_sw128(sa + k * 32, 16, 1024), make_smem_desc_sw128(sb + k * 32, 16, 1024),
+                               (kb > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous K block's MMAs have retired: its stage goes back to the producer
+      if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
+    }
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
+
+    // ---- epilogue, 64 columns at a time.  The staging chunk is XOR-swizzled (column ^ 8 (row & 3)) so that both the fragment
+    // stores and the row-segment loads are free of bank conflicts.
+    const int flags = p.flags;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (64 * j >= n_valid) break;  // warpgroup-uniform
+      named_bar_sync(1 + c, 128);    // the previous chunk has been read out of the staging buffer
+#pragma unroll
+      for (int i = 32 * j; i < 32 * j + 32; i += 2) {
+        const int r = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);
+        const int cc = 8 * ((i >> 2) - 8 * j) + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(stage + r * 64 + (cc ^ ((r & 3) << 3))) = make_float2(acc[i], acc[i + 1]);
+      }
+      const int cl = 64 * j + cq;
+      const bool col_ok = cl < n_valid;
+      const int col = col_base + cl;
+      named_bar_sync(1 + c, 128);
+      float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (p.bias != nullptr && col_ok) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
+      float cs[4] = {0.f, 0.f, 0.f, 0.f};
+      cp_async_wait_all();  // this thread's inputs of chunk j have landed
+#pragma unroll 4
+      for (int i = 0; i < 8; ++i) {
+        const int r = 16 * w + 2 * i + (lane >> 4);
+        const float4 v4 = *reinterpret_cast<const float4*>(stage + r * 64 + (cq ^ ((r & 3) << 3)));
+        if (!col_ok || r >= rows_here) continue;
+        float v[4] = {v4.x + b4.x, v4.y + b4.y, v4.z + b4.z, v4.w + b4.w};
+        const long long row = static_cast<long long>(m0) + 64 * c + r;
+        if (flags & EPI_GELU) {
+          __nv_bfloat16* o2 =
+              p.out2.p ? static_cast<__nv_bfloat16*>(p.out2.p) + mb * p.out2.bs + row * p.out2.ld + col : nullptr;
+          if (flags & EPI_GELU_STORE_GRAD) {
+            float g[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) v[k] = gelu_with_grad_f(v[k], g[k]);
+            if (o2 != nullptr) *reinterpret_cast<uint2*>(o2) = pack_bf16x4(g);
+          } else {
+            if (o2 != nullptr) *reinterpret_cast<uint2*>(o2) = pack_bf16x4(v);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) v[k] = gelu_f(v[k]);
+          }
+        }
+        if (flags & EPI_DGELU) {
+          const uint2 a = pf[(0 * 8 + i) * 128 + t];
+          const float2 f0 = unpack_bf16x2(a.x), f1 = unpack_bf16x2(a.y);
+          const float f[4] = {f0.x, f0.y, f1.x, f1.y};
+#pragma unroll
+          for (int k = 0; k < 4; ++k) v[k] *= (flags & EPI_AUX_IS_GRAD) ? f[k] : gelu_grad_f(f[k]);
+        }
+        if (p.res1.p != nullptr) add_bf16x4(v, pf[(1 * 8 + i) * 128 + t]);
+        if (p.res2.p != nullptr) add_bf16x4(v, pf[(2 * 8 + i) * 128 + t]);
+        *reinterpret_cast<uint2*>(static_cast<__nv_bfloat16*>(p.out.p) + mb * p.out.bs + row * p.out.ld + col) = pack_bf16x4(v);
+        if (flags & EPI_COLSUM) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) cs[k] += __bfloat162float(__float2bfloat16_rn(v[k]));
+        }
+      }
+      if (j < 3) prefetch(j + 1);  // this thread's slots have been read
+      if (flags & EPI_COLSUM) {
+        // column sums of the stored values over this warpgroup's 64 rows: lane pairs, then the 4 warps through the staging
+        // buffer, then one atomic per column
+#pragma unroll
+        for (int k = 0; k < 4; ++k) cs[k] += __shfl_xor_sync(0xffffffffu, cs[k], 16);
+        named_bar_sync(1 + c, 128);  // the chunk has been read: the buffer is free
+        if (lane < 16) *reinterpret_cast<float4*>(stage + w * 64 + cq) = make_float4(cs[0], cs[1], cs[2], cs[3]);
+        named_bar_sync(1 + c, 128);
+        if (t < 64 && 64 * j + t < n_valid)
+          atomicAdd(p.colsum + col_base + 64 * j + t, stage[t] + stage[64 + t] + stage[128 + t] + stage[192 + t]);
+      }
+    }
   }
 }
 
