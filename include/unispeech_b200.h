@@ -66,7 +66,8 @@ int b200s_gemm_rows(const void* a, long long a_bs, long long a_rs, int rows, int
 
 /* dW[n, k] (+=) sum_{b,r} Y[b,r,n] * X[b,r,k]   (fp32, row stride dw_ld): the weight gradient of the GEMMs above
  * (autograd of nn.Linear / nn.Conv1d).  Both operands are read MN-major by wgmma; X rows may overlap
- * (conv im2col view).  Split-K over (batch, row) blocks.  N % 8 == 0, K % 8 == 0. */
+ * (conv im2col view).  The reduction over (batch, 64-row) blocks is split across CTAs and summed with fp32 atomics (K >= 256:
+ * stream-K over 128 x 256 tiles; narrower: split-K over 128 x 64 tiles).  N % 8 == 0, K % 8 == 0. */
 int b200s_gemm_wgrad(const void* y, long long y_bs, long long y_rs, const void* x, long long x_bs,
                      long long x_rs, int rows, int batches, int N, int K, float* dw, long long dw_ld,
                      b200s_stream stream);

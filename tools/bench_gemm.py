@@ -2,9 +2,10 @@
 
     python tools/bench_gemm.py [--reps 20] [--only NAME] [--large]
 Default: the shapes of the WavLM-Base 16 x 15 s step.  --large: every b200s_gemm_rows call of one WavLM-Large 8 x 20 s training
-step (pre-LN encoder, conv stack in layer_norm mode), each with the epilogue the engine passes, then the layer weight gradients.
+step (pre-LN encoder, conv stack in layer_norm mode), each with the epilogue the engine passes, then every b200s_gemm_wgrad call of
+the same step with the views the engine passes.
 Prints one line per shape: time, algorithmic TFLOP/s, fraction of the bf16 peak and, for --large, the shape's FLOP-weighted share
-of the gemm_rows family in one step.  Each --large shape is checked once against an fp32 torch reference.
+of its family in one step.  Each --large shape is checked once against an fp32 torch reference.
 """
 import argparse
 import json
@@ -83,6 +84,73 @@ def large_rows_cases():
             n_u = (Ts[i - 1] - rho + s - 1) // s
             cases.append((f"conv{i}_dgrad_p{rho}", 1, n_u, B, nm * C, C, C, Tg * C, s * C, Tp[i - 1] * C, rho * C, ()))
     return cases
+
+
+def large_wgrad_cases():
+    """(name, calls per step, rows, batches, N, K, y_rs, y_bs, y_off, x_rs, x_bs) of every b200s_gemm_wgrad call of one WavLM-Large
+    8 x 20 s step, with the views the engine passes: the layer GEMMs over all B*T frames, conv1-6 per utterance with X read through
+    the overlapping-row view (row stride s*C) and dY from the lead-row gradient buffer, post_extract_proj per utterance."""
+    B, T, D, Fd, C, layers = 8, 999, 1024, 4096, 512, 24
+    M = B * T
+    cases = [
+        ("qkv", layers, M, 1, 3 * D, D, 3 * D, 0, 0, D, 0),
+        ("out_proj", layers, M, 1, D, D, D, 0, 0, D, 0),
+        ("fc1", layers, M, 1, Fd, D, Fd, 0, 0, D, 0),
+        ("fc2", layers, M, 1, D, Fd, D, 0, 0, Fd, 0),
+        ("post_extract_proj", 1, T, B, D, C, D, T * D, 0, C, T * C),
+    ]
+    convs = [(C, 10, 5)] + [(C, 3, 2)] * 4 + [(C, 2, 2)] * 2
+    Ts, t = [], 20 * 16000
+    for (_, k, s) in convs:
+        t = (t - k) // s + 1
+        Ts.append(t)
+    Tp = [_even(t) for t in Ts]
+    for i in range(1, len(convs)):
+        _, k, s = convs[i]
+        lead = (k + s - 1) // s - 1
+        Tg = _even((Ts[i - 1] + s - 1) // s + lead + 1)
+        cases.append((f"conv{i}", 1, Ts[i], B, C, k * C, C, Tg * C, lead * C, s * C, Tp[i - 1] * C))
+    return cases
+
+
+def run_large_wgrad(args, dev, peak):
+    cases = large_wgrad_cases()
+    total = sum(n * 2.0 * rows * b * N * K for (_, n, rows, b, N, K, *_r) in cases)
+    print(f"gemm_wgrad family, one WavLM-Large 8 x 20 s step: {total / 1e12:.2f} TFLOP")
+    print(f"{'case':18s} {'calls':>5s} {'rows':>7s} {'N':>5s} {'K':>5s} {'ms':>8s} {'TFLOP/s':>8s} {'frac':>6s} {'share':>6s} "
+          f"{'rel_err':>8s}")
+    fam_ms = 0.0
+    for name, n, rows, b, N, K, y_rs, y_bs, y_off, x_rs, x_bs in cases:
+        if args.only and name not in args.only.split(','):
+            continue
+        torch.manual_seed(0)
+        y_elems = y_off + ((b - 1) * y_bs if b > 1 else 0) + (rows - 1) * y_rs + N
+        x_elems = ((b - 1) * x_bs if b > 1 else 0) + (rows - 1) * x_rs + K
+        y = torch.randn(y_elems, device=dev).to(BF)
+        x = torch.randn(x_elems, device=dev).to(BF)
+        yv = y[y_off:]
+        dw = torch.zeros(N, K, device=dev)
+        fn = lambda: ops.gemm_wgrad(yv, y_bs, y_rs, x, x_bs, x_rs, rows, b, N, K, dw, K)  # noqa: E731
+        # one checked call (onto zeros), then the timed ones (accumulating)
+        fn()
+        torch.cuda.synchronize()
+        ref = torch.zeros(N, K, device=dev)
+        for bb in range(b):
+            ref += y.as_strided((rows, N), (y_rs, 1), y_off + bb * y_bs).float().t() @ \
+                x.as_strided((rows, K), (x_rs, 1), bb * x_bs).float()
+        err = ((dw - ref).abs().max() / ref.abs().max()).item()
+        del ref
+        ms = timeit(fn, args.reps)
+        flops = 2.0 * rows * b * N * K
+        tf = flops / (ms * 1e-3) / 1e12
+        fam_ms += n * ms
+        print(f"{name:18s} {n:5d} {rows * b:7d} {N:5d} {K:5d} {ms:8.4f} {tf:8.1f} {tf / peak:6.3f} {n * flops / total:6.3f} "
+              f"{err:8.1e}", flush=True)
+        del y, x, yv, dw
+        torch.cuda.empty_cache()
+    if not args.only:
+        print(f"family: {fam_ms:.2f} ms per step, {total / (fam_ms * 1e-3) / 1e12:.1f} TFLOP/s "
+              f"({total / (fam_ms * 1e-3) / 1e12 / peak:.3f} of peak)")
 
 
 def run_large_rows(args, dev, peak):
@@ -182,10 +250,8 @@ def main():
         cases.append((name + "_wgrad", "convw", T_out, 16, k * 512, 512))
     if args.large:
         run_large_rows(args, dev, peak)
-        M = 8 * 999
-        cases = []
-        for name, N, K in (("wgrad_qkv", 3072, 1024), ("wgrad_o", 1024, 1024), ("wgrad_fc1", 4096, 1024), ("wgrad_fc2", 1024, 4096)):
-            cases.append((name, "wgrad", M, 1, K, N))
+        run_large_wgrad(args, dev, peak)
+        return
     print(f"{'case':14s} {'ms':>8s} {'TFLOP/s':>9s} {'frac':>6s}")
     for name, kind, rows, batches, K, N in cases:
         if args.only and name not in args.only.split(','):

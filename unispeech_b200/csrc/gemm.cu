@@ -282,7 +282,7 @@ static int gemm_wgrad_impl(const void* y, long long y_bs, long long y_rs, const 
   B200_CHECK_ARG(y && x && dw, "gemm_wgrad: null pointer");
   B200_CHECK_ARG(rows > 0 && batches > 0 && K > 0 && N > 0, "gemm_wgrad: bad sizes");
   B200_CHECK_ARG(N % 8 == 0 && K % 8 == 0, "gemm_wgrad: N=%d, K=%d must be multiples of 8", N, K);
-  const int block_n = (K >= 128) ? 128 : 64;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
 
   CUtensorMap ta, tb;
   ViewSpec va{y, {N, rows, batches, 1}, {y_rs, batches > 1 ? y_bs : 0, 0}, {64, 64, 1, 1}};
@@ -297,10 +297,33 @@ static int gemm_wgrad_impl(const void* y, long long y_bs, long long y_rs, const 
   p.m_tile_valid = 128;
   p.m_tiles_per_batch = ceil_div(N, 128);
   p.n_total = K;
-  p.n_out_stride = block_n;
-  p.n_tile_valid = block_n;
   p.k_blocks_per_batch = ceil_div(rows, 64);
   p.k_blocks = p.k_blocks_per_batch * batches;
+  p.flags = EPI_OUT_F32 | EPI_ATOMIC;
+  fill_epilogue(p, nullptr);
+  p.out = {dw, 0, dw_ld};
+  // ragged batch: row blocks beyond a batch's valid rows are neither loaded nor multiplied
+  p.k_valid = k_valid;
+
+  if (K >= 256) {
+    // persistent 128 x 256 stream-K kernel.  Narrower outputs keep the 128 x 64 tiles, which compute no padded columns.
+    p.m_tiles = p.m_tiles_per_batch;
+    static std::once_flag once;
+    static cudaError_t attr_err = cudaSuccess;
+    std::call_once(once, [] {
+      attr_err = cudaFuncSetAttribute(gemm_ws_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WsCfg::kSmemBytes);
+    });
+    B200_CHECK_CUDA(attr_err);
+    const long long work = static_cast<long long>(p.m_tiles) * ceil_div(K, 256) * p.k_blocks;
+    B200_CHECK_CUDA(launch_pdl(gemm_ws_wgrad_kernel, dim3(static_cast<unsigned>(std::min<long long>(work, sm_count()))),
+                               dim3(WsCfg::kThreads), WsCfg::kSmemBytes, st, ta, tb, p));
+    B200_CHECK_LAUNCH();
+    return 0;
+  }
+
+  const int block_n = 64;
+  p.n_out_stride = block_n;
+  p.n_tile_valid = block_n;
   const int tiles = p.m_tiles_per_batch * ceil_div(K, block_n);
   int splits = ceil_div(2 * sm_count(), tiles);
   if (splits > p.k_blocks) splits = p.k_blocks;
@@ -310,15 +333,8 @@ static int gemm_wgrad_impl(const void* y, long long y_bs, long long y_rs, const 
   // A coords: (m0 + sub, k0, kbatch, 0)   B coords: (n_tile*block_n + sub, k0, kbatch, 0)
   p.ca[0][1] = 1; p.ca[0][7] = 1; p.ca[1][4] = 1; p.ca[2][5] = 1;
   p.cb[0][3] = block_n; p.cb[0][7] = 1; p.cb[1][4] = 1; p.cb[2][5] = 1;
-  p.flags = EPI_OUT_F32 | EPI_ATOMIC;
-  fill_epilogue(p, nullptr);
-  p.out = {dw, 0, dw_ld};
-  // ragged batch: row blocks beyond a batch's valid rows are neither loaded nor multiplied
-  p.k_valid = k_valid;
   dim3 grid(ceil_div(K, block_n), p.m_tiles_per_batch, splits);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return block_n == 128 ? launch_gemm<128, true, true>(ta, tb, p, grid, st)
-                        : launch_gemm<64, true, true>(ta, tb, p, grid, st);
+  return launch_gemm<64, true, true>(ta, tb, p, grid, st);
 }
 
 int b200s_gemm_wgrad(const void* y, long long y_bs, long long y_rs, const void* x, long long x_bs, long long x_rs,

@@ -10,7 +10,8 @@
 // weight-gradient GEMMs), selected per operand.  All the "view" tricks of the WavLM path (strided
 // Conv1d as an overlapping-row view, grouped pos_conv taps, per-batch tiles) are expressed on the host
 // as <=4-D TMA tensor maps plus a small integer matrix that maps tile indices to TMA coordinates.
-// Row GEMMs (K-major, bf16 out) with N >= 256 run the persistent 128 x 256 gemm_ws_kernel further down instead.
+// Row GEMMs (K-major, bf16 out) with N >= 256 run the persistent 128 x 256 gemm_ws_kernel further down instead, and weight
+// gradients with K >= 256 its stream-K sibling gemm_ws_wgrad_kernel.
 #pragma once
 #include "ptx.cuh"
 
@@ -179,11 +180,8 @@ __device__ __forceinline__ void epilogue_chunk32(const GemmParams& p, const EpiR
         float* o = e.out_f32 + col;
         if (flags & EPI_ATOMIC) {
           // 128-bit vector reductions (REDG.E.ADD.F32x4): the split-K epilogue is bound by LSU issue, not bytes
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(o), "f"(a8[0]), "f"(a8[1]), "f"(a8[2]), "f"(a8[3])
-                       : "memory");
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(o + 4), "f"(a8[4]), "f"(a8[5]), "f"(a8[6]),
-                       "f"(a8[7])
-                       : "memory");
+          red_add_f32x4(o, a8[0], a8[1], a8[2], a8[3]);
+          red_add_f32x4(o + 4, a8[4], a8[5], a8[6], a8[7]);
         } else if (flags & EPI_ACCUM) {
           float4 o0 = *reinterpret_cast<float4*>(o), o1 = *reinterpret_cast<float4*>(o + 4);
           o0.x += a8[0]; o0.y += a8[1]; o0.z += a8[2]; o0.w += a8[3];
@@ -415,6 +413,23 @@ __device__ __forceinline__ void add_bf16x4(float* v, uint2 w) {
 }
 __device__ __forceinline__ uint2 pack_bf16x4(const float* v) { return make_uint2(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3])); }
 
+// Epilogue staging of the 128 x 256 kernels.  Columns 64 j .. 64 j + 63 of a consumer warpgroup's m64n256 accumulators go into
+// its 64 x 64 fp32 buffer, XOR-swizzled (column ^ 8 (row & 3)) so that both the fragment stores and the row-segment loads are
+// free of bank conflicts.  Warp w then reads rows 16 w + 2 i + lane / 16 (i = 0..7), 4 columns (ws_lane_col) per lane.
+__device__ __forceinline__ void ws_stage_chunk(const float* acc, float* stage, int j, int w, int lane) {
+#pragma unroll
+  for (int i = 32 * j; i < 32 * j + 32; i += 2) {
+    const int r = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);
+    const int cc = 8 * ((i >> 2) - 8 * j) + 2 * (lane & 3);
+    *reinterpret_cast<float2*>(stage + r * 64 + (cc ^ ((r & 3) << 3))) = make_float2(acc[i], acc[i + 1]);
+  }
+}
+__device__ __forceinline__ int ws_lane_col(int lane) { return 4 * (lane & 15); }
+__device__ __forceinline__ int ws_chunk_row(int w, int i, int lane) { return 16 * w + 2 * i + (lane >> 4); }
+__device__ __forceinline__ float4 ws_load_row(const float* stage, int r, int cq) {
+  return *reinterpret_cast<const float4*>(stage + r * 64 + (cq ^ ((r & 3) << 3)));
+}
+
 __global__ void __launch_bounds__(384, 1) gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA,
                                                          const __grid_constant__ CUtensorMap tmB,
                                                          const __grid_constant__ GemmParams p) {
@@ -471,7 +486,7 @@ __global__ void __launch_bounds__(384, 1) gemm_ws_kernel(const __grid_constant__
   const int t = threadIdx.x & 127, w = t >> 5;
   float* stage = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes + c * Cfg::kEpiBytes);
   uint2* pf = reinterpret_cast<uint2*>(smem + kStages * Cfg::kStageBytes + 2 * Cfg::kEpiBytes + c * Cfg::kPfBytes);
-  const int cq = 4 * (lane & 15);  // epilogue: this lane's 4 columns of a 64-column chunk
+  const int cq = ws_lane_col(lane);  // epilogue: this lane's 4 columns of a 64-column chunk
   const EpiTensor* const pf_src[3] = {&p.aux, &p.res1, &p.res2};
   float acc[128];                  // written by each tile's first MMA (scale_d = 0)
   int it = 0;
@@ -491,7 +506,7 @@ __global__ void __launch_bounds__(384, 1) gemm_ws_kernel(const __grid_constant__
           if (e.p == nullptr) continue;
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
-            const int r = 16 * w + 2 * i + (lane >> 4);
+            const int r = ws_chunk_row(w, i, lane);
             if (r < rows_here)
               cp_async_8(pf + (q * 8 + i) * 128 + t, static_cast<const __nv_bfloat16*>(e.p) + mb * e.bs +
                                                          (static_cast<long long>(m0) + 64 * c + r) * e.ld + col_base + cl);
@@ -518,19 +533,13 @@ __global__ void __launch_bounds__(384, 1) gemm_ws_kernel(const __grid_constant__
     wgmma_wait<0>();
     if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
 
-    // ---- epilogue, 64 columns at a time.  The staging chunk is XOR-swizzled (column ^ 8 (row & 3)) so that both the fragment
-    // stores and the row-segment loads are free of bank conflicts.
+    // ---- epilogue, 64 columns at a time (ws_stage_chunk)
     const int flags = p.flags;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       if (64 * j >= n_valid) break;  // warpgroup-uniform
       named_bar_sync(1 + c, 128);    // the previous chunk has been read out of the staging buffer
-#pragma unroll
-      for (int i = 32 * j; i < 32 * j + 32; i += 2) {
-        const int r = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);
-        const int cc = 8 * ((i >> 2) - 8 * j) + 2 * (lane & 3);
-        *reinterpret_cast<float2*>(stage + r * 64 + (cc ^ ((r & 3) << 3))) = make_float2(acc[i], acc[i + 1]);
-      }
+      ws_stage_chunk(acc, stage, j, w, lane);
       const int cl = 64 * j + cq;
       const bool col_ok = cl < n_valid;
       const int col = col_base + cl;
@@ -541,8 +550,8 @@ __global__ void __launch_bounds__(384, 1) gemm_ws_kernel(const __grid_constant__
       cp_async_wait_all();  // this thread's inputs of chunk j have landed
 #pragma unroll 4
       for (int i = 0; i < 8; ++i) {
-        const int r = 16 * w + 2 * i + (lane >> 4);
-        const float4 v4 = *reinterpret_cast<const float4*>(stage + r * 64 + (cq ^ ((r & 3) << 3)));
+        const int r = ws_chunk_row(w, i, lane);
+        const float4 v4 = ws_load_row(stage, r, cq);
         if (!col_ok || r >= rows_here) continue;
         float v[4] = {v4.x + b4.x, v4.y + b4.y, v4.z + b4.z, v4.w + b4.w};
         const long long row = static_cast<long long>(m0) + 64 * c + r;
@@ -586,6 +595,157 @@ __global__ void __launch_bounds__(384, 1) gemm_ws_kernel(const __grid_constant__
         named_bar_sync(1 + c, 128);
         if (t < 64 && 64 * j + t < n_valid)
           atomicAdd(p.colsum + col_base + 64 * j + t, stage[t] + stage[64 + t] + stage[128 + t] + stage[192 + t]);
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------ persistent 128 x 256 stream-K weight gradient
+// dW[N, K] += sum over token rows of Y[row, n] X[row, k] (b200s_gemm_wgrad with K >= 256; p.m_rows = N, p.n_total = K).  Both
+// operands are MN-major and the reduction runs over K blocks = (batch, 64-row block).  Warp roles, ring and staging buffers are
+// gemm_ws_kernel's; a stage holds A as two 64 x 64 boxes (128 rows of dW x 64 tokens) and B as four (256 columns x 64 tokens).
+// Stream-K: the (tile, live K block) iteration space, tile-major, is cut into gridDim.x equal contiguous ranges.  A CTA accumulates
+// each piece of a tile in its range in registers and adds it to dW with vector fp32 reductions, row-coalesced through the staging
+// buffer, so there is no fix-up pass and no tile-count quantisation.
+// Walk order: the K blocks of tile t are visited rotated by rot(t) = t * Kl - (start of the range holding the tile's first block),
+// Kl = live K blocks.  At step s of its range a CTA then reads K block s + d * L (mod Kl), L = range length, d = which piece of
+// its tile it is working on.  The CTAs running together form a few fronts, each reading the same 64 token rows of Y and X at the
+// same time, and the fronts cover disjoint K blocks over the run, so Y and X are read from HBM about once.  (Unrotated, each CTA
+// would read token rows of its own, and the operands would come from HBM up to once per tile.)
+// Ragged batches: only live K blocks (below k_valid) are in the iteration space, so the ranges stay equal in work.
+__device__ __forceinline__ int wgrad_live_blocks(const GemmParams& p, int b) {
+  return p.k_valid == nullptr ? p.k_blocks_per_batch : min(p.k_blocks_per_batch, (max(__ldg(p.k_valid + b), 0) + 63) / 64);
+}
+
+__global__ void __launch_bounds__(384, 1) gemm_ws_wgrad_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                               const __grid_constant__ CUtensorMap tmB,
+                                                               const __grid_constant__ GemmParams p) {
+  pdl_launch_dependents();
+  using Cfg = WsCfg;
+  constexpr int kStages = Cfg::kStages;
+  const int wg = threadIdx.x >> 7;
+  const int lane = threadIdx.x & 31;
+  const int n_tiles = (p.n_total + 255) / 256;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  __shared__ uint64_t full_bar[kStages];
+  __shared__ uint64_t empty_bar[kStages];
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+#pragma unroll
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  const int batches = p.k_blocks / p.k_blocks_per_batch;
+  int kl = 0;
+  for (int b = 0; b < batches; ++b) kl += wgrad_live_blocks(p, b);
+  const long long total = static_cast<long long>(p.m_tiles) * n_tiles * kl;
+  const long long g_begin = blockIdx.x * total / gridDim.x, g_end = (blockIdx.x + 1) * total / gridDim.x;
+  // the pieces of this CTA's range: tile t, its K blocks j0 .. j1 - 1 in walk order
+  auto piece = [&](long long g, int& t, int& j0, int& j1) {
+    t = static_cast<int>(g / kl);
+    j0 = static_cast<int>(g - static_cast<long long>(t) * kl);
+    j1 = static_cast<int>(min(static_cast<long long>(kl), j0 + (g_end - g)));
+  };
+
+  if (wg == 0) {
+    // ------------------------------------------------------------ TMA producer
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int it = 0;
+      for (long long g = g_begin; g < g_end;) {
+        int t, j0, j1;
+        piece(g, t, j0, j1);
+        g += j1 - j0;
+        const int mt = t / n_tiles, n_tile = t - mt * n_tiles;
+        const long long x = static_cast<long long>(t) * kl;
+        const long long i0 = ((x + 1) * gridDim.x + total - 1) / total - 1;  // the range holding block 0 of tile t
+        int l = j0 + static_cast<int>((x - i0 * total / gridDim.x) % kl);  // rotated live block index
+        if (l >= kl) l -= kl;
+        int kbatch = 0;
+        while (l >= wgrad_live_blocks(p, kbatch)) l -= wgrad_live_blocks(p, kbatch++);
+        for (int j = j0; j < j1; ++j, ++it) {
+          const int s = it % kStages;
+          mbar_wait(&empty_bar[s], ((it / kStages) & 1) ^ 1);
+          uint8_t* sa = smem + s * Cfg::kStageBytes;
+          uint8_t* sb = sa + Cfg::kABytes;
+          mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
+#pragma unroll
+          for (int i = 0; i < 2; ++i) tma_load_4d(sa + i * 8192, &tmA, &full_bar[s], mt * 128 + 64 * i, l * 64, kbatch, 0);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) tma_load_4d(sb + i * 8192, &tmB, &full_bar[s], n_tile * 256 + 64 * i, l * 64, kbatch, 0);
+          if (++l == wgrad_live_blocks(p, kbatch)) {  // next live block, wrapping around the batches
+            l = 0;
+            do {
+              if (++kbatch == batches) kbatch = 0;
+            } while (wgrad_live_blocks(p, kbatch) == 0);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------- consumers: warpgroup c owns rows 64 c .. 64 c + 63 of a tile
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;
+  const int w = (threadIdx.x & 127) >> 5;
+  float* stage = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes + c * Cfg::kEpiBytes);
+  const int cq = ws_lane_col(lane);
+  float acc[128];  // written by each piece's first MMA (scale_d = 0)
+  int it = 0;
+  for (long long g = g_begin; g < g_end;) {
+    int t, j0, j1;
+    piece(g, t, j0, j1);
+    g += j1 - j0;
+    for (int j = 0; j < j1 - j0; ++j, ++it) {
+      const int s = it % kStages;
+      mbar_wait(&full_bar[s], (it / kStages) & 1);
+      const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes) + c * 8192;  // this warpgroup's 64 rows of dW x 64 tokens
+      const uint32_t sb = smem_u32(smem + s * Cfg::kStageBytes + Cfg::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n256k16<1, 1>(acc, make_smem_desc_sw128(sa + k * 2048, 8192, 1024),
+                               make_smem_desc_sw128(sb + k * 2048, 8192, 1024), (j > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous K block's MMAs have retired: its stage goes back to the producer
+      if (j > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
+    }
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
+
+    // ---- dW += the piece, 64 columns at a time (ws_stage_chunk), 16 lanes per 64-column row segment
+    const int mt = t / n_tiles, n_tile = t - mt * n_tiles;
+    const int m0 = mt * 128, col_base = n_tile * 256;
+    const int n_valid = min(256, p.n_total - col_base);
+    const int rows_here = min(128, p.m_rows - m0) - 64 * c;  // valid rows of this warpgroup's half (may be <= 0)
+    float* out = static_cast<float*>(p.out.p) + (static_cast<long long>(m0) + 64 * c) * p.out.ld + col_base;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (64 * j >= n_valid) break;  // warpgroup-uniform
+      named_bar_sync(1 + c, 128);    // the previous chunk has been read out of the staging buffer
+      ws_stage_chunk(acc, stage, j, w, lane);
+      named_bar_sync(1 + c, 128);
+      const int cl = 64 * j + cq;
+      if (cl < n_valid) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int r = ws_chunk_row(w, i, lane);
+          if (r < rows_here) {
+            const float4 v = ws_load_row(stage, r, cq);
+            red_add_f32x4(out + r * p.out.ld + cl, v.x, v.y, v.z, v.w);
+          }
+        }
       }
     }
   }

@@ -112,6 +112,11 @@ __device__ __forceinline__ void cp_async_8(void* smem_dst, const void* gsrc) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
+// 128-bit vector fp32 reduction into global memory (REDG.E.ADD.F32x4); p 16-byte aligned
+__device__ __forceinline__ void red_add_f32x4(float* p, float a, float b, float c, float d) {
+  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+
 // ---------------------------------------------------------------- wgmma (warpgroup MMA)
 // Shared-memory matrix descriptor (sm_90 format, cute/arch/mma_sm90_desc.hpp field layout):
 //   [0,14) start address >> 4, [16,30) leading byte offset >> 4, [32,46) stride byte offset >> 4, [62,64) layout (1 = SWIZZLE_128B).
