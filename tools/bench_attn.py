@@ -1,10 +1,16 @@
 """Micro-benchmark of the attention kernels at the WavLM-Base (16 x 749, 12 heads) and -Large (8 x 999, 16 heads) shapes.
-    python tools/bench_attn.py [--reps 10] [--only base|large] [--dropout 0.1]"""
-import argparse, os, sys
+    python tools/bench_attn.py [--reps 10] [--only base|large] [--dropout 0.1]
+Each line gives the time, the algorithmic TFLOP/s and its fraction of the bf16 peak (MEASURED_PEAKS.json when present, else
+the H100 SXM data sheet).  At the Large shape every backward is also checked once against autograd of the fp32 reference
+(dq / dk / dv, d gate, d tab; the tolerances of tests/test_kernels_gpu.py::test_attn_bwd); with dropout the reference applies
+the keep mask the forward kernel wrote."""
+import argparse, os, subprocess, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 from unispeech_b200 import ops
+from bench_gemm import load_peak
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--reps", type=int, default=10)
@@ -12,6 +18,64 @@ ap.add_argument("--only", default=None)
 ap.add_argument("--dropout", type=float, default=0.0, help="also time the kernels with dropout on the probabilities")
 args = ap.parse_args()
 dev = torch.device("cuda:0")
+peak, peak_src = load_peak()
+try:
+    card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True, check=True).stdout.strip()
+except (OSError, subprocess.CalledProcessError):
+    card = f"{torch.cuda.get_device_name(0)}, power limit unknown"
+print(f"GPU: {card}; peak: {peak} TFLOP/s ({peak_src})", flush=True)
+
+
+def attn_ref(qkv, gate, tab, B, T, H, scale, keep=None, p=0.0):
+    """fp32 attention with the gated relative-position bias; `keep` [B,H,T,T] (bool) drops probabilities, scaled by 1/(1-p)."""
+    D = H * 64
+    q, k, v = (x.view(B, T, H, 64).transpose(1, 2) for x in qkv.float().split(D, dim=-1))
+    s = torch.matmul(q, k.transpose(-1, -2)) * scale
+    if tab is not None:
+        i = torch.arange(T, device=qkv.device)[:, None]
+        j = torch.arange(T, device=qkv.device)[None, :]
+        s = s + gate.unsqueeze(-1) * tab[:, (j - i) + T - 1].unsqueeze(0)
+    pr = torch.softmax(s, dim=-1)
+    if keep is not None:
+        pr = pr * keep / (1.0 - p)
+    return torch.matmul(pr, v).transpose(1, 2).reshape(B, T, D)
+
+
+def keep_mask(words, B, T, H):
+    """The forward's dropout keep bits as [B,H,T,T] bool: bit i & 31 of word [(b*H+h)*4N + i/32, j]."""
+    N = (T + 127) // 128
+    w = words.view(B * H, 4 * N, 128 * N)[:, :, :T]
+    i = torch.arange(T, device=words.device)
+    rows = w[:, i // 32, :]                                   # [BH, T, T]
+    return ((rows >> (i % 32).view(1, T, 1).to(torch.int32)) & 1).bool().view(B, H, T, T)
+
+
+def check_bwd(name, run, qkv, gate, tab, dout, dqkv, dgate, dtab, B, T, H, keep=None, p=0.0):
+    """One more call of `run` against autograd of the fp32 reference; prints the worst error over each tolerance."""
+    if dtab is not None:
+        dtab.zero_()  # accumulated by every call
+    run()
+    torch.cuda.synchronize()
+    qr = qkv.float().requires_grad_(True)
+    gr = gate.clone().requires_grad_(True) if gate is not None else None
+    tr = tab.clone().requires_grad_(True) if tab is not None else None
+    attn_ref(qr, gr, tr, B, T, H, 0.125, keep, p).backward(dout.float())
+    errs = [("dqkv", dqkv.float(), qr.grad)]
+    if tab is not None:
+        errs += [("dgate", dgate, gr.grad), ("dtab", dtab, tr.grad)]
+    parts, ok = [], True
+    for k, got, ref in errs:
+        r = (got - ref).abs().max().item() / (0.03 * max(1.0, ref.abs().max().item()))
+        ok &= r < 1.0
+        parts.append(f"{k} {r:.3f}")
+    print(f"       check {name}: error / tolerance: {', '.join(parts)} -> {'ok' if ok else 'FAIL'}", flush=True)
+    del qr, gr, tr
+    torch.cuda.empty_cache()
+    return ok
+
+
+all_ok = True
 for name, B, T, H in (("base", 16, 749, 12), ("large", 8, 999, 16)):
     if args.only and args.only != name:
         continue
@@ -55,4 +119,13 @@ for name, B, T, H in (("base", 16, 749, 12), ("large", 8, 999, 16)):
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / args.reps
         mult = 1.0 if k.startswith("fwd") else 2.5
-        print(f"{name:6s} {k:18s} {ms*1e3:9.1f} us   {fl*mult/ms/1e9:8.1f} TFLOP/s (algorithmic)", flush=True)
+        tf = fl * mult / ms / 1e9
+        print(f"{name:6s} {k:18s} {ms*1e3:9.1f} us   {tf:8.1f} TFLOP/s (algorithmic)  {tf / peak:6.3f} of peak", flush=True)
+        if name == "large" and k.startswith("bwd"):
+            bias = k != "bwd_fused_nobias"
+            keep = keep_mask(words, B, T, H) if k == "bwd_fused_dropout" else None
+            all_ok &= check_bwd(k, fn, qkv, gate if bias else None, tab if bias else None, dout, dqkv, dgate, dtab if bias else None,
+                                B, T, H, keep, args.dropout)
+            del keep
+if not all_ok:
+    sys.exit(1)

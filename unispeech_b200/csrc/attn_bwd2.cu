@@ -1,20 +1,39 @@
 // Fused attention backward with the gated relative-position bias (autograd of WavLM/modules.py:521-563): ONE tensor-core
 // kernel produces dQ, dK, dV, d gate and d tab, so the probabilities are recomputed once.  wgmma + TMA (sm_90a).
 //
-// CTA = 128 keys of one (batch, head); it walks over the 128-row query tiles.  Two consumer warpgroups (WG w = 0, 1) and one TMA
-// warp.  Per query tile i, WG w owns query rows 64 w .. 64 w + 63 for the scores and key rows 64 w .. 64 w + 63 for the dK / dV
-// accumulators (registers, across the whole loop).  Everything element-wise is done on the wgmma accumulator fragments:
-//   for each 64-key half hf:
-//     S  = Q_i K_hf^T,  dP = dO_i V_hf^T                     wgmma m64n64k16 (64 query rows of this WG)
-//     P  = exp2(S*scale*log2e + gate_i*log2e*tab[j-i] + keymask_j - lse_i);   dS = P o (dP - Delta_i) * scale
-//     P, dS -> shared memory, bf16 [128 queries][128 keys] operand tiles (two 64-key blocks); gate*dS/scale -> a bf16 staging
-//     tile for the d tab diagonal sums (one tile: the first half's sums are taken before the second half is staged);
-//     d gate_i += sum_j dS_ij tab[j-i] (quad shuffles, one atomic per row)
+// CTA = 128 keys of one (batch, head); it walks over the 128-row query tiles with two warpgroups (WG w = 0, 1).  The scores
+// are computed transposed: WG w owns key rows 64 w .. 64 w + 63 against all 128 queries of the
+// tile, which are also the rows of its dK / dV accumulators (registers, across the whole loop).  Per query tile:
+//   S^T = K_w Q^T, dP^T = V_w dO^T          wgmma m64n128k16, two commit groups
+//   P^T = exp2(S^T*scale*log2e + gate_i*log2e*tab[j-i] + keymask_j - lse_i)      on the S^T fragments while dP^T is still
+//                                           on the tensor pipe;  dS^T = P^T o (dP^T - Delta_i) * scale  after it lands
+//   dV += P^T dO                            A = P^T as bf16 register fragments (wgmma RS form), B = dO MN-major: P never goes
+//                                           through shared memory
+//   dS^T -> shared memory (bf16 [2 query blocks][128 keys][64 queries], SWIZZLE_128B); gate*dS/scale -> a bf16 [128][130]
+//   staging tile; d gate_i = sum_j dS_ij tab[j-i]: a column sum of the fragments (shuffles + one shared slot per warp),
+//   one global atomic per query and tile
 //   (all 256 threads) barrier, then
-//   dV += P^T dO_i, dK += dS^T Q_i     A = P / dS tile read MN-major (M = this WG's 64 keys), B = dO / Q MN-major
-//   dQ_i = dS K                        A = dS read K-major (this WG's 64 queries), added to an fp32 [B,T,D] buffer with vector
-//                                      reductions (one writer CTA per key tile and query element)
-//   d tab[d] = sum_i gate_i dS_{i,i+d}  diagonal sums of the staged tiles, per-CTA accumulators, flushed with atomics at the end
+//   dK += dS^T Q                            A = this WG's rows of the dS^T tile (K-major), B = Q MN-major
+//   dQ_i = dS K                             this WG's 64 queries: A = dS^T tile read MN-major, B = K MN-major
+//   d tab[d] = sum_i gate_i dS_{i,i+d}      diagonal sums of the staged tile while the dV / dK / dQ MMAs run; per-CTA
+//                                           accumulators, flushed with atomics at the end
+//   dQ (fp32) -> the WG's half of the staging tile (it aliases the WG's own gate*dS rows), then one thread adds it into
+//   the fp32 [B,T,D] buffer with TMA bulk-tensor reductions (the box clips at T); the buffer is rewritten only after the
+//   reduction has read it
+// Thread 0 loads K / V once and refills a 2-stage ring of Q / dO tiles with TMA as soon as both warpgroups are done with a
+// stage; the per-query lse, Delta*scale and gate terms of the next tile are loaded into registers while the tile's dK / dQ
+// MMAs run and stored to their stage at its end.
+// Registers: the S^T and dP^T fragments and the dK / dV accumulators alone take 192 per thread, and ptxas uses 243-255 (CUDA
+// 12.9).  Hence:
+// - No producer warpgroup.  With one (384 threads, setmaxnreg.dec<40> / setmaxnreg.inc<232>) an earlier revision of this
+//   kernel, which also took dS^T as a register operand, compiled with 364-424 bytes of spills per variant, against 0-60 for
+//   the same code at 256 threads.
+// - dK reads dS^T from shared memory, not registers: 32 more registers live through the dS^T pass spilled.
+// - Query tiles do not overlap: issuing tile qi+1's S^T / dP^T (128 registers) before tile qi's dK / dQ group retires does
+//   not fit, and the two warpgroups run in step (the dS^T tile and the staging tile are shared by both).  Overlap is within a
+//   tile: exp2 with the dP^T chain, and the diagonal sums, the d gate flush and the next tile's loads with dV / dK / dQ.
+// - The two bias variants keep a few bytes of spill (8 / 4): ptxas parks this thread's two key-mask words on the stack
+//   before the loop and reloads them once per query tile.
 // Dropout: the keep bit of (query i, key j) is bit i & 31 of word drop_mask[block(i), j], written by the forward kernel.
 // Padding: a CTA whose 128 keys are all padded writes zero dK / dV rows and exits; query tiles that are fully padded at the end
 // of the utterance are not visited (their probabilities are zero: the forward leaves lse = +inf there).
@@ -33,24 +52,23 @@ __device__ __forceinline__ float ex2f(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void red_add_v2(float* dst, float a, float b) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(a), "f"(b) : "memory");
-}
 
 // shared-memory map (bytes from the 1024-aligned base)
 constexpr int kFK = 0;             // K tile          16 KB
 constexpr int kFV = 16384;         // V tile          16 KB
 constexpr int kFQ = 32768;         // Q tiles, 2 stages x 16 KB
 constexpr int kFDO = 65536;        // dO tiles, 2 stages x 16 KB
-constexpr int kFP = 98304;         // P  : [128 queries][128 keys] as two 64-key blocks, 32 KB
-constexpr int kFDS = 131072;       // dS : same layout, 32 KB
-constexpr int kFW = 163840;        // gate*dS staging for the diagonal sums: one [128 queries][66] bf16 tile
-constexpr int kWStride2 = 66;      // bf16 per staged row (33 words: conflict-free row writes and diagonal reads)
-constexpr int kFWBytes = 128 * kWStride2 * 2;   // 16896
-constexpr int kFTab = kFW + kFWBytes;            // 180736: tab slice [(N+1)*128], dtab_acc[(N+1)*128]
-constexpr int kConsumers = 256;                  // two warpgroups
-constexpr int kFThreads = kConsumers + 32;       // + the TMA warp
-constexpr int kProdWarp = kConsumers / 32;
+constexpr int kFDS = 98304;        // dS^T: [2 query blocks][128 keys][64 queries] bf16, 32 KB
+constexpr int kFW = 131072;        // gate*dS staging for the diagonal sums: [128 keys][kWStride] bf16 (33280 B) ...
+constexpr int kWStride = 130;      // bf16 per staged row (65 words: conflict-free diagonal reads)
+constexpr int kFDQ1 = 17408;       // ... aliased by the dQ staging of WG 0 at kFW and of WG 1 at kFW + kFDQ1 (16 KB each:
+                                   // two [64 queries][32] fp32 SWIZZLE_128B boxes), inside each WG's own staged rows
+constexpr int kFWBytes = kFDQ1 + 16384;          // 33792
+constexpr int kFScal = kFW + kFWBytes;           // 164864: per stage lse, Delta*scale, gate*log2e, gate/scale [4][128] fp32
+constexpr int kFDg = kFScal + 2 * 4 * 512;       // 168960: d gate partial column sums [8 warps][128] fp32
+constexpr int kFTab = kFDg + 8 * 512;            // 173056: tab slice [(N+1)*128], dtab_acc[(N+1)*128] fp32
+// Budget: 173056 + 2*(N+1)*512 + 1024 (alignment) = 207872 bytes at N = 32 (T = 4096, bias), under 227 KB per block.
+constexpr int kFThreads = 256;                   // two warpgroups
 
 }  // namespace
 
@@ -62,12 +80,13 @@ static inline int attn_bwd_smem_bytes(int N, bool bias) {
 template <bool HAS_BIAS, bool DROP>
 __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tm_qkv,
                                                                       const __grid_constant__ CUtensorMap tm_do,
-                                                                      const __grid_constant__ AttnParams p,
-                                                                      float* __restrict__ dq_acc) {
+                                                                      const __grid_constant__ CUtensorMap tm_dq,
+                                                                      const __grid_constant__ AttnParams p) {
   pdl_grid_sync();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int k0 = blockIdx.x * kAttnTile, h = blockIdx.y, b = blockIdx.z;
   const int T = p.T, D = p.D, N = p.n_tiles;
+  const long long bh = static_cast<long long>(b) * p.H + h;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, still a __shared__ pointer (LDS/STS, not generic)
@@ -75,12 +94,13 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
   uint8_t* sV = smem + kFV;
   uint8_t* sQ = smem + kFQ;
   uint8_t* sDO = smem + kFDO;
-  uint8_t* sP = smem + kFP;
   uint8_t* sDS = smem + kFDS;
+  float* scal = reinterpret_cast<float*>(smem + kFScal);
+  float* dgp = reinterpret_cast<float*>(smem + kFDg);
   float* tab_s = reinterpret_cast<float*>(smem + kFTab);  // slice[l] = tab[h, l + tab_base]
   float* dtab_acc = tab_s + (HAS_BIAS ? (N + 1) * kAttnTile : 0);  // [(N+1)*128]
 
-  __shared__ uint64_t kv_full, qdo_full[2], qdo_free[2];
+  __shared__ uint64_t kv_full, qdo_full[2];
   __shared__ uint32_t key_mask_s[4];  // bit j of word j>>5: key k0 + j is padded / beyond T
 
   // ---- padding: which of this CTA's keys are masked, and how many query tiles hold a valid query.  ONE pass over the
@@ -121,16 +141,14 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     }
   }
 
-  if (warp == kProdWarp && lane == 0) {
-    // the producer thread initialises the barriers itself and puts K, V and the first Q / dO tiles in flight right away: they
+  if (tid == 0) {
+    // thread 0 initialises the barriers itself and puts K, V and the first Q / dO tiles in flight right away: they
     // land while the rest of the CTA is still filling the tables (the other warps see the barriers after the __syncthreads below)
     tma_prefetch_desc(&tm_qkv);
     tma_prefetch_desc(&tm_do);
+    tma_prefetch_desc(&tm_dq);
     mbar_init(&kv_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&qdo_full[i], 1);
-      mbar_init(&qdo_free[i], kConsumers / 32);  // one arrival per consumer warp once its MMAs reading the stage have retired
-    }
+    for (int i = 0; i < 2; ++i) mbar_init(&qdo_full[i], 1);
     fence_mbar_init();
     mbar_expect_tx(&kv_full, 32768);
     tma_load_4d(sK, &tm_qkv, &kv_full, D + h * kHeadDim, k0, b, 0);
@@ -153,202 +171,262 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       dtab_acc[l] = 0.f;
     }
   }
-  __syncthreads();
-
-  if (warp == kProdWarp) {
-    // ================================================================== TMA producer: Q / dO stage refills
-    if (lane == 0) {
-      for (int qi = 2; qi < NQ; ++qi) {
-        const int s = qi & 1;
-        mbar_wait(&qdo_free[s], ((qi - 2) >> 1) & 1);  // the MMAs of tile qi-2 have retired
-        mbar_expect_tx(&qdo_full[s], 32768);
-        tma_load_4d(sQ + s * 16384, &tm_qkv, &qdo_full[s], h * kHeadDim, qi * kAttnTile, b, 0);
-        tma_load_4d(sDO + s * 16384, &tm_do, &qdo_full[s], h * kHeadDim, qi * kAttnTile, b, 0);
+  // per-query terms of a query tile, two per thread: threads 0..127 lse and Delta*scale, threads 128..255 gate*log2e and
+  // gate/scale of query tid & 127 (lse = +inf marks out-of-range queries: p = exp2(-inf) = 0)
+  const float inv_scale = 1.0f / p.scale;
+  auto load_terms = [&](int qi, float& t0, float& t1) {
+    const int i = qi * kAttnTile + (tid & 127);
+    t0 = tid < kAttnTile ? INFINITY : 0.f;
+    t1 = 0.f;
+    if (i < T) {
+      if (tid < kAttnTile) {
+        t0 = p.lse[bh * T + i];
+        t1 = p.delta[bh * T + i] * p.scale;
+      } else if (HAS_BIAS) {
+        const float gate = (p.gate != nullptr) ? p.gate[bh * T + i] : 1.0f;
+        t0 = gate * kLog2e;
+        t1 = gate * inv_scale;
       }
     }
-  } else {
-    // ==================================================================== consumer warpgroups
-    const int w = warp >> 2;                 // warpgroup: query rows 64 w.. of each tile, key rows 64 w.. of dK / dV
+  };
+  auto store_terms = [&](int qi, float t0, float t1) {
+    float* ts = scal + (qi & 1) * 4 * kAttnTile + (tid >> 7) * 2 * kAttnTile + (tid & 127);
+    ts[0] = t0;
+    ts[kAttnTile] = t1;
+  };
+  {
+    float t0, t1;
+    load_terms(0, t0, t1);
+    store_terms(0, t0, t1);
+  }
+  __syncthreads();
+
+  {
+    const int w = warp >> 2;                 // warpgroup: key rows 64 w .. 64 w + 63
     const int wq = warp & 3;
-    const int fr = 64 * w + 16 * wq + (lane >> 2);   // first of this thread's two fragment rows (the other is fr + 8)
+    const int kr = 64 * w + 16 * wq + (lane >> 2);   // first of this thread's two fragment key rows (the other is kr + 8)
     const int fc = 2 * (lane & 3);                    // column of fragment element 0 inside each 8-column group
     const float sc = p.scale * kLog2e;
-    const float inv_scale = 1.0f / p.scale;
-    const bool any_masked = (key_mask_s[0] | key_mask_s[1] | key_mask_s[2] | key_mask_s[3]) != 0u;  // uniform over the CTA
-    const long long bh = static_cast<long long>(b) * p.H + h;
+    bool row_masked[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) row_masked[rr] = ((key_mask_s[(kr + 8 * rr) >> 5] >> ((kr + 8 * rr) & 31)) & 1u) != 0u;
+    const bool flusher = (tid & 127) == 0;   // issues this WG's dQ reductions
+    uint8_t* dq_stage = smem + kFW + w * kFDQ1;
+    const uint32_t ak = smem_u32(sK) + w * 8192, av = smem_u32(sV) + w * 8192;
+    uint32_t* wtile = reinterpret_cast<uint32_t*>(smem + kFW);
 
     float dv_acc[32], dk_acc[32];  // written by the first tile's MMAs (scale_d = 0)
 
-    // diagonal sums of the staged gate*dS tile of (query tile qi, key half hf).  Task (e, s): elements (i = (jj - e) & 127, jj)
-    // for jj = 16 s .. 16 s + 15: diagonal jj - i = e (not wrapped, jj >= e) or e - 128 (wrapped).  The wrap point is a per-task
-    // constant, so every load is base + immediate.
-    auto diag_task = [&](int qi, int hf, int e, int s) {
-      const uint32_t* wtile = reinterpret_cast<const uint32_t*>(smem + kFW);
-      const int w0 = e - 16 * s;  // columns jj = 16 s + c with c < w0 are on the wrapped diagonal
-      const uint32_t base_nw = smem_u32(wtile) + static_cast<uint32_t>((16 * s - e) * kWStride2 + 16 * s) * 2u;
-      const uint32_t base_w = base_nw + static_cast<uint32_t>(kAttnTile * kWStride2 * 2);
+    // diagonal sums of the staged gate*dS tile of query tile qi.  Task (e, s): elements (key (ii + e) & 127, query ii) for
+    // ii = 16 s .. 16 s + 15: diagonal key - query = e (not wrapped, ii + e < 128) or e - 128 (wrapped).  The wrap point is a
+    // per-task constant, so every load is base + immediate.
+    auto diag_task = [&](int qi, int e, int s) {
+      const int w0 = kAttnTile - e - 16 * s;  // queries ii = 16 s + c with c >= w0 are on the wrapped diagonal
+      const uint32_t base_nw = smem_u32(wtile) + static_cast<uint32_t>(((16 * s + e) * kWStride + 16 * s) * 2);
+      const uint32_t base_w = base_nw - static_cast<uint32_t>(kAttnTile * kWStride * 2);
       float acc_all = 0.f, acc_nw = 0.f;
 #pragma unroll
       for (int c = 0; c < 16; ++c) {
-        const bool wrapped = c < w0;
+        const bool wrapped = c >= w0;
         uint32_t v16;
-        asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v16) : "r"((wrapped ? base_w : base_nw) + c * (kWStride2 + 1) * 2));
+        asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v16) : "r"((wrapped ? base_w : base_nw) + c * (kWStride + 1) * 2));
         const float v = __uint_as_float(v16 << 16);
         acc_all += v;
         if (!wrapped) acc_nw += v;
       }
-      const int l_nw = hf * 64 - qi * kAttnTile + e + N * kAttnTile - 1;
-      if (w0 < 16) atomicAdd(&dtab_acc[l_nw], acc_nw);
-      if (w0 > 0) atomicAdd(&dtab_acc[l_nw - kAttnTile], acc_all - acc_nw);
+      const int l_nw = e - qi * kAttnTile + N * kAttnTile - 1;
+      if (w0 > 0) atomicAdd(&dtab_acc[l_nw], acc_nw);
+      if (w0 < 16) atomicAdd(&dtab_acc[l_nw - kAttnTile], acc_all - acc_nw);
     };
 
+    mbar_wait(&kv_full, 0);
     for (int qi = 0; qi < NQ; ++qi) {
       const int st = qi & 1;
-      // per-row scalars of this thread's two fragment rows; lse = +inf marks out-of-range queries (p = exp2(-inf) = 0)
-      float r_lse[2], r_dsc[2], r_gl[2], r_gos[2];
-#pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        const int i = qi * kAttnTile + fr + 8 * rr;
-        float lse = INFINITY, delta = 0.f, gate = 0.f;
-        if (i < T) {
-          lse = p.lse[bh * T + i];
-          delta = p.delta[bh * T + i];
-          if (HAS_BIAS) gate = (p.gate != nullptr) ? p.gate[bh * T + i] : 1.0f;
-        }
-        r_lse[rr] = lse;
-        r_dsc[rr] = delta * p.scale;
-        r_gl[rr] = gate * kLog2e;
-        r_gos[rr] = gate * inv_scale;
-      }
-      float dg[2] = {0.f, 0.f};
-      mbar_wait(&kv_full, 0);
       mbar_wait(&qdo_full[st], (qi >> 1) & 1);
-      const uint32_t aq = smem_u32(sQ + st * 16384) + w * 8192, ad = smem_u32(sDO + st * 16384) + w * 8192;
+      const uint32_t bq = smem_u32(sQ + st * 16384), bdo = smem_u32(sDO + st * 16384);
+      float s_acc[64], d_acc[64];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n128k16<0, 0>(s_acc, make_smem_desc_sw128(ak + k * 32, 16, 1024), make_smem_desc_sw128(bq + k * 32, 16, 1024),
+                               k > 0 ? 1u : 0u);
+      wgmma_commit();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n128k16<0, 0>(d_acc, make_smem_desc_sw128(av + k * 32, 16, 1024), make_smem_desc_sw128(bdo + k * 32, 16, 1024),
+                               k > 0 ? 1u : 0u);
+      wgmma_commit();
+      // dropout keep words of this thread's two key rows for the tile's four 32-query blocks
+      uint32_t kw[2][4];
+      if (DROP) {
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+          for (int blk = 0; blk < 4; ++blk)
+            kw[rr][blk] = p.drop_mask[(bh * (4 * N) + qi * 4 + blk) * (N * kAttnTile) + k0 + kr + 8 * rr];
+      }
+      // the previous tile's dQ reduction has read this WG's staging buffer before the buffer is written again
+      if (qi > 0) {
+        if (flusher) bulk_wait_read0();
+        named_bar_sync(2 + w, 128);
+      }
+      const float* ts = scal + st * 4 * kAttnTile;   // lse, Delta*scale, gate*log2e, gate/scale of the tile's queries
+      const int tb0 = kr + N * kAttnTile - 1 - qi * kAttnTile;   // tab_s index of (key row kr, query 0)
 
-#pragma unroll 1
-      for (int hf = 0; hf < 2; ++hf) {
-        float s_acc[32], d_acc[32];
-        const uint32_t bk = smem_u32(sK) + hf * 8192, bv = smem_u32(sV) + hf * 8192;
-        wgmma_fence();
+      // P^T on the S^T fragments while the dP^T chain runs (fp32, in place)
+      wgmma_wait<1>();
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          wgmma_m64n64k16<0, 0>(s_acc, make_smem_desc_sw128(aq + k * 32, 16, 1024), make_smem_desc_sw128(bk + k * 32, 16, 1024),
-                                k > 0 ? 1u : 0u);
+      for (int g = 0; g < 16; ++g) {
+        const float2 lse = *reinterpret_cast<const float2*>(ts + 8 * g + fc);
+        float2 gl = make_float2(0.f, 0.f);
+        if (HAS_BIAS) gl = *reinterpret_cast<const float2*>(ts + 2 * kAttnTile + 8 * g + fc);
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          wgmma_m64n64k16<0, 0>(d_acc, make_smem_desc_sw128(ad + k * 32, 16, 1024), make_smem_desc_sw128(bv + k * 32, 16, 1024),
-                                k > 0 ? 1u : 0u);
-        wgmma_commit();
-        // dropout keep words of this thread's key columns (bit = query row & 31; both fragment rows are in one 32-row block)
-        const uint32_t* mrow = nullptr;
-        if (DROP) mrow = p.drop_mask + (bh * (4 * N) + ((qi * kAttnTile + fr) >> 5)) * (N * kAttnTile) + k0 + hf * 64 + fc;
-        wgmma_wait<0>();
-        uint32_t* wtile = reinterpret_cast<uint32_t*>(smem + kFW);
+        for (int rr = 0; rr < 2; ++rr) {
 #pragma unroll
-        for (int g = 0; g < 8; ++g) {        // 8-column group
-          uint2 kw = make_uint2(0u, 0u);     // keep words of columns fc, fc + 1 of the group
-          if (DROP) kw = *reinterpret_cast<const uint2*>(mrow + 8 * g);
-#pragma unroll
-          for (int rr = 0; rr < 2; ++rr) {   // fragment row
-            const int r = fr + 8 * rr;
-            const int i = qi * kAttnTile + r;
-            float pr2[2], ds2[2], w2[2];
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int idx = 4 * g + 2 * rr + e;
-              const int jj = hf * 64 + 8 * g + fc + e;   // key column inside the tile
-              float tb = 0.f;
-              if (HAS_BIAS) tb = tab_s[jj - r + N * kAttnTile - 1 - qi * kAttnTile];
-              float x = fmaf(s_acc[idx], sc, -r_lse[rr]);
-              if (HAS_BIAS) x = fmaf(r_gl[rr], tb, x);
-              float pr = ex2f(x);
-              if (any_masked) pr = ((key_mask_s[jj >> 5] >> (jj & 31)) & 1u) ? 0.f : pr;
-              float dpv = d_acc[idx];
-              bool keep = true;
-              if (DROP) {  // O = (P o M) V / (1-p):  dP = M o (dO V^T) / (1-p);  dV takes the dropped probabilities (scaled at the end)
-                keep = (((e ? kw.y : kw.x) >> (i & 31)) & 1u) != 0u;
-                dpv = keep ? dpv * p.drop_rp : 0.f;
-              }
-              const float ds = pr * fmaf(dpv, p.scale, -r_dsc[rr]);  // dS * scale
-              pr2[e] = keep ? pr : 0.f;
-              ds2[e] = ds;
-              w2[e] = 0.f;
-              if (HAS_BIAS) {
-                dg[rr] = fmaf(ds, tb, dg[rr]);
-                w2[e] = r_gos[rr] * ds;
-              }
-            }
-            // bf16 pairs into the operand tiles (K-major SWIZZLE_128B, block hf) and the diagonal staging tile
-            const int c = 8 * g + fc;  // column inside the 64-key block
-            const uint32_t off = static_cast<uint32_t>(hf * 16384 + r * 128 + ((g ^ (r & 7)) << 4) + (c & 7) * 2);
-            *reinterpret_cast<uint32_t*>(sP + off) = pack_bf16x2(pr2[0], pr2[1]);
-            *reinterpret_cast<uint32_t*>(sDS + off) = pack_bf16x2(ds2[0], ds2[1]);
-            if (HAS_BIAS) wtile[r * (kWStride2 / 2) + (c >> 1)] = pack_bf16x2(w2[0], w2[1]);
+          for (int e = 0; e < 2; ++e) {
+            const int idx = 4 * g + 2 * rr + e;
+            float x = fmaf(s_acc[idx], sc, -(e ? lse.y : lse.x));
+            if (HAS_BIAS) x = fmaf(e ? gl.y : gl.x, tab_s[tb0 + 8 * rr - (8 * g + fc + e)], x);
+            const float pr = ex2f(x);
+            s_acc[idx] = row_masked[rr] ? 0.f : pr;
           }
         }
-        if (HAS_BIAS && hf == 0) {  // the first half's diagonal sums, then the staging tile is free for the second half
-          named_bar_sync(1, kConsumers);
-          diag_task(qi, 0, tid & 127, tid >> 7);
-          diag_task(qi, 0, tid & 127, (tid >> 7) + 2);
-          named_bar_sync(1, kConsumers);
+      }
+
+      // dS^T after dP^T lands; bf16 operands for dV / dK, the dS^T tile and the staging tile; d gate column partials
+      wgmma_wait<0>();
+      uint32_t p16[32];
+#pragma unroll
+      for (int hq = 0; hq < 2; ++hq) {   // query halves: 16 d gate partials live at a time
+      float dg[16];
+#pragma unroll
+      for (int g = 8 * hq; g < 8 * hq + 8; ++g) {
+        const float2 dsc = *reinterpret_cast<const float2*>(ts + kAttnTile + 8 * g + fc);
+        float2 gos = make_float2(0.f, 0.f);
+        if (HAS_BIAS) gos = *reinterpret_cast<const float2*>(ts + 3 * kAttnTile + 8 * g + fc);
+        dg[2 * g - 16 * hq] = 0.f;
+        dg[2 * g + 1 - 16 * hq] = 0.f;
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int r = kr + 8 * rr;
+          float pd2[2], ds2[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int idx = 4 * g + 2 * rr + e;
+            const float pr = s_acc[idx];
+            float dpv = d_acc[idx];
+            bool keep = true;
+            if (DROP) {  // O = (P o M) V / (1-p):  dP = M o (dO V^T) / (1-p);  dV takes the dropped probabilities (scaled at the end)
+              keep = ((kw[rr][g >> 2] >> ((8 * g + fc + e) & 31)) & 1u) != 0u;
+              dpv = keep ? dpv * p.drop_rp : 0.f;
+            }
+            const float ds = pr * fmaf(dpv, p.scale, -(e ? dsc.y : dsc.x));  // dS * scale
+            pd2[e] = keep ? pr : 0.f;
+            ds2[e] = ds;
+            if (HAS_BIAS) dg[2 * g + e - 16 * hq] = fmaf(ds, tab_s[tb0 + 8 * rr - (8 * g + fc + e)], dg[2 * g + e - 16 * hq]);
+          }
+          p16[2 * g + rr] = pack_bf16x2(pd2[0], pd2[1]);
+          // dS^T tile: query block g >> 3, row = key, 16-byte chunk g & 7 (SWIZZLE_128B)
+          *reinterpret_cast<uint32_t*>(sDS + (g >> 3) * 16384 + r * 128 + (((g & 7) ^ (r & 7)) << 4) + fc * 2) =
+              pack_bf16x2(ds2[0], ds2[1]);
+          if (HAS_BIAS) wtile[r * (kWStride / 2) + 4 * g + (fc >> 1)] = pack_bf16x2((gos.x) * ds2[0], (gos.y) * ds2[1]);
         }
       }
       if (HAS_BIAS && p.dgate != nullptr) {
+        // column sums over the warp's 16 key rows (reduce-scatter over lane bits 2..4): lane l keeps columns
+        // 64 hq + 8 (l >> 2) + fc + e, e = 0, 1
+        float a[8], c4[4], c2[2];
+        {
+          const bool up = (lane & 16) != 0;
 #pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          float v = dg[rr];
-          v += __shfl_xor_sync(0xffffffffu, v, 1);
-          v += __shfl_xor_sync(0xffffffffu, v, 2);
-          const int i = qi * kAttnTile + fr + 8 * rr;
-          if ((lane & 3) == 0 && i < T) atomicAdd(p.dgate + bh * T + i, v * inv_scale);
+          for (int i = 0; i < 8; ++i) a[i] = (up ? dg[i + 8] : dg[i]) + __shfl_xor_sync(0xffffffffu, up ? dg[i] : dg[i + 8], 16);
         }
+        {
+          const bool up = (lane & 8) != 0;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) c4[i] = (up ? a[i + 4] : a[i]) + __shfl_xor_sync(0xffffffffu, up ? a[i] : a[i + 4], 8);
+        }
+        {
+          const bool up = (lane & 4) != 0;
+#pragma unroll
+          for (int i = 0; i < 2; ++i) c2[i] = (up ? c4[i + 2] : c4[i]) + __shfl_xor_sync(0xffffffffu, up ? c4[i] : c4[i + 2], 4);
+        }
+        *reinterpret_cast<float2*>(dgp + warp * kAttnTile + 64 * hq + 8 * (lane >> 2) + fc) = make_float2(c2[0], c2[1]);
       }
-      fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      named_bar_sync(1, kConsumers);
+      }
 
-      // ---- dV += P^T dO, dK += dS^T Q (this WG's 64 keys), dQ = dS K (this WG's 64 queries)
-      {
-        const uint32_t ap = smem_u32(sP) + w * 16384, ads = smem_u32(sDS) + w * 16384;
-        const uint32_t bdo = smem_u32(sDO + st * 16384), bq = smem_u32(sQ + st * 16384);
-        const uint32_t adq = smem_u32(sDS) + w * 8192, bk = smem_u32(sK);
-        float dq[32];
-        wgmma_fence();
+      // ---- dV += P^T dO (this WG's 64 keys; A = P^T from registers)
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 8; ++k)  // K = 128 queries, 16 per step
-          wgmma_m64n64k16<1, 1>(dv_acc, make_smem_desc_sw128(ap + k * 2048, 16384, 1024),
-                                make_smem_desc_sw128(bdo + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+      for (int k = 0; k < 8; ++k)  // K = 128 queries, 16 per step
+        wgmma_m64n64k16_rs<1>(dv_acc, p16 + 4 * k, make_smem_desc_sw128(bdo + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
+      named_bar_sync(1, kFThreads);
+
+      // ---- dK += dS^T Q (this WG's 64 keys; A = its rows of the dS^T tile, K-major).  From shared memory rather than registers:
+      // 32 more live registers through the dS^T pass would spill.
 #pragma unroll
-        for (int k = 0; k < 8; ++k)
-          wgmma_m64n64k16<1, 1>(dk_acc, make_smem_desc_sw128(ads + k * 2048, 16384, 1024),
-                                make_smem_desc_sw128(bq + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+      for (int k = 0; k < 8; ++k)
+        wgmma_m64n64k16<0, 1>(dk_acc, make_smem_desc_sw128(smem_u32(sDS) + (k >> 2) * 16384 + w * 8192 + (k & 3) * 32, 16, 1024),
+                              make_smem_desc_sw128(bq + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+      // ---- dQ = dS K (this WG's 64 queries; A = the dS^T tile read MN-major, K = 128 keys, 16 per step)
+      float dq[32];
 #pragma unroll
-        for (int k = 0; k < 8; ++k)  // K = 128 keys: two 64-key blocks, 16 per step
-          wgmma_m64n64k16<0, 1>(dq, make_smem_desc_sw128(adq + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
-                                make_smem_desc_sw128(bk + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
-        wgmma_commit();
-        if (HAS_BIAS) {  // the second half's diagonal sums while the MMAs run (256 threads, 2 tasks each)
-          diag_task(qi, 1, tid & 127, tid >> 7);
-          diag_task(qi, 1, tid & 127, (tid >> 7) + 2);
-        }
-        wgmma_wait<0>();
-        if (lane == 0) mbar_arrive(&qdo_free[st]);
-        // dQ rows of this WG -> fp32 reductions into dq_acc[b, q, h*64 + col]  (the staged dS already carries the softmax scale)
+      for (int k = 0; k < 8; ++k)
+        wgmma_m64n64k16<1, 1>(dq, make_smem_desc_sw128(smem_u32(sDS) + w * 16384 + k * 2048, 16384, 1024),
+                              make_smem_desc_sw128(smem_u32(sK) + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+      wgmma_commit();
+      // the next tile's per-query terms: loaded while the MMAs run, stored once this tile's have been read (not earlier: live
+      // across the exp2 pass they would push that pass over the register budget)
+      float nt0, nt1;
+      if (qi + 1 < NQ) load_terms(qi + 1, nt0, nt1);
+      if (HAS_BIAS) {  // the diagonal sums and the d gate flush while the MMAs run
+#pragma unroll 1
+        for (int s = tid >> 7; s < 8; s += 2) diag_task(qi, tid & 127, s);
+        if (p.dgate != nullptr && tid < kAttnTile) {
+          const int i = qi * kAttnTile + tid;
+          float v = 0.f;
 #pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          const int q = qi * kAttnTile + fr + 8 * rr;
-          if (q < T) {
-            float* dst = dq_acc + (static_cast<long long>(b) * T + q) * D + h * kHeadDim + fc;
-#pragma unroll
-            for (int g = 0; g < 8; ++g) red_add_v2(dst + 8 * g, dq[4 * g + 2 * rr], dq[4 * g + 2 * rr + 1]);
-          }
+          for (int wp = 0; wp < 8; ++wp) v += dgp[wp * kAttnTile + tid];
+          if (i < T) atomicAdd(p.dgate + bh * T + i, v * inv_scale);
         }
       }
-      named_bar_sync(1, kConsumers);  // P / dS / staging tiles may be overwritten by the next tile
+      wgmma_wait<0>();
+      if (qi + 1 < NQ) store_terms(qi + 1, nt0, nt1);
+      named_bar_sync(1, kFThreads);  // the Q / dO stage, the staging, dS^T and d gate tiles of this query tile are consumed
+      if (tid == 0 && qi + 2 < NQ) {
+        mbar_expect_tx(&qdo_full[st], 32768);
+        tma_load_4d(sQ + st * 16384, &tm_qkv, &qdo_full[st], h * kHeadDim, (qi + 2) * kAttnTile, b, 0);
+        tma_load_4d(sDO + st * 16384, &tm_do, &qdo_full[st], h * kHeadDim, (qi + 2) * kAttnTile, b, 0);
+      }
+
+      // dQ rows of this WG -> the staging boxes ([64 queries][32 fp32], SWIZZLE_128B; the staged dS already carries the
+      // softmax scale) -> TMA reductions into dq_acc[b, q, h*64 + col]
+      {
+        const int r0 = 16 * wq + (lane >> 2);
+#pragma unroll
+        for (int g = 0; g < 8; ++g)
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int r = r0 + 8 * rr, col = 8 * g + fc;
+            *reinterpret_cast<float2*>(dq_stage + (col >> 5) * 8192 + r * 128 + ((((col & 31) >> 2) ^ (r & 7)) << 4) + (col & 3) * 4) =
+                make_float2(dq[4 * g + 2 * rr], dq[4 * g + 2 * rr + 1]);
+          }
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(2 + w, 128);
+      if (flusher && qi * kAttnTile + 64 * w < T) {
+        tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage), h * kHeadDim, qi * kAttnTile + 64 * w, b);
+        tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage) + 8192, h * kHeadDim + 32, qi * kAttnTile + 64 * w, b);
+        bulk_commit();
+      }
     }
+    if (flusher) bulk_wait0();
     // ---- dK / dV rows of this WG (keys k0 + 64 w ..): bf16 pairs straight from the fragments
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
-      const int key = k0 + fr + 8 * rr;
+      const int key = k0 + kr + 8 * rr;
       if (key < T) {
         __nv_bfloat16* dst = p.dqkv + (static_cast<long long>(b) * T + key) * (3 * D) + h * kHeadDim + fc;
 #pragma unroll
@@ -361,9 +439,9 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     }
   }
 
-  __syncthreads();
   if (HAS_BIAS) {
     // per-CTA accumulators -> global (the relative-position table is shared by all layers: atomics)
+    named_bar_sync(1, kFThreads);
     if (p.dtab != nullptr) {
       for (int l = tid; l < (N + 1) * kAttnTile; l += kFThreads) {
         const int gi = l + tab_base;
@@ -417,6 +495,7 @@ __global__ void __launch_bounds__(256) attn_dq_convert_kernel(float* __restrict_
 }
 
 int make_qkv_tmap(CUtensorMap* out, const void* qkv, int T, int B, int D3, int box_rows);
+int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_rows);
 
 
 // Delta pre-kernel, the fused kernel and the dQ conversion on one stream (see the entry points below for the contract).
@@ -431,9 +510,10 @@ static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, c
       tab != nullptr ? dgate : nullptr));
   B200_CHECK_LAUNCH();
 
-  CUtensorMap tm_qkv, tm_do;
+  CUtensorMap tm_qkv, tm_do, tm_dq;
   if (make_qkv_tmap(&tm_qkv, qkv, T, B, 3 * D, kAttnTile)) return -3;
   if (make_qkv_tmap(&tm_do, dout, T, B, D, kAttnTile)) return -3;
+  if (make_f32_rows_tmap(&tm_dq, dq_acc, T, B, D, 64)) return -3;
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.T = T; p.H = H; p.B = B; p.D = D;
@@ -453,11 +533,11 @@ static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, c
   const int smem = attn_bwd_smem_bytes(N, tab != nullptr);
   B200_CHECK_ARG(smem <= 232448 - 512, "attn_bwd: T=%d needs %d bytes of shared memory", T, smem);
   dim3 grid(N, H, B);
-  void (*kern)(const CUtensorMap, const CUtensorMap, const AttnParams, float*) =
+  void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnParams) =
       tab != nullptr ? (drop ? attn_bwd_fused_kernel<true, true> : attn_bwd_fused_kernel<true, false>)
                      : (drop ? attn_bwd_fused_kernel<false, true> : attn_bwd_fused_kernel<false, false>);
   B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFThreads), smem, st, tm_qkv, tm_do, p, dq_acc));
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFThreads), smem, st, tm_qkv, tm_do, tm_dq, p));
   B200_CHECK_LAUNCH();
   const long long nvec = rows * (D / 8);
   const int blocks = static_cast<int>(std::min<long long>(ceil_div_ll(nvec, 256), static_cast<long long>(sm_count()) * 16));

@@ -116,6 +116,28 @@ int make_qkv_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int
   return make_tmap(out, v);
 }
 
+// [B, T, cols] fp32 row-major (the attention backward's dQ accumulator): rank 3 (cols, T, B), so a box clips at T inside each
+// utterance; box = 32 columns (one 128-byte swizzle row) x box_rows rows.  Used as the destination of TMA reductions.
+int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_rows) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) {
+    set_last_error("cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
+    return -3;
+  }
+  const cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(T), static_cast<cuuint64_t>(B)};
+  const cuuint64_t strides[2] = {static_cast<cuuint64_t>(cols) * 4, static_cast<cuuint64_t>(T) * cols * 4};
+  const cuuint32_t box[3] = {32, static_cast<cuuint32_t>(box_rows), 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled failed (%d) for the fp32 [%d, %d, %d] map", static_cast<int>(r), B, T, cols);
+    return -3;
+  }
+  return 0;
+}
+
 // ------------------------------------------------------------------ launch
 template <int BLOCK_N, bool A_MN, bool B_MN>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
