@@ -106,21 +106,21 @@ int b200s_posconv_wgrad(const void* dy, long long dy_bs, long long dy_rs, const 
  * Replaces compute_bias + gate multiply + F.multi_head_attention_forward (WavLM/modules.py:417-455,504-563); the
  * [B*H,T,T] bias is never materialised (it is Toeplitz).  qkv: bf16 [B,T,3D] fused projection output; gate: fp32
  * [B,H,T] or NULL (=1); tab: fp32 [H,2T-1] or NULL (no bias); key_pad: uint8 [B,T] or NULL; out: bf16 [B,T,D];
- * lse: fp32 [B,H,T] log2-domain log-sum-exp (saved for backward).  head_dim = 64; T <= 3840 with the bias table (shared-memory
- * copies of its slice), T <= 4096 without. */
+ * lse: fp32 [B,H,T] log2-domain log-sum-exp (saved for backward).  head_dim = 64; any T >= 1 with B*H*T < 2^32 (the
+ * kernel stages the bias window and key mask per key tile: its shared memory does not depend on T). */
 int b200s_attn_fwd(const void* qkv, const float* gate, const float* tab, const uint8_t* key_pad, void* out,
                    float* lse, int B, int T, int H, float scale, b200s_stream stream);
 
 /* Backward of b200s_attn_fwd (autograd of the same lines).  delta: fp32 [B,H,T] workspace; dqkv: bf16 [B,T,3D];
- * dgate: fp32 [B,H,T] (written); dtab: fp32 [H,2T-1] (+=, shared by all layers: WavLM/WavLM.py:549,594-599).  T <= 4096; runs the
- * fused kernel below with an fp32 dQ buffer allocated on the stream for the call. */
+ * dgate: fp32 [B,H,T] (written); dtab: fp32 [H,2T-1] (+=, shared by all layers: WavLM/WavLM.py:549,594-599).  Any T >= 1;
+ * runs the fused kernel below with an fp32 dQ buffer allocated on the stream for the call. */
 int b200s_attn_bwd(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                    const uint8_t* key_pad, const float* lse, float* delta, void* dqkv, float* dgate, float* dtab,
                    int B, int T, int H, float scale, b200s_stream stream);
 
 /* Same contract as b200s_attn_bwd, computed by ONE fused tensor-core kernel (csrc/attn_bwd2.cu: probabilities recomputed
  * once, dK/dV accumulated in registers, dQ reduced across key tiles in fp32).  dq_acc: fp32 [B,T,D] workspace that must be ZERO
- * on entry and is zero again on return.  T <= 2048. */
+ * on entry and is zero again on return.  Any T >= 1 (constant shared memory). */
 int b200s_attn_bwd_fused(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                          const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv,
                          float* dgate, float* dtab, int B, int T, int H, float scale, b200s_stream stream);
@@ -129,7 +129,8 @@ int b200s_attn_bwd_fused(const void* qkv, const void* out, const void* dout, con
  * F.multi_head_attention_forward, WavLM/modules.py:551): O = (softmax(..) o M) V / (1 - p).  M comes from the counter-based
  * hash of csrc/dropout.cuh keyed by (key0, key1, (b*H+h)*T + i, j); the forward kernel also records it as a bit mask
  * (drop_mask: b200s_attn_dropout_mask_words(B,T,H) uint32 words) which the fused backward re-reads, so the backward needs
- * no key.  drop_p = 0 is exactly b200s_attn_fwd / b200s_attn_bwd_fused (drop_mask may be NULL). */
+ * no key.  drop_p = 0 is exactly b200s_attn_fwd / b200s_attn_bwd_fused (drop_mask may be NULL).  B*H*T < 2^32 (the row
+ * counter of the hash); the mask takes B*H*T^2/8 bytes (134 MB per layer for one utterance of T = 8192 with 16 heads). */
 int b200s_attn_fwd_dropout(const void* qkv, const float* gate, const float* tab, const uint8_t* key_pad, void* out,
                            float* lse, int B, int T, int H, float scale, float drop_p, uint32_t key0, uint32_t key1,
                            uint32_t* drop_mask, b200s_stream stream);

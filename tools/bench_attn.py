@@ -1,5 +1,8 @@
 """Micro-benchmark of the attention kernels at the WavLM-Base (16 x 749, 12 heads) and -Large (8 x 999, 16 heads) shapes.
-    python tools/bench_attn.py [--reps 10] [--only base|large] [--dropout 0.1]
+    python tools/bench_attn.py [--reps 10] [--only base|large|long] [--dropout 0.1]
+`--only long` times one utterance with 16 heads at T = 8192 (164 s: the forward and both backward entry points) and
+T = 16384 (the forward), and checks every call once against the fp32 reference one head at a time (one [T, T] fp32
+matrix is 1 GB at T = 16384).
 Each line gives the time, the algorithmic TFLOP/s and its fraction of the bf16 peak (MEASURED_PEAKS.json when present, else
 the H100 SXM data sheet).  At the Large shape every backward is also checked once against autograd of the fp32 reference
 (dq / dk / dv, d gate, d tab; the tolerances of tests/test_kernels_gpu.py::test_attn_bwd); with dropout the reference applies
@@ -75,7 +78,84 @@ def check_bwd(name, run, qkv, gate, tab, dout, dqkv, dgate, dtab, B, T, H, keep=
     return ok
 
 
+def timed(fn):
+    for _ in range(2):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(args.reps):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / args.reps
+
+
+def head_cols(h, D):
+    return torch.cat([torch.arange(h * 64, h * 64 + 64) + o for o in (0, D, 2 * D)]).to(dev)
+
+
+def check_long(name, run, qkv, gate, tab, out, lse, dout, dqkv, dgate, dtab, B, T, H):
+    """One more call of `run` against the fp32 reference, one head at a time: the forward's output and lse, or the backward's
+    dq / dk / dv, d gate and d tab (tolerances of check_bwd)."""
+    D = H * 64
+    if dtab is not None:
+        dtab.zero_()
+    run()
+    torch.cuda.synchronize()
+    worst, fwd = 0.0, name.startswith("fwd")
+    for h in range(H):
+        c = head_cols(h, D)
+        qr = qkv[..., c].float().requires_grad_(not fwd)
+        gr = gate[:, h:h + 1].clone().requires_grad_(not fwd)
+        tr = tab[h:h + 1].clone().requires_grad_(not fwd)
+        if fwd:
+            with torch.no_grad():
+                ref = attn_ref(qr, gr, tr, B, T, 1, 0.125)
+            pairs = [(out[..., h * 64:(h + 1) * 64].float(), ref)]
+        else:
+            attn_ref(qr, gr, tr, B, T, 1, 0.125).backward(dout[..., h * 64:(h + 1) * 64].float())
+            pairs = [(dqkv[..., c].float(), qr.grad), (dgate[:, h], gr.grad[:, 0]), (dtab[h], tr.grad[0])]
+        for got, want in pairs:
+            worst = max(worst, (got - want).abs().max().item() / (0.03 * max(1.0, want.abs().max().item())))
+        del qr, gr, tr, pairs
+        torch.cuda.empty_cache()
+    ok = worst < 1.0
+    print(f"       check {name} T={T}: worst error / tolerance over the heads {worst:.3f} -> {'ok' if ok else 'FAIL'}", flush=True)
+    return ok
+
+
 all_ok = True
+if args.only == "long":
+    B, H = 1, 16
+    D = H * 64
+    for T, kinds in ((8192, ("fwd", "bwd_fused", "bwd_2kernel")), (16384, ("fwd",))):
+        torch.manual_seed(0)
+        qkv = torch.randn(B, T, 3 * D, device=dev).to(torch.bfloat16)
+        gate = torch.rand(B, H, T, device=dev) * 2 + 0.2
+        tab = torch.randn(H, 2 * T - 1, device=dev)
+        out = torch.empty(B, T, D, device=dev, dtype=torch.bfloat16)
+        lse = torch.empty(B, H, T, device=dev)
+        dout = torch.randn(B, T, D, device=dev).to(torch.bfloat16)
+        delta = torch.empty(B, H, T, device=dev)
+        dqkv = torch.zeros(B, T, 3 * D, device=dev, dtype=torch.bfloat16)
+        dgate = torch.zeros(B, H, T, device=dev)
+        dtab = torch.zeros(H, 2 * T - 1, device=dev)
+        dq_acc = torch.zeros(B, T, D, device=dev)
+        fns = {
+            "fwd": lambda: ops.attn_fwd(qkv, gate, tab, None, out, lse, B, T, H, 0.125),
+            "bwd_fused": lambda: ops.attn_bwd_fused(qkv, out, dout, gate, tab, None, lse, delta, dq_acc, dqkv, dgate, dtab, B, T, H,
+                                                    0.125),
+            "bwd_2kernel": lambda: ops.attn_bwd(qkv, out, dout, gate, tab, None, lse, delta, dqkv, dgate, dtab, B, T, H, 0.125),
+        }
+        fl = 4.0 * B * H * T * T * 64
+        for k in kinds:
+            ms = timed(fns[k])
+            tf = fl * (1.0 if k == "fwd" else 2.5) / ms / 1e9
+            print(f"long   {k:18s} T={T:5d} {ms*1e3:10.1f} us   {tf:8.1f} TFLOP/s (algorithmic)  {tf / peak:6.3f} of peak", flush=True)
+            all_ok &= check_long(k, fns[k], qkv, gate, tab, out, lse, dout, dqkv, dgate, dtab, B, T, H)
+        del qkv, gate, tab, out, lse, dout, delta, dqkv, dgate, dtab, dq_acc, fns
+        torch.cuda.empty_cache()
 for name, B, T, H in (("base", 16, 749, 12), ("large", 8, 999, 16)):
     if args.only and args.only != name:
         continue

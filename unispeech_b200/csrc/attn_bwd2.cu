@@ -15,15 +15,15 @@
 //   (all 256 threads) barrier, then
 //   dK += dS^T Q                            A = this WG's rows of the dS^T tile (K-major), B = Q MN-major
 //   dQ_i = dS K                             this WG's 64 queries: A = dS^T tile read MN-major, B = K MN-major
-//   d tab[d] = sum_i gate_i dS_{i,i+d}      diagonal sums of the staged tile while the dV / dK / dQ MMAs run; per-CTA
-//                                           accumulators, flushed with atomics at the end
+//   d tab[d] = sum_i gate_i dS_{i,i+d}      diagonal sums of the staged tile while the dV / dK / dQ MMAs run, into two
+//                                           128-float shared blocks (see below) flushed with atomics
 //   dQ (fp32) -> the WG's half of the staging tile (it aliases the WG's own gate*dS rows), then one thread adds it into
 //   the fp32 [B,T,D] buffer with TMA bulk-tensor reductions (the box clips at T); the buffer is rewritten only after the
 //   reduction has read it
 // Thread 0 loads K / V once and refills a 2-stage ring of Q / dO tiles with TMA as soon as both warpgroups are done with a
 // stage; the per-query lse, Delta*scale and gate terms of the next tile are loaded into registers while the tile's dK / dQ
 // MMAs run and stored to their stage at its end.
-// Registers: the S^T and dP^T fragments and the dK / dV accumulators alone take 192 per thread, and ptxas uses 243-255 (CUDA
+// Registers: the S^T and dP^T fragments and the dK / dV accumulators alone take 192 per thread, and ptxas uses 248-255 (CUDA
 // 12.9).  Hence:
 // - No producer warpgroup.  With one (384 threads, setmaxnreg.dec<40> / setmaxnreg.inc<232>) an earlier revision of this
 //   kernel, which also took dS^T as a register operand, compiled with 364-424 bytes of spills per variant, against 0-60 for
@@ -32,8 +32,16 @@
 // - Query tiles do not overlap: issuing tile qi+1's S^T / dP^T (128 registers) before tile qi's dK / dQ group retires does
 //   not fit, and the two warpgroups run in step (the dS^T tile and the staging tile are shared by both).  Overlap is within a
 //   tile: exp2 with the dP^T chain, and the diagonal sums, the d gate flush and the next tile's loads with dV / dK / dQ.
-// - The two bias variants keep a few bytes of spill (8 / 4): ptxas parks this thread's two key-mask words on the stack
-//   before the loop and reloads them once per query tile.
+// - The bias variant without dropout keeps 4 bytes of spill (a loop-invariant value stored before the query loop and
+//   reloaded once per query tile); the other three variants have none.
+// Bias window: inside a tile the bias of (key row kr, query column c) is tab[h, m - 128 + k0 - 128 qi + T - 1] with the window
+// coordinate m = kr - c + 128 in [1, 255], kept in a 256-float shared window at a fixed place (every read is base + immediate,
+// which the register budget needs).  The window of tile qi + 1 is the window of tile qi shifted by 128, so once tile qi's reads
+// are behind its middle barrier, threads 0..127 move the lower half up and copy the one new entry each into the lower half
+// (cp.async: no register is carried across the MMAs).  Shared memory is 176,128 bytes for every T.
+// d tab: two 128-float accumulator blocks, lower (m < 128: the wrapped diagonal tasks) and upper (m >= 128).  The upper block of
+// tile qi gets no contribution from a later tile, so after tile qi it is flushed to global memory, the lower block moves up
+// (it continues as the upper block of tile qi + 1) and the lower block is cleared.  At most NQ * 128 + 128 global atomics per CTA.
 // Dropout: the keep bit of (query i, key j) is bit i & 31 of word drop_mask[block(i), j], written by the forward kernel.
 // Padding: a CTA whose 128 keys are all padded writes zero dK / dV rows and exits; query tiles that are fully padded at the end
 // of the utterance are not visited (their probabilities are zero: the forward leaves lse = +inf there).
@@ -66,16 +74,11 @@ constexpr int kFDQ1 = 17408;       // ... aliased by the dQ staging of WG 0 at k
 constexpr int kFWBytes = kFDQ1 + 16384;          // 33792
 constexpr int kFScal = kFW + kFWBytes;           // 164864: per stage lse, Delta*scale, gate*log2e, gate/scale [4][128] fp32
 constexpr int kFDg = kFScal + 2 * 4 * 512;       // 168960: d gate partial column sums [8 warps][128] fp32
-constexpr int kFTab = kFDg + 8 * 512;            // 173056: tab slice [(N+1)*128], dtab_acc[(N+1)*128] fp32
-// Budget: 173056 + 2*(N+1)*512 + 1024 (alignment) = 207872 bytes at N = 32 (T = 4096, bias), under 227 KB per block.
+constexpr int kFSmem = kFDg + 8 * 512 + 1024;    // 174080 bytes with the alignment slack, for every T (+ 2 KB static: bias
+                                                 // window and d tab blocks)
 constexpr int kFThreads = 256;                   // two warpgroups
 
 }  // namespace
-
-// shared memory of the fused backward for N key tiles (with or without the relative-position bias)
-static inline int attn_bwd_smem_bytes(int N, bool bias) {
-  return kFTab + static_cast<int>(sizeof(float)) * ((bias ? (N + 1) * kAttnTile : 0) + (N + 1) * kAttnTile) + 1024;
-}
 
 template <bool HAS_BIAS, bool DROP>
 __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tm_qkv,
@@ -97,8 +100,9 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
   uint8_t* sDS = smem + kFDS;
   float* scal = reinterpret_cast<float*>(smem + kFScal);
   float* dgp = reinterpret_cast<float*>(smem + kFDg);
-  float* tab_s = reinterpret_cast<float*>(smem + kFTab);  // slice[l] = tab[h, l + tab_base]
-  float* dtab_acc = tab_s + (HAS_BIAS ? (N + 1) * kAttnTile : 0);  // [(N+1)*128]
+  // static, not in the dynamic map: addressed by immediates, which keeps the bias variants within their register budget
+  __shared__ __align__(16) float win_s[2 * kAttnTile];    // bias window of the current query tile, by m
+  __shared__ float dtab_acc[2 * kAttnTile];                // d tab blocks: lower (m < 128), upper
 
   __shared__ uint64_t kv_full, qdo_full[2];
   __shared__ uint32_t key_mask_s[4];  // bit j of word j>>5: key k0 + j is padded / beyond T
@@ -160,16 +164,12 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     }
   }
 
-  // per-CTA tables: slice[l] = tab[h, l + base], base = k0 - (N*128-1) + (T-1); element (query i, key k0 + j) -> l = j - i + N*128-1
-  const int tab_base = k0 - (N * kAttnTile - 1) + (T - 1);
-  if (HAS_BIAS) {
-    const int len = (N + 1) * kAttnTile;
-    const float* tab_h = p.tab + static_cast<long long>(h) * (2 * T - 1);
-    for (int l = tid; l < len; l += kFThreads) {
-      const int gi = l + tab_base;
-      tab_s[l] = (gi >= 0 && gi < 2 * T - 1) ? tab_h[gi] : 0.f;
-      dtab_acc[l] = 0.f;
-    }
+  // global index of window entry m of query tile qi: tab[h, m + win_base - 128 qi] (0 outside [0, 2T - 1))
+  const int win_base = k0 - kAttnTile + (T - 1);
+  if (HAS_BIAS) {  // tile 0's window, one entry per thread; cleared d tab blocks
+    const int gi = tid + win_base;
+    win_s[tid] = (gi >= 0 && gi < 2 * T - 1) ? p.tab[static_cast<long long>(h) * (2 * T - 1) + gi] : 0.f;
+    dtab_acc[tid] = 0.f;
   }
   // per-query terms of a query tile, two per thread: threads 0..127 lse and Delta*scale, threads 128..255 gate*log2e and
   // gate/scale of query tid & 127 (lse = +inf marks out-of-range queries: p = exp2(-inf) = 0)
@@ -234,9 +234,8 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
         acc_all += v;
         if (!wrapped) acc_nw += v;
       }
-      const int l_nw = e - qi * kAttnTile + N * kAttnTile - 1;
-      if (w0 > 0) atomicAdd(&dtab_acc[l_nw], acc_nw);
-      if (w0 < 16) atomicAdd(&dtab_acc[l_nw - kAttnTile], acc_all - acc_nw);
+      if (w0 > 0) atomicAdd(&dtab_acc[kAttnTile + e], acc_nw);   // upper block (m = e + 128)
+      if (w0 < 16) atomicAdd(&dtab_acc[e], acc_all - acc_nw);    // lower block (m = e)
     };
 
     mbar_wait(&kv_full, 0);
@@ -271,7 +270,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
         named_bar_sync(2 + w, 128);
       }
       const float* ts = scal + st * 4 * kAttnTile;   // lse, Delta*scale, gate*log2e, gate/scale of the tile's queries
-      const int tb0 = kr + N * kAttnTile - 1 - qi * kAttnTile;   // tab_s index of (key row kr, query 0)
+      const int tb0 = kr + kAttnTile;   // win_s index of (key row kr, query 0)
 
       // P^T on the S^T fragments while the dP^T chain runs (fp32, in place)
       wgmma_wait<1>();
@@ -286,7 +285,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
           for (int e = 0; e < 2; ++e) {
             const int idx = 4 * g + 2 * rr + e;
             float x = fmaf(s_acc[idx], sc, -(e ? lse.y : lse.x));
-            if (HAS_BIAS) x = fmaf(e ? gl.y : gl.x, tab_s[tb0 + 8 * rr - (8 * g + fc + e)], x);
+            if (HAS_BIAS) x = fmaf(e ? gl.y : gl.x, win_s[tb0 + 8 * rr - (8 * g + fc + e)], x);
             const float pr = ex2f(x);
             s_acc[idx] = row_masked[rr] ? 0.f : pr;
           }
@@ -323,7 +322,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
             const float ds = pr * fmaf(dpv, p.scale, -(e ? dsc.y : dsc.x));  // dS * scale
             pd2[e] = keep ? pr : 0.f;
             ds2[e] = ds;
-            if (HAS_BIAS) dg[2 * g + e - 16 * hq] = fmaf(ds, tab_s[tb0 + 8 * rr - (8 * g + fc + e)], dg[2 * g + e - 16 * hq]);
+            if (HAS_BIAS) dg[2 * g + e - 16 * hq] = fmaf(ds, win_s[tb0 + 8 * rr - (8 * g + fc + e)], dg[2 * g + e - 16 * hq]);
           }
           p16[2 * g + rr] = pack_bf16x2(pd2[0], pd2[1]);
           // dS^T tile: query block g >> 3, row = key, 16-byte chunk g & 7 (SWIZZLE_128B)
@@ -380,7 +379,18 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       // the next tile's per-query terms: loaded while the MMAs run, stored once this tile's have been read (not earlier: live
       // across the exp2 pass they would push that pass over the register budget)
       float nt0, nt1;
-      if (qi + 1 < NQ) load_terms(qi + 1, nt0, nt1);
+      if (qi + 1 < NQ) {
+        load_terms(qi + 1, nt0, nt1);
+        if (HAS_BIAS && tid < kAttnTile) {
+          // the window of tile qi + 1 (this tile's reads are behind the barrier above): the lower half moves up, the new
+          // entry m = tid comes straight from global memory
+          win_s[kAttnTile + tid] = win_s[tid];
+          const int gi = tid + win_base - (qi + 1) * kAttnTile;
+          const bool ok = gi >= 0;   // gi < 2T - 1 holds
+          cp_async_4_zfill(win_s + tid, p.tab + static_cast<long long>(h) * (2 * T - 1) + (ok ? gi : 0), ok);
+          cp_async_commit();
+        }
+      }
       if (HAS_BIAS) {  // the diagonal sums and the d gate flush while the MMAs run
 #pragma unroll 1
         for (int s = tid >> 7; s < 8; s += 2) diag_task(qi, tid & 127, s);
@@ -393,7 +403,10 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
         }
       }
       wgmma_wait<0>();
-      if (qi + 1 < NQ) store_terms(qi + 1, nt0, nt1);
+      if (qi + 1 < NQ) {
+        store_terms(qi + 1, nt0, nt1);
+        if (HAS_BIAS && tid < kAttnTile) cp_async_wait_all();
+      }
       named_bar_sync(1, kFThreads);  // the Q / dO stage, the staging, dS^T and d gate tiles of this query tile are consumed
       if (tid == 0 && qi + 2 < NQ) {
         mbar_expect_tx(&qdo_full[st], 32768);
@@ -421,6 +434,16 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
         tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage) + 8192, h * kHeadDim + 32, qi * kAttnTile + 64 * w, b);
         bulk_commit();
       }
+      if (HAS_BIAS && tid >= kAttnTile) {
+        // this tile's upper d tab block is complete (its diagonal sums are behind the closing barrier): flush it, move the lower
+        // block up and clear it, before tile qi + 1's diagonal sums start after that tile's middle barrier
+        const int e = tid - kAttnTile;
+        const int gi = e + win_base + kAttnTile - qi * kAttnTile;
+        const float v = dtab_acc[kAttnTile + e];
+        dtab_acc[kAttnTile + e] = dtab_acc[e];
+        dtab_acc[e] = 0.f;
+        if (p.dtab != nullptr && gi < 2 * T - 1 && v != 0.f) atomicAdd(p.dtab + static_cast<long long>(h) * (2 * T - 1) + gi, v);
+      }
     }
     if (flusher) bulk_wait0();
     // ---- dK / dV rows of this WG (keys k0 + 64 w ..): bf16 pairs straight from the fragments
@@ -439,16 +462,12 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     }
   }
 
-  if (HAS_BIAS) {
-    // per-CTA accumulators -> global (the relative-position table is shared by all layers: atomics)
-    named_bar_sync(1, kFThreads);
-    if (p.dtab != nullptr) {
-      for (int l = tid; l < (N + 1) * kAttnTile; l += kFThreads) {
-        const int gi = l + tab_base;
-        const float v = dtab_acc[l];
-        if (gi >= 0 && gi < 2 * T - 1 && v != 0.f) atomicAdd(p.dtab + static_cast<long long>(h) * (2 * T - 1) + gi, v);
-      }
-    }
+  if (HAS_BIAS && p.dtab != nullptr && tid >= kAttnTile) {
+    // the last tile's lower d tab block, which this thread moved to the upper block at the end of the loop -> global (the
+    // relative-position table is shared by all layers: atomics)
+    const int gi = (tid - kAttnTile) + win_base - (NQ - 1) * kAttnTile;
+    const float v = dtab_acc[tid];
+    if (gi >= 0 && gi < 2 * T - 1 && v != 0.f) atomicAdd(p.dtab + static_cast<long long>(h) * (2 * T - 1) + gi, v);
   }
 }
 
@@ -530,8 +549,7 @@ static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, c
   p.drop_mask = const_cast<uint32_t*>(drop_mask);
   p.drop_rp = 1.0f / (1.0f - drop_p);
   const int N = p.n_tiles;
-  const int smem = attn_bwd_smem_bytes(N, tab != nullptr);
-  B200_CHECK_ARG(smem <= 232448 - 512, "attn_bwd: T=%d needs %d bytes of shared memory", T, smem);
+  const int smem = kFSmem;
   dim3 grid(N, H, B);
   void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnParams) =
       tab != nullptr ? (drop ? attn_bwd_fused_kernel<true, true> : attn_bwd_fused_kernel<true, false>)
@@ -560,7 +578,7 @@ int b200s_attn_bwd(const void* qkv, const void* out, const void* dout, const flo
                    const uint8_t* key_pad, const float* lse, float* delta, void* dqkv, float* dgate, float* dtab, int B,
                    int T, int H, float scale, b200s_stream stream) {
   B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv, "attn_bwd: null pointer");
-  B200_CHECK_ARG(T >= 1 && T <= 4096, "attn_bwd: T=%d out of range (1..4096)", T);
+  B200_CHECK_ARG(T >= 1, "attn_bwd: T=%d out of range", T);
   B200_CHECK_ARG(!tab || (dgate && dtab), "attn_bwd: bias given but dgate/dtab missing");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t bytes = sizeof(float) * static_cast<size_t>(B) * T * H * kHeadDim;
@@ -582,7 +600,7 @@ int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* d
   B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv && dq_acc, "attn_bwd_fused: null pointer");
   B200_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f, "attn_bwd_fused: dropout p=%f out of range [0,1)", static_cast<double>(drop_p));
   B200_CHECK_ARG(drop_p == 0.f || drop_mask != nullptr, "attn_bwd_fused: dropout needs the mask written by b200s_attn_fwd_dropout");
-  B200_CHECK_ARG(T >= 1 && T <= 2048, "attn_bwd_fused: T=%d out of range (1..2048)", T);
+  B200_CHECK_ARG(T >= 1, "attn_bwd_fused: T=%d out of range", T);
   B200_CHECK_ARG(!tab || (dgate && dtab), "attn_bwd_fused: bias given but dgate/dtab missing");
   return attn_bwd_launch(qkv, out, dout, gate, tab, key_pad, lse, delta, dq_acc, dqkv, dgate, dtab, B, T, H, scale, drop_p,
                          drop_mask, static_cast<cudaStream_t>(stream));

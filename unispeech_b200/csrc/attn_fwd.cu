@@ -16,8 +16,13 @@
 // Padding: key tiles that are fully padded at the END of the utterance are skipped (the loop runs over n_eff tiles), and a CTA
 // whose 128 query rows are all padded only writes zeros -- padded frames never influence valid ones (keys are masked) and the
 // reference's values there are unspecified garbage, so the ragged batch does not pay for its padding.
-// The per-head Toeplitz bias table is kept in shared memory as FOUR copies shifted by 0..3 elements, so the 32 consecutive
-// entries a thread needs per 32-column chunk are 8 aligned 128-bit loads instead of 32 scalar ones.
+// Bias and key mask are staged per key tile, so shared memory does not grow with T: key tile n reads the 255 consecutive bias
+// entries slice[k0 .. k0 + 254] (slice[k] = tab[h, k + T - 1 - (q0 + 127)]), kept as FOUR copies shifted by 0..3 elements so
+// that the 32 consecutive entries a thread needs per 32-column chunk are 8 aligned 128-bit loads instead of 32 scalar ones,
+// next to the tile's 128-float additive key mask and its flag.  The TMA warp, idle between its K / V issues, fills that stage
+// one tile ahead (tile n in buffer n & 1) and arrives on the buffer's mbarrier; the stage of tile n - 2 is free once the
+// v_empty arrival of that tile has been seen.  The table is at most a few MB and stays in L2.
+// Shared memory: 149504 B of Q / K / V / P / scores + 2 x 4752 B of stages + 1024 B alignment = 160032 B for every T.
 #include "../../include/unispeech_b200.h"
 #include "attn_common.cuh"
 #include "common.h"
@@ -51,14 +56,15 @@ constexpr int kFwdV = 32768;                    // 16 KB
 constexpr int kFwdP = 49152;                    // 32 KB: [2 key blocks][128 rows][64 keys] bf16
 constexpr int kSPitch = kAttnTile + 4;          // fp32 score row (floats)
 constexpr int kFwdS = 81920;                    // fp32 scores [128][kSPitch]
-constexpr int kFwdTab = kFwdS + kAttnTile * kSPitch * 4;  // 149504: fp32 bias-table copies, key mask, tile flags
+constexpr int kFwdStage = kFwdS + kAttnTile * kSPitch * 4;  // 149504: two per-key-tile stages (bias copies, key mask)
 constexpr int kFwdThreads = 160;                // one warpgroup + TMA warp
 constexpr int kTabCopies = 4;
+// floats of ONE bias-table copy: 256 window entries + 8 so that consecutive copies start 8 banks apart (conflict-free 128-bit
+// loads across the quarter warp, whose lanes alternate between the four copies)
+constexpr int kTabStride = 2 * kAttnTile + 8;
+constexpr int kStageFloats = kTabCopies * kTabStride + kAttnTile + 4;   // copies, key mask, flag (+3 floats of padding)
+constexpr int kFwdSmem = kFwdStage + 2 * kStageFloats * 4 + 1024;       // 160032 (+ 1024 for the alignment of the base)
 constexpr float kRebase = 1.2089258e24f;        // 2^80: a tile whose row sum reaches this is re-based on its own maximum
-
-// floats of ONE bias-table copy: (N + 1) * 128 entries + 8 so that consecutive copies start 8 banks apart (conflict-free
-// 128-bit loads across the quarter warp, whose lanes alternate between the four copies)
-__host__ __device__ constexpr int fwd_tab_stride(int N) { return (N + 1) * kAttnTile + 8; }
 
 __device__ __forceinline__ void lds_row32(const float* src, uint32_t* r) {
 #pragma unroll
@@ -84,30 +90,27 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
   uint8_t* sV = smem + kFwdV;
   uint8_t* sP = smem + kFwdP;
   float* s_f = reinterpret_cast<float*>(smem + kFwdS);
-  float* tab_s = reinterpret_cast<float*>(smem + kFwdTab);           // [4][fwd_tab_stride(N)]: copy c holds slice[i + c]
-  const int tab_stride = fwd_tab_stride(N);
-  float* kbias = tab_s + (HAS_BIAS ? kTabCopies * tab_stride : 0);  // [N*128]
-  int* tile_flags = reinterpret_cast<int*>(kbias + N * kAttnTile);  // [N]: 0 no masked key, 1 some, 2 all
+  // stage of key tile n in buffer n & 1: [4][kTabStride] bias copies (copy c holds window[i + c], window[i] = slice[k0 + i]),
+  // then the tile's 128-float additive key mask, then its flag (0 no masked key, 1 some, 2 all)
+  float* stage = reinterpret_cast<float*>(smem + kFwdStage);
 
-  __shared__ uint64_t q_full, k_full, k_empty, v_full, v_empty;
+  __shared__ uint64_t q_full, k_full, k_empty, v_full, v_empty, stage_full[2];
   __shared__ float row_scale[kAttnTile];  // per query row: re-base factor of the current tile, then 1 / row sum for the epilogue
 
-  // ---- key padding: additive mask, per-tile flags, number of key tiles that hold any valid key, and whether any of this CTA's
-  // 128 query rows is live.  ONE pass over the utterance's pad bytes (every thread takes a few), shared-memory counters, one
-  // barrier: the prologue pays a single global-load latency instead of one per key tile.
+  // ---- key padding: the number of key tiles that hold any valid key, and whether any of this CTA's 128 query rows is live.
+  // ONE pass over the utterance's pad bytes (every thread takes a few), shared-memory counters, one barrier: the prologue pays a
+  // single global-load latency instead of one per key tile.
   __shared__ int n_eff_s, live_s;
-  for (int t = tid; t < N; t += kFwdThreads) tile_flags[t] = 0;   // masked keys per tile (turned into 0 / 1 / 2 below)
-  if (tid == 0) { n_eff_s = 1; live_s = 0; }
+  if (tid == 0) { n_eff_s = p.key_pad != nullptr ? 1 : N; live_s = 0; }
   __syncthreads();
-  {
+  if (p.key_pad != nullptr) {
     int last_valid = -1;
     bool live = false;
-    for (int j = tid; j < N * kAttnTile; j += kFwdThreads) {
-      const bool masked = (j >= T) || (p.key_pad != nullptr && p.key_pad[static_cast<long long>(b) * T + j] != 0);
-      kbias[j] = masked ? -INFINITY : 0.f;
-      if (masked) atomicAdd(&tile_flags[j / kAttnTile], 1);
-      else last_valid = j;                                     // increasing j: the last hit is the largest
-      if (!masked && j >= q0 && j < q0 + kAttnTile) live = true;
+    for (int j = tid; j < T; j += kFwdThreads) {
+      if (p.key_pad[static_cast<long long>(b) * T + j] == 0) {
+        last_valid = j;                                        // increasing j: the last hit is the largest
+        if (j >= q0 && j < q0 + kAttnTile) live = true;
+      }
     }
     if (last_valid >= 0) atomicMax(&n_eff_s, last_valid / kAttnTile + 1);
     if (live) live_s = 1;
@@ -124,20 +127,18 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
     }
     return;
   }
-  for (int t = tid; t < N; t += kFwdThreads) {  // counts -> 0 no masked key, 1 some, 2 all (read after the barrier below)
-    const int c = tile_flags[t];
-    tile_flags[t] = (c == 0) ? 0 : (c == kAttnTile ? 2 : 1);
-  }
 
   if (warp == 4 && lane == 0) {
-    // the TMA thread initialises the barriers itself and puts Q and the first K / V tiles in flight right away: they land while
-    // the rest of the CTA is still filling the bias-table copies (the other warps see the barriers after the __syncthreads below)
+    // the TMA thread initialises the barriers itself and puts Q and the first K / V tiles in flight right away (the other
+    // warps see the barriers after the __syncthreads below)
     tma_prefetch_desc(&tm);
     mbar_init(&q_full, 1);
     mbar_init(&k_full, 1);
     mbar_init(&v_full, 1);
     mbar_init(&k_empty, 4);   // one arrival per warp of the warpgroup once its S MMAs have retired
     mbar_init(&v_empty, 4);   // ... once its PV MMAs have retired
+    mbar_init(&stage_full[0], 32);   // one arrival per lane of the TMA warp once its part of the stage is stored
+    mbar_init(&stage_full[1], 32);
     fence_mbar_init();
     mbar_expect_tx(&q_full, 16384);
     tma_load_4d(sQ, &tm, &q_full, h * kHeadDim, q0, b, 0);
@@ -146,30 +147,62 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
     mbar_expect_tx(&v_full, 16384);
     tma_load_4d(sV, &tm, &v_full, 2 * D + h * kHeadDim, 0, b, 0);
   }
-  if (HAS_BIAS) {
-    const int len = (N + 1) * kAttnTile;
-    const int base = (T - 1) - (q0 + kAttnTile - 1);
-    const float* tab_h = p.tab + static_cast<long long>(h) * (2 * T - 1);
-    for (int i = tid; i < kTabCopies * len; i += kFwdThreads) {
-      const int c = i / len, k = i - c * len;
-      const int gi = k + c + base;
-      tab_s[c * tab_stride + k] = (gi >= 0 && gi < 2 * T - 1) ? tab_h[gi] : 0.f;
-    }
-  }
   __syncthreads();
 
   if (warp == 4) {
     // ------------------------------------------------------------------ TMA producer warp
-    if (lane == 0) {
-      for (int n = 1; n < n_eff; ++n) {  // (Q and tile 0 were issued in the prologue)
-        const uint32_t ph = (n - 1) & 1;
-        mbar_wait(&k_empty, ph);
+    // stage of key tile n: lane l loads window entries l + 32 t (259 are needed: 255 read + the 3 of the widest shift) and
+    // stores each into the copies that hold it, and builds the key mask of keys k0 + 4 l .. k0 + 4 l + 3
+    auto fill_stage = [&](int n) {
+      float* stg = stage + (n & 1) * kStageFloats;
+      const int k0 = n * kAttnTile;
+      if (HAS_BIAS) {
+        const int base = k0 + (T - 1) - (q0 + kAttnTile - 1);
+        const float* tab_h = p.tab + static_cast<long long>(h) * (2 * T - 1);
+        float v[9];
+#pragma unroll
+        for (int t = 0; t < 9; ++t) {
+          const int i = lane + 32 * t, gi = base + i;
+          v[t] = (i < 2 * kAttnTile + kTabCopies - 1 && gi >= 0 && gi < 2 * T - 1) ? tab_h[gi] : 0.f;
+        }
+#pragma unroll
+        for (int t = 0; t < 9; ++t)
+#pragma unroll
+          for (int c = 0; c < kTabCopies; ++c) {
+            const int k = lane + 32 * t - c;
+            if (k >= 0 && k < 2 * kAttnTile) stg[c * kTabStride + k] = v[t];
+          }
+      }
+      float kb[4];
+      int cnt = 0;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int j = k0 + 4 * lane + e;
+        const bool masked = (j >= T) || (p.key_pad != nullptr && p.key_pad[static_cast<long long>(b) * T + j] != 0);
+        kb[e] = masked ? -INFINITY : 0.f;
+        cnt += masked ? 1 : 0;
+      }
+      reinterpret_cast<float4*>(stg + kTabCopies * kTabStride)[lane] = make_float4(kb[0], kb[1], kb[2], kb[3]);
+      cnt = __reduce_add_sync(0xffffffffu, cnt);
+      if (lane == 0) reinterpret_cast<int*>(stg)[kTabCopies * kTabStride + kAttnTile] = (cnt == 0) ? 0 : (cnt == kAttnTile ? 2 : 1);
+      mbar_arrive(&stage_full[n & 1]);
+    };
+    fill_stage(0);
+    if (n_eff > 1) fill_stage(1);
+    for (int n = 1; n < n_eff; ++n) {  // (Q and tile 0 were issued in the prologue)
+      const uint32_t ph = (n - 1) & 1;
+      mbar_wait(&k_empty, ph);
+      if (lane == 0) {
         mbar_expect_tx(&k_full, 16384);
         tma_load_4d(sK, &tm, &k_full, D + h * kHeadDim, n * kAttnTile, b, 0);
-        mbar_wait(&v_empty, ph);
+      }
+      mbar_wait(&v_empty, ph);
+      if (lane == 0) {
         mbar_expect_tx(&v_full, 16384);
         tma_load_4d(sV, &tm, &v_full, 2 * D + h * kHeadDim, n * kAttnTile, b, 0);
       }
+      // tile n - 1 has retired its PV MMAs, so its stage (buffer (n + 1) & 1) has been read: fill it with tile n + 1
+      if (n + 1 < n_eff) fill_stage(n + 1);
     }
   } else {
     // ------------------------------------------------------------------ the warpgroup: MMAs + softmax, thread = query row
@@ -185,10 +218,10 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
       gl = g * kLog2e;
     }
     const float sc = p.scale * kLog2e;
-    // this row's window of the bias table: entry (key j) = slice[j + 127 - r]; copy a = (127 - r) & 3 is the one in which that
-    // window starts on a 16-byte boundary
+    // this row's part of a tile's bias window: entry (key k0 + j) = window[j + 127 - r]; copy a = (127 - r) & 3 is the one in
+    // which that part starts on a 16-byte boundary
     const int toff = kAttnTile - 1 - r;
-    const float4* tab4 = reinterpret_cast<const float4*>(tab_s + (toff & 3) * tab_stride + (toff & ~3));
+    const int tab_off = (toff & 3) * kTabStride + (toff & ~3);
     // dropout on the probabilities: per-row hash keys, and where this warp's 32 rows keep their bits (one word per key column)
     uint32_t rk0 = 0, rk1 = 0;
     uint32_t* mask_row = nullptr;
@@ -221,7 +254,11 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
       }
       if (lane == 0) mbar_arrive(&k_empty);  // this warp's S MMAs have retired: K may be refilled
       named_bar_sync(1, kAttnTile);           // the whole score tile is staged
-      const bool msk = tile_flags[n] != 0;
+      mbar_wait(&stage_full[n & 1], (n >> 1) & 1);
+      const float* stg = stage + (n & 1) * kStageFloats;
+      const float4* tab4 = reinterpret_cast<const float4*>(stg + tab_off);
+      const float* kbias = stg + kTabCopies * kTabStride;
+      const bool msk = reinterpret_cast<const int*>(stg)[kTabCopies * kTabStride + kAttnTile] != 0;
 
       auto tile_max = [&]() {  // row maximum of the exponent argument over this tile (bias and key mask included)
         float mx = -INFINITY;
@@ -232,14 +269,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             float4 tb = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (HAS_BIAS) tb = tab4[(k0 + c0) / 4 + q];
+            if (HAS_BIAS) tb = tab4[c0 / 4 + q];
             float x0 = __uint_as_float(su[4 * q]) * sc, x1 = __uint_as_float(su[4 * q + 1]) * sc;
             float x2 = __uint_as_float(su[4 * q + 2]) * sc, x3 = __uint_as_float(su[4 * q + 3]) * sc;
             if (HAS_BIAS) {
               x0 = fmaf(gl, tb.x, x0); x1 = fmaf(gl, tb.y, x1); x2 = fmaf(gl, tb.z, x2); x3 = fmaf(gl, tb.w, x3);
             }
             if (msk) {
-              const float4 kb = *reinterpret_cast<const float4*>(kbias + k0 + c0 + 4 * q);
+              const float4 kb = *reinterpret_cast<const float4*>(kbias + c0 + 4 * q);
               x0 += kb.x; x1 += kb.y; x2 += kb.z; x3 += kb.w;
             }
             mx = fmaxf(fmaxf(mx, fmaxf(x0, x1)), fmaxf(x2, x3));
@@ -270,8 +307,8 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             float4 tb = make_float4(0.f, 0.f, 0.f, 0.f), kb = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (HAS_BIAS) tb = tab4[(k0 + c0) / 4 + q];
-            if (kMsk) kb = *reinterpret_cast<const float4*>(kbias + k0 + c0 + 4 * q);
+            if (HAS_BIAS) tb = tab4[c0 / 4 + q];
+            if (kMsk) kb = *reinterpret_cast<const float4*>(kbias + c0 + 4 * q);
             const float tbv[4] = {tb.x, tb.y, tb.z, tb.w};
             const float kbv[4] = {kb.x, kb.y, kb.z, kb.w};
 #pragma unroll
@@ -402,9 +439,8 @@ int b200s_attn_fwd_dropout(const void* qkv, const float* gate, const float* tab,
   memset(&p, 0, sizeof(p));
   p.T = T; p.H = H; p.B = B; p.D = D;
   p.n_tiles = ceil_div(T, kAttnTile);
-  const int smem = kFwdTab + sizeof(float) * ((tab != nullptr ? kTabCopies * fwd_tab_stride(p.n_tiles) : 0) + p.n_tiles * kAttnTile) +
-                   sizeof(int) * p.n_tiles + 1024;
-  B200_CHECK_ARG(T >= 1 && smem <= 232448 - 1024, "attn_fwd: T=%d out of range (needs %d bytes of shared memory)", T, smem);
+  B200_CHECK_ARG(T >= 1, "attn_fwd: T=%d out of range", T);
+  const int smem = kFwdSmem;
   if (make_qkv_tmap(&tm, qkv, T, B, 3 * D, kAttnTile)) return -3;
   p.scale = scale;
   p.gate = gate; p.tab = tab; p.key_pad = key_pad;

@@ -117,6 +117,10 @@ __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_
 __device__ __forceinline__ void cp_async_8(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
+// 4-byte asynchronous global -> shared copy that writes zero instead when !valid (gsrc is then not read)
+__device__ __forceinline__ void cp_async_4_zfill(void* smem_dst, const void* gsrc, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(valid ? 4 : 0) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 

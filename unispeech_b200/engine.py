@@ -619,10 +619,6 @@ class Engine:
         p_h = d.p if d is not None else 0.0
         p_a = d.p_attn if d is not None else 0.0
         p_act = d.p_act if d is not None else 0.0
-        t_fused = 2048   # longest input of the fused attention backward (its shared-memory tables grow with T)
-        if p_a > 0 and T > t_fused:
-            raise NotImplementedError(f"attention_dropout > 0 is implemented in the fused attention kernels for T <= {t_fused} frames "
-                                      f"(got T={T}); set attention_dropout=0 for longer inputs")
         st = dict(x=x, drop=d)
         rag = self.ragged_valid if pad_u8 is not None else None   # int32 [B] valid frames (ragged batch) or None
         want_gate = tab is not None and cfg.gru_rel_pos
@@ -771,20 +767,16 @@ class Engine:
         delta = f(B, H, T)
         gate = st["gate"]
         dgate = f(B, H, T) if tab is not None else None
-        if T <= 2048:
-            key = (B, T, D)
-            if getattr(self, "_dq_acc_key", None) != key:  # fp32 dQ accumulator: zero on entry, re-zeroed by the kernel
-                self._dq_acc = torch.zeros(B, T, D, dtype=torch.float32, device=dev)
-                self._dq_acc_key = key
-            if p_a > 0:
-                ops.attn_bwd_fused_dropout(st["qkv"], st["ao"], dao, gate, tab, pad, st["lse"], delta, self._dq_acc, dqkv, dgate,
-                                           dtab if tab is not None else None, B, T, H, 64 ** -0.5, p_a, st["dmask"])
-            else:
-                ops.attn_bwd_fused(st["qkv"], st["ao"], dao, gate, tab, pad, st["lse"], delta, self._dq_acc, dqkv, dgate,
-                                   dtab if tab is not None else None, B, T, H, 64 ** -0.5)
+        key = (B, T, D)
+        if getattr(self, "_dq_acc_key", None) != key:  # fp32 dQ accumulator: zero on entry, re-zeroed by the kernel
+            self._dq_acc = torch.zeros(B, T, D, dtype=torch.float32, device=dev)
+            self._dq_acc_key = key
+        if p_a > 0:
+            ops.attn_bwd_fused_dropout(st["qkv"], st["ao"], dao, gate, tab, pad, st["lse"], delta, self._dq_acc, dqkv, dgate,
+                                       dtab if tab is not None else None, B, T, H, 64 ** -0.5, p_a, st["dmask"])
         else:
-            ops.attn_bwd(st["qkv"], st["ao"], dao, gate, tab, pad, st["lse"], delta, dqkv, dgate,
-                         dtab if tab is not None else None, B, T, H, 64 ** -0.5)
+            ops.attn_bwd_fused(st["qkv"], st["ao"], dao, gate, tab, pad, st["lse"], delta, self._dq_acc, dqkv, dgate,
+                               dtab if tab is not None else None, B, T, H, 64 ** -0.5)
         ops.colsum(dqkv, T * 3 * D, 3 * D, T, B, 3 * D, g(a.q_proj.bias).view(-1), valid=rag)  # q,k,v bias grads are adjacent in the flat buffer
         attn_in = st["xn"] if pre_ln else x
         dxg = None
