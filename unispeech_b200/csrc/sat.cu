@@ -243,10 +243,12 @@ __global__ void __launch_bounds__(256) f32_to_bf16_rows_kernel(const float* __re
 
 // Gumbel(0,1) sample of element `ctr` from the counter-based hash of dropout.cuh: u = (bits + 0.5) / 2^32 in (0,1), g = -log(-log u).
 // (F.gumbel_softmax draws -log(Exponential(1)) from torch's Philox stream, which no other implementation reproduces; the oracle
-// restates THIS generator, exactly like the dropout masks.)
+// restates THIS generator, exactly like the dropout masks.)  The accurate logf, not __logf: __logf's error near 1 is absolute
+// (up to 2^-21.4), while -log u there is as small as 6e-8, so the largest noise values -- the ones that pick the code and
+// dominate the soft sample's gradient -- would be off by percents.
 __device__ __forceinline__ float gumbel_noise(uint32_t k0, uint32_t k1, uint32_t ctr) {
   const float u = (static_cast<float>(drop_bits(k0, k1, ctr)) + 0.5f) * 2.3283064365386963e-10f;
-  return -__logf(-__logf(fminf(u, 0.99999994f)));
+  return -logf(-logf(fminf(u, 0.99999994f)));
 }
 
 // ---------------------------------------------------------------- Gumbel vector quantizer, hard codes
