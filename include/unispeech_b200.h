@@ -228,11 +228,14 @@ uint32_t b200s_dropout_bits(uint32_t key0, uint32_t key1, uint32_t ctr);
 uint32_t b200s_dropout_row_key(uint32_t key, uint32_t row, int which);
 uint32_t b200s_dropout_threshold16(float p);
 
-/* x[b,t,:] = mask_emb where mask[b,t]; = 0 where pad[b,t]   (apply_mask WavLM/WavLM.py:285-286; x[padding_mask]=0 :574-575) */
+/* x[b,t,:] = mask_emb where mask[b,t]; = 0 where pad[b,t]   (apply_mask WavLM/WavLM.py:285-286; x[padding_mask]=0 :574-575);
+ * then x[b,:,c] = 0 where chan_mask[b,c] (uint8 [B, D], the channel mask of apply_mask :288-307, or NULL).  Backward: dx = 0
+ * wherever the forward overwrote x; dmask_emb[c] (+=) sums dx over masked, unpadded frames whose channel c is not masked.
+ * mask, pad and chan_mask may each be NULL. */
 int b200s_frame_mask_fwd(void* x, long long x_bs, long long x_rs, int T, int B, int D, const uint8_t* mask,
-                         const uint8_t* pad, const float* mask_emb, b200s_stream stream);
+                         const uint8_t* pad, const float* mask_emb, const uint8_t* chan_mask, b200s_stream stream);
 int b200s_frame_mask_bwd(void* dx, long long x_bs, long long x_rs, int T, int B, int D, const uint8_t* mask,
-                         const uint8_t* pad, float* dmask_emb, b200s_stream stream);
+                         const uint8_t* pad, float* dmask_emb, const uint8_t* chan_mask, b200s_stream stream);
 
 /* gate[b,h,t] of gru_rel_pos from the RAW layer input (WavLM/modules.py:523-533) and its backward */
 int b200s_gate_fwd(const void* x, long long x_bs, long long x_rs, int T, int B, int H, const float* grep_w,
@@ -247,23 +250,27 @@ int b200s_relpos_table_bwd(const float* dtab, const int* lut, int n, int H, floa
 
 /* ============================ conv layer 0 (csrc/conv0.cu) ============================ */
 
-/* Conv1d(1,C,k,stride s, no bias) + GroupNorm(C,C) (mode 0) or LayerNorm over channels (mode 1) + GELU on the raw
+/* Conv1d(1,C,k,stride s, optional bias) + GroupNorm(C,C) (mode 0) or LayerNorm over channels (mode 1) + GELU on the raw
  * waveform (WavLM/WavLM.py:400-426).  wav fp32 [B,L]; w fp32 [C,1,k]; out bf16 channels-last.  stats: fp64 [B,C,2]
- * (mode 0);  fmean/frstd: fp32 [B,T] (mode 1).  C in {64, 512}. */
+ * (mode 0);  fmean/frstd: fp32 [B,T] (mode 1).  C in {64, 512}.  bias fp32 [C] or NULL (conv_bias=True): added before the
+ * LayerNorm in mode 1; in mode 0 the per-(utterance, channel) GroupNorm removes a per-channel constant exactly, so the bias is
+ * not applied there and its gradient is zero.  Backward: dbias (+=, mode 1, needs bias) = sum over (b, t) of the gradient at
+ * the raw convolution output; mode 0 leaves it untouched. */
 int b200s_conv0_fwd(const float* wav, long long L, int B, int T, int C, int k, int s, const float* w,
                     const float* gamma, const float* beta, int mode, double* stats, float* fmean, float* frstd,
-                    void* out, long long out_bs, b200s_stream stream);
+                    void* out, long long out_bs, const float* bias, b200s_stream stream);
 int b200s_conv0_bwd(const float* wav, long long L, int B, int T, int C, int k, int s, const float* w,
                     const float* gamma, const float* beta, int mode, const double* stats, float* bstats,
                     const float* fmean, const float* frstd, const void* da, long long da_bs, float* dw,
-                    float* dgamma, float* dbeta, b200s_stream stream);
+                    float* dgamma, float* dbeta, const float* bias, float* dbias, b200s_stream stream);
 /* Same, with a bf16 workspace [B, ws_bs/C rows >= T, C] for the gradient w.r.t. the raw convolution output (mode 1 only; may
  * alias `da`, which is then consumed): the LayerNorm-mode backward becomes one pass over the frames plus one streaming
  * weight-gradient reduction instead of two full recomputing passes. */
 int b200s_conv0_bwd_ws(const float* wav, long long L, int B, int T, int C, int k, int s, const float* w,
                        const float* gamma, const float* beta, int mode, const double* stats, float* bstats,
                        const float* fmean, const float* frstd, const void* da, long long da_bs, void* dconv_ws,
-                       long long ws_bs, float* dw, float* dgamma, float* dbeta, b200s_stream stream);
+                       long long ws_bs, float* dw, float* dgamma, float* dbeta, const float* bias, float* dbias,
+                       b200s_stream stream);
 
 /* ============================ parameter preparation (csrc/prep.cu) ============================ */
 

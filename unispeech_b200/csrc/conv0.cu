@@ -1,4 +1,4 @@
-// First layer of ConvFeatureExtractionModel: Conv1d(1, C, k=10, stride=5, bias=False) on the raw waveform, fused with its
+// First layer of ConvFeatureExtractionModel: Conv1d(1, C, k=10, stride=5, bias=conv_bias) on the raw waveform, fused with its
 // normalisation and GELU (WavLM/WavLM.py:400-426,485-504).  Cin = 1 makes this HBM-bound (20 flop per output element),
 // so it is a CUDA-core kernel: one warp per output frame, each lane owns C/32 channels, weights in shared memory,
 // channels-last bf16 output [B, Tpad, C].  The conv output is never stored: statistics passes and the backward
@@ -91,6 +91,16 @@ __device__ __forceinline__ void load_frame(const __nv_bfloat16* in, float* v, in
   }
 }
 
+// conv[c] += bias[c] for this lane's channels (conv_bias=True, WavLM/WavLM.py:400-403)
+template <int C>
+__device__ __forceinline__ void add_bias(const float* __restrict__ bias, int lane, float* acc) {
+  using M = LaneMap<C>;
+#pragma unroll
+  for (int g = 0; g < M::NG; ++g)
+#pragma unroll
+    for (int v = 0; v < M::V; ++v) acc[g * M::V + v] += bias[M::chan(lane, g, v)];
+}
+
 // block-wide reduction of per-lane channel partials (acc[CPL] per warp) into dst via atomics
 template <int C, typename T>
 __device__ __forceinline__ void block_channel_atomic(const float* acc, T* dst, int stride, float* red /*[8][C]*/) {
@@ -163,7 +173,7 @@ __global__ void __launch_bounds__(256) conv0_fwd_kernel(const float* __restrict_
                                                         const float* __restrict__ beta,
                                                         const double* __restrict__ stats, float* __restrict__ fmean,
                                                         float* __restrict__ frstd, __nv_bfloat16* __restrict__ out,
-                                                        long long out_bs) {
+                                                        long long out_bs, const float* __restrict__ bias) {
   pdl_grid_sync();
   using M = LaneMap<C>;
   extern __shared__ float smem[];
@@ -188,6 +198,7 @@ __global__ void __launch_bounds__(256) conv0_fwd_kernel(const float* __restrict_
 #pragma unroll
       for (int i = 0; i < M::CPL; ++i) acc[i] = gelu_f((acc[i] - mean[i]) * rstd[i] * g[i] + be[i]);
     } else {
+      if (bias != nullptr) add_bias<C>(bias, lane, acc);
       float su = 0.f;
 #pragma unroll
       for (int i = 0; i < M::CPL; ++i) su += acc[i];
@@ -275,7 +286,8 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
                                                            const float* __restrict__ fmean, const float* __restrict__ frstd,
                                                            const __nv_bfloat16* __restrict__ da, long long da_bs, int j0,
                                                            float* __restrict__ dw, float* __restrict__ dgamma,
-                                                           float* __restrict__ dbeta) {
+                                                           float* __restrict__ dbeta, const float* __restrict__ bias,
+                                                           float* __restrict__ dbias) {
   pdl_grid_sync();
   using M = LaneMap<C>;
   extern __shared__ float smem[];
@@ -286,7 +298,7 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
   const int b = blockIdx.y;
   const float* wav_b = wav + static_cast<long long>(b) * L;
   float g[M::CPL], be[M::CPL], mean[M::CPL], rstd[M::CPL], m1[M::CPL], m2[M::CPL];
-  float ag[M::CPL], ab[M::CPL];
+  float ag[M::CPL], ab[M::CPL], adb[M::CPL];
   float acc_dw[JT][M::CPL];
 #pragma unroll
   for (int gi = 0; gi < M::NG; ++gi)
@@ -303,7 +315,7 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
   if (MODE == 0) gn_mean_rstd<C>(stats + static_cast<long long>(b) * C * 2, T, lane, mean, rstd);
 #pragma unroll
   for (int i = 0; i < M::CPL; ++i) {
-    ag[i] = ab[i] = 0.f;
+    ag[i] = ab[i] = adb[i] = 0.f;
 #pragma unroll
     for (int j = 0; j < JT; ++j) acc_dw[j][i] = 0.f;
   }
@@ -319,6 +331,7 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
         d[i] = rstd[i] * (dxh - m1[i] - xh * m2[i]);
       }
     } else {
+      if (bias != nullptr) add_bias<C>(bias, lane, acc);
       const float m = fmean[static_cast<long long>(b) * T + t], r = frstd[static_cast<long long>(b) * T + t];
       float q1 = 0.f, q2 = 0.f;
 #pragma unroll
@@ -336,7 +349,10 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
       q1 = warp_sum(q1) * (1.0f / C);
       q2 = warp_sum(q2) * (1.0f / C);
 #pragma unroll
-      for (int i = 0; i < M::CPL; ++i) d[i] = r * (d[i] - q1 - acc[i] * q2);
+      for (int i = 0; i < M::CPL; ++i) {
+        d[i] = r * (d[i] - q1 - acc[i] * q2);
+        adb[i] += d[i];  // d bias: the tap whose input is 1
+      }
     }
 #pragma unroll
     for (int j = 0; j < JT; ++j) {
@@ -351,6 +367,7 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
   if (MODE == 1 && j0 == 0) {
     block_channel_atomic<C, float>(ag, dgamma, 1, red);
     block_channel_atomic<C, float>(ab, dbeta, 1, red);
+    if (dbias != nullptr) block_channel_atomic<C, float>(adb, dbias, 1, red);
   }
 }
 
@@ -367,7 +384,7 @@ __global__ void __launch_bounds__(256, 2) conv0_ln_bwd_dconv_kernel(const float*
                                                                     const float* __restrict__ fmean, const float* __restrict__ frstd,
                                                                     const __nv_bfloat16* da, long long da_bs, __nv_bfloat16* dconv,
                                                                     long long dc_bs, float* __restrict__ dgamma,
-                                                                    float* __restrict__ dbeta) {
+                                                                    float* __restrict__ dbeta, const float* __restrict__ bias) {
   pdl_grid_sync();
   using M = LaneMap<C>;
   extern __shared__ float smem[];
@@ -391,6 +408,7 @@ __global__ void __launch_bounds__(256, 2) conv0_ln_bwd_dconv_kernel(const float*
   for (int t = blockIdx.x * 8 + warp; t < T; t += gridDim.x * 8) {
     float acc[M::CPL], d[M::CPL];
     conv_frame<C>(wav_b, L, t, k, s, w_s, lane, acc, nullptr);
+    if (bias != nullptr) add_bias<C>(bias, lane, acc);
     load_frame<C>(da + b * da_bs + static_cast<long long>(t) * C, d, lane);
     const float m = fmean[static_cast<long long>(b) * T + t], r = frstd[static_cast<long long>(b) * T + t];
     float q1 = 0.f, q2 = 0.f;
@@ -419,7 +437,7 @@ __global__ void __launch_bounds__(256, 2) conv0_ln_bwd_dconv_kernel(const float*
 template <int C, int K>
 __global__ void __launch_bounds__(256) conv0_dw_from_dconv_kernel(const float* __restrict__ wav, long long L, int T, int k, int s,
                                                                   const __nv_bfloat16* __restrict__ dconv, long long dc_bs,
-                                                                  float* __restrict__ dw) {
+                                                                  float* __restrict__ dw, float* __restrict__ dbias) {
   pdl_grid_sync();
   using M = LaneMap<C>;
   extern __shared__ float smem[];
@@ -427,11 +445,13 @@ __global__ void __launch_bounds__(256) conv0_dw_from_dconv_kernel(const float* _
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int b = blockIdx.y;
   const float* wav_b = wav + static_cast<long long>(b) * L;
-  float acc_dw[K][M::CPL];
+  float acc_dw[K][M::CPL], acc_db[M::CPL];
 #pragma unroll
-  for (int j = 0; j < K; ++j)
+  for (int i = 0; i < M::CPL; ++i) {
+    acc_db[i] = 0.f;
 #pragma unroll
-    for (int i = 0; i < M::CPL; ++i) acc_dw[j][i] = 0.f;
+    for (int j = 0; j < K; ++j) acc_dw[j][i] = 0.f;
+  }
   for (int t = blockIdx.x * 8 + warp; t < T; t += gridDim.x * 8) {
     float d[M::CPL];
     load_frame<C>(dconv + b * dc_bs + static_cast<long long>(t) * C, d, lane);
@@ -443,10 +463,15 @@ __global__ void __launch_bounds__(256) conv0_dw_from_dconv_kernel(const float* _
 #pragma unroll
       for (int i = 0; i < M::CPL; ++i) acc_dw[j][i] = fmaf(d[i], xj, acc_dw[j][i]);
     }
+    if (dbias != nullptr) {  // the tap whose input is 1
+#pragma unroll
+      for (int i = 0; i < M::CPL; ++i) acc_db[i] += d[i];
+    }
   }
 #pragma unroll
   for (int j = 0; j < K; ++j)
     if (j < k) block_channel_atomic<C, float>(acc_dw[j], dw + j, k, red);  // dw layout [C, 1, k]
+  if (dbias != nullptr) block_channel_atomic<C, float>(acc_db, dbias, 1, red);
 }
 
 int conv0_gn_stats_launch(const float* wav, long long L, int B, int T, int C, int k, int s, const float* w, double* stats,
@@ -485,7 +510,7 @@ extern "C" {
 // (fmean/frstd: fp32 [B,T] outputs).  wav fp32 [B,L]; w fp32 [C,1,k]; out bf16 [B, out_bs/C rows, C].
 int b200s_conv0_fwd(const float* wav, long long L, int B, int T, int C, int k, int s, const float* w, const float* gamma,
                     const float* beta, int mode, double* stats, float* fmean, float* frstd, void* out, long long out_bs,
-                    b200s_stream stream) {
+                    const float* bias, b200s_stream stream) {
   B200_CHECK_ARG(wav && w && gamma && beta && out, "conv0_fwd: null pointer");
   B200_CHECK_ARG(k <= kMaxTaps && k >= 1, "conv0_fwd: kernel size %d > %d", k, kMaxTaps);
   B200_CHECK_ARG((mode == 0 && stats) || (mode == 1 && fmean && frstd), "conv0_fwd: missing statistics buffers");
@@ -494,12 +519,15 @@ int b200s_conv0_fwd(const float* wav, long long L, int B, int T, int C, int k, i
   DISPATCH_C(C, {
     const size_t sm_w = sizeof(float) * kMaxTaps * kC, sm_red = sizeof(float) * 8 * kC;
     if (mode == 0) {
+      // GroupNorm(C, C) normalises every (utterance, channel) over all its frames: a per-channel constant shifts that mean by
+      // bias[c] and leaves the variance unchanged, so the bias cancels exactly -- it is not applied (and gets no gradient)
       (void)sm_red;
+      (void)bias;
       if (int rc = conv0_gn_stats_launch(wav, L, B, T, kC, k, s, w, stats, st)) return rc;  // analytic, from the autocorrelation
       return conv0_gn_fwd_apply_launch(wav, L, B, T, kC, k, s, w, gamma, beta, stats, out, out_bs, st);
     } else {
       B200_CHECK_CUDA(launch_pdl(conv0_fwd_kernel<kC, 1>, dim3(grid), dim3(256), sm_w, st, wav, L, T, k, s, w, gamma, beta, nullptr, fmean, frstd,
-                                                      static_cast<__nv_bfloat16*>(out), out_bs));
+                                                      static_cast<__nv_bfloat16*>(out), out_bs, bias));
     }
     B200_CHECK_LAUNCH();
   })
@@ -513,10 +541,11 @@ int b200s_conv0_fwd(const float* wav, long long L, int B, int T, int C, int k, i
 int b200s_conv0_bwd_ws(const float* wav, long long L, int B, int T, int C, int k, int s, const float* w, const float* gamma,
                        const float* beta, int mode, const double* stats, float* bstats, const float* fmean,
                        const float* frstd, const void* da, long long da_bs, void* dconv_ws, long long ws_bs, float* dw,
-                       float* dgamma, float* dbeta, b200s_stream stream) {
+                       float* dgamma, float* dbeta, const float* bias, float* dbias, b200s_stream stream) {
   B200_CHECK_ARG(wav && w && gamma && beta && da && dw && dgamma && dbeta, "conv0_bwd: null pointer");
   B200_CHECK_ARG(k <= kMaxTaps && k >= 1, "conv0_bwd: kernel size %d > %d", k, kMaxTaps);
   B200_CHECK_ARG((mode == 0 && stats && bstats) || (mode == 1 && fmean && frstd), "conv0_bwd: missing statistics");
+  B200_CHECK_ARG(!dbias || bias, "conv0_bwd: dbias needs bias");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   dim3 grid(conv0_grid_x(T), B);
   const __nv_bfloat16* dap = static_cast<const __nv_bfloat16*>(da);
@@ -524,6 +553,7 @@ int b200s_conv0_bwd_ws(const float* wav, long long L, int B, int T, int C, int k
     const size_t sm = sizeof(float) * (kMaxTaps + 8) * kC;
     constexpr int JT = 5;
     if (mode == 0) {
+      // (GroupNorm mode: the bias cancels in the forward pass, its gradient is exactly zero -- dbias is left untouched)
       (void)grid;
       if (int rc = conv0_gn_bwd_launch(wav, L, B, T, kC, k, s, w, gamma, beta, stats, bstats, da, da_bs, dw, dgamma, dbeta, st))
         return rc;
@@ -531,18 +561,18 @@ int b200s_conv0_bwd_ws(const float* wav, long long L, int B, int T, int C, int k
       B200_CHECK_CUDA(cudaFuncSetAttribute(conv0_ln_bwd_dconv_kernel<kC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            static_cast<int>(sm)));
       B200_CHECK_CUDA(launch_pdl(conv0_ln_bwd_dconv_kernel<kC>, dim3(grid), dim3(256), sm, st, wav, L, T, k, s, w, gamma, beta, fmean,
-                                 frstd, dap, da_bs, static_cast<__nv_bfloat16*>(dconv_ws), ws_bs, dgamma, dbeta));
+                                 frstd, dap, da_bs, static_cast<__nv_bfloat16*>(dconv_ws), ws_bs, dgamma, dbeta, bias));
       B200_CHECK_LAUNCH();
       const size_t sm_red = sizeof(float) * 8 * kC;
       B200_CHECK_CUDA(launch_pdl(conv0_dw_from_dconv_kernel<kC, 10>, dim3(grid), dim3(256), sm_red, st, wav, L, T, k, s,
-                                 static_cast<const __nv_bfloat16*>(dconv_ws), ws_bs, dw));
+                                 static_cast<const __nv_bfloat16*>(dconv_ws), ws_bs, dw, dbias));
       B200_CHECK_LAUNCH();
     } else {
       B200_CHECK_CUDA(cudaFuncSetAttribute(conv0_bwd_dw_kernel<kC, 1, JT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            static_cast<int>(sm)));
       for (int j0 = 0; j0 < k; j0 += JT) {
         B200_CHECK_CUDA(launch_pdl(conv0_bwd_dw_kernel<kC, 1, JT>, dim3(grid), dim3(256), sm, st, wav, L, T, k, s, w, gamma, beta, nullptr, nullptr, fmean,
-                                                             frstd, dap, da_bs, j0, dw, dgamma, dbeta));
+                                                             frstd, dap, da_bs, j0, dw, dgamma, dbeta, bias, dbias));
         B200_CHECK_LAUNCH();
       }
     }
@@ -553,9 +583,9 @@ int b200s_conv0_bwd_ws(const float* wav, long long L, int B, int T, int C, int k
 int b200s_conv0_bwd(const float* wav, long long L, int B, int T, int C, int k, int s, const float* w, const float* gamma,
                     const float* beta, int mode, const double* stats, float* bstats, const float* fmean,
                     const float* frstd, const void* da, long long da_bs, float* dw, float* dgamma, float* dbeta,
-                    b200s_stream stream) {
+                    const float* bias, float* dbias, b200s_stream stream) {
   return b200s_conv0_bwd_ws(wav, L, B, T, C, k, s, w, gamma, beta, mode, stats, bstats, fmean, frstd, da, da_bs, nullptr, 0, dw,
-                            dgamma, dbeta, stream);
+                            dgamma, dbeta, bias, dbias, stream);
 }
 
 }  // extern "C"

@@ -969,10 +969,19 @@ __global__ void __launch_bounds__(256) grad_multiply_kernel(__nv_bfloat16* __res
 // ------------------------------------------------------------------------------------------------ frame masking
 // x[b,t,:] = 0 where pad[b,t];  = mask_emb where mask[b,t] and not pad   (apply_mask WavLM/WavLM.py:285-286, then
 // x[padding_mask] = 0 WavLM/WavLM.py:574-575).  In place on a [B,T,D] view.
+// CHAN: channel masking, the second half of apply_mask (WavLM/WavLM.py:288-307): x[b,:,c] = 0 where chan[b,c], applied after
+// the mask_emb line, so a time-masked frame loses its masked channels too.  Every unpadded row is visited then; a bf16 pair
+// is cleared by bit masking, so the values that survive are the input's bits.
+__device__ __forceinline__ uint32_t chan_keep_bits(uint16_t cm) {  // cm: chan[c] in the low byte, chan[c + 1] in the high byte
+  return ((cm & 0x00FFu) ? 0xFFFF0000u : 0xFFFFFFFFu) & ((cm & 0xFF00u) ? 0x0000FFFFu : 0xFFFFFFFFu);
+}
+
+template <bool CHAN>
 __global__ void __launch_bounds__(256) frame_mask_fwd_kernel(__nv_bfloat16* __restrict__ x, RowView xv, int D,
                                                              long long rows, const uint8_t* __restrict__ mask,
                                                              const uint8_t* __restrict__ pad,
-                                                             const float* __restrict__ mask_emb) {
+                                                             const float* __restrict__ mask_emb,
+                                                             const uint8_t* __restrict__ chan) {
   pdl_grid_sync();
   const int lane = threadIdx.x & 31;
   const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
@@ -980,19 +989,38 @@ __global__ void __launch_bounds__(256) frame_mask_fwd_kernel(__nv_bfloat16* __re
   for (long long r = warp_global; r < rows; r += nwarps) {
     const bool p = pad != nullptr && pad[r] != 0;
     const bool m = mask != nullptr && mask[r] != 0;
-    if (!p && !m) continue;
-    __nv_bfloat16* xr = x + xv.off(r);
-    for (int c = lane * 2; c < D; c += 64) {
-      const uint32_t w = p ? 0u : pack_bf16x2(mask_emb[c], mask_emb[c + 1]);
-      *reinterpret_cast<uint32_t*>(xr + c) = w;
+    if constexpr (!CHAN) {
+      if (!p && !m) continue;
+      __nv_bfloat16* xr = x + xv.off(r);
+      for (int c = lane * 2; c < D; c += 64) {
+        const uint32_t w = p ? 0u : pack_bf16x2(mask_emb[c], mask_emb[c + 1]);
+        *reinterpret_cast<uint32_t*>(xr + c) = w;
+      }
+    } else {
+      __nv_bfloat16* xr = x + xv.off(r);
+      const uint8_t* cr = chan + static_cast<long long>(static_cast<unsigned>(r) / static_cast<unsigned>(xv.rows_per_batch)) * D;
+      for (int c = lane * 2; c < D; c += 64) {
+        uint32_t* px = reinterpret_cast<uint32_t*>(xr + c);
+        if (p) {
+          *px = 0u;
+          continue;
+        }
+        const uint16_t cm = *reinterpret_cast<const uint16_t*>(cr + c);
+        if (!m && cm == 0) continue;  // untouched pair
+        const uint32_t w = m ? pack_bf16x2(mask_emb[c], mask_emb[c + 1]) : *px;
+        *px = w & chan_keep_bits(cm);
+      }
     }
   }
 }
 // backward: d mask_emb += sum over masked & unpadded rows of dx;  dx rows that were overwritten get zero gradient.
+// CHAN: entries of masked channels were overwritten too: their dx is zero and they add nothing to d mask_emb.
+template <bool CHAN>
 __global__ void __launch_bounds__(256) frame_mask_bwd_kernel(__nv_bfloat16* __restrict__ dx, RowView xv, int D,
                                                              long long rows, const uint8_t* __restrict__ mask,
                                                              const uint8_t* __restrict__ pad,
-                                                             float* __restrict__ dmask_emb) {
+                                                             float* __restrict__ dmask_emb,
+                                                             const uint8_t* __restrict__ chan) {
   pdl_grid_sync();
   const int lane = threadIdx.x & 31;
   const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
@@ -1006,18 +1034,41 @@ __global__ void __launch_bounds__(256) frame_mask_bwd_kernel(__nv_bfloat16* __re
   for (long long r = warp_global; r < rows; r += nwarps) {
     const bool p = pad != nullptr && pad[r] != 0;
     const bool m = mask != nullptr && mask[r] != 0;
-    if (!p && !m) continue;
-    __nv_bfloat16* xr = dx + xv.off(r);
+    if constexpr (!CHAN) {
+      if (!p && !m) continue;
+      __nv_bfloat16* xr = dx + xv.off(r);
 #pragma unroll
-    for (int i = 0; i < kMaxIter; ++i) {
-      const int c = lane * 2 + 64 * i;
-      if (c < D) {
-        if (!p) {
-          const float2 f = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(xr + c));
-          acc[i][0] += f.x;
-          acc[i][1] += f.y;
+      for (int i = 0; i < kMaxIter; ++i) {
+        const int c = lane * 2 + 64 * i;
+        if (c < D) {
+          if (!p) {
+            const float2 f = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(xr + c));
+            acc[i][0] += f.x;
+            acc[i][1] += f.y;
+          }
+          *reinterpret_cast<uint32_t*>(xr + c) = 0u;
         }
-        *reinterpret_cast<uint32_t*>(xr + c) = 0u;
+      }
+    } else {
+      __nv_bfloat16* xr = dx + xv.off(r);
+      const uint8_t* cr = chan + static_cast<long long>(static_cast<unsigned>(r) / static_cast<unsigned>(xv.rows_per_batch)) * D;
+#pragma unroll
+      for (int i = 0; i < kMaxIter; ++i) {
+        const int c = lane * 2 + 64 * i;
+        if (c < D) {
+          uint32_t* px = reinterpret_cast<uint32_t*>(xr + c);
+          const uint16_t cm = p ? 0xFFFFu : *reinterpret_cast<const uint16_t*>(cr + c);
+          if (m && !p) {
+            const float2 f = unpack_bf16x2(*px);
+            acc[i][0] += (cm & 0x00FFu) ? 0.f : f.x;
+            acc[i][1] += (cm & 0xFF00u) ? 0.f : f.y;
+          }
+          if (m || p) {
+            *px = 0u;
+          } else if (cm != 0) {
+            *px &= chan_keep_bits(cm);
+          }
+        }
       }
     }
   }
@@ -1533,28 +1584,30 @@ int b200s_grad_multiply(void* g, long long g_bs, long long g_rs, const void* x, 
 }
 
 int b200s_frame_mask_fwd(void* x, long long x_bs, long long x_rs, int T, int B, int D, const uint8_t* mask,
-                         const uint8_t* pad, const float* mask_emb, b200s_stream stream) {
+                         const uint8_t* pad, const float* mask_emb, const uint8_t* chan_mask, b200s_stream stream) {
   B200_CHECK_ARG(x, "frame_mask_fwd: null pointer");
   B200_CHECK_ARG(D % 2 == 0, "frame_mask_fwd: D must be even");
   B200_CHECK_ARG(!mask || mask_emb, "frame_mask_fwd: mask needs mask_emb");
-  if (!mask && !pad) return 0;
+  if (!mask && !pad && !chan_mask) return 0;
   const long long rows = static_cast<long long>(T) * B;
   RowView xv{x_bs, x_rs, T};
-  B200_CHECK_CUDA(launch_pdl(frame_mask_fwd_kernel, dim3(row_grid(rows, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<__nv_bfloat16*>(x), xv, D, rows, mask, pad, mask_emb));
+  auto kern = chan_mask ? frame_mask_fwd_kernel<true> : frame_mask_fwd_kernel<false>;
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(row_grid(rows, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream),
+      static_cast<__nv_bfloat16*>(x), xv, D, rows, mask, pad, mask_emb, chan_mask));
   B200_CHECK_LAUNCH();
   return 0;
 }
 
 int b200s_frame_mask_bwd(void* dx, long long x_bs, long long x_rs, int T, int B, int D, const uint8_t* mask,
-                         const uint8_t* pad, float* dmask_emb, b200s_stream stream) {
+                         const uint8_t* pad, float* dmask_emb, const uint8_t* chan_mask, b200s_stream stream) {
   B200_CHECK_ARG(dx, "frame_mask_bwd: null pointer");
   B200_CHECK_ARG(D <= 2048 && D % 2 == 0, "frame_mask_bwd: D=%d must be even and <= 2048", D);
-  if (!mask && !pad) return 0;
+  if (!mask && !pad && !chan_mask) return 0;
   const long long rows = static_cast<long long>(T) * B;
   RowView xv{x_bs, x_rs, T};
-  B200_CHECK_CUDA(launch_pdl(frame_mask_bwd_kernel, dim3(row_grid(rows, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<__nv_bfloat16*>(dx), xv, D, rows, mask, pad, dmask_emb));
+  auto kern = chan_mask ? frame_mask_bwd_kernel<true> : frame_mask_bwd_kernel<false>;
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(row_grid(rows, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream),
+      static_cast<__nv_bfloat16*>(dx), xv, D, rows, mask, pad, dmask_emb, chan_mask));
   B200_CHECK_LAUNCH();
   return 0;
 }

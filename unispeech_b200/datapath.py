@@ -22,7 +22,10 @@ _SITE_MASK = 0x7F000003
 def span_mask_device(B: int, T: int, device, mask_prob: float, mask_length: int, min_masks: int = 2,
                      padding_mask: Optional[torch.Tensor] = None, seed: Optional[int] = None) -> torch.Tensor:
     """bool [B, T] on `device`: the masked frames of one batch (static span length, overlapping spans -- the released recipes).
-    `padding_mask`: bool [B, T] frame-level mask ON THE DEVICE (padded tail True) or None.  No host synchronisation."""
+    `padding_mask`: bool [B, T] frame-level mask ON THE DEVICE (padded tail True) or None.  No host synchronisation.
+    The same call draws the channel mask of apply_mask (WavLM/WavLM.py:288-307) when given the channel axis and the reference's
+    channel arguments: `span_mask_device(B, encoder_embed_dim, device, mask_channel_prob, mask_channel_length, min_masks=0)`
+    (no padding mask; T <= 4096 covers every released width)."""
     if seed is None:
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())
     valid = None

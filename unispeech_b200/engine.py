@@ -351,6 +351,7 @@ class Engine:
             cv = conv_valid_rows(self.conv_valid_last, convs, geo.T).to(dev, non_blocking=True)
         st["cv"] = cv
         vrow = (lambda i: cv[i]) if cv is not None else (lambda i: None)
+        cbias = [blk[0].bias for blk in m.feature_extractor.conv_layers]  # conv_bias=True: fp32 [C] per layer, else None
         blk0 = m.feature_extractor.conv_layers[0]
         _, k0, s0 = convs[0]
         a0 = torch.empty(B, geo.Tp[0], C, dtype=BF, device=dev)
@@ -359,7 +360,7 @@ class Engine:
             fmean = torch.empty(B, geo.T[0], dtype=torch.float32, device=dev)
             frstd = torch.empty(B, geo.T[0], dtype=torch.float32, device=dev)
             ops.conv0_fwd(wav, L_, B, geo.T[0], C, k0, s0, blk0[0].weight, norm0.weight, norm0.bias, 1, None, fmean, frstd,
-                          a0, geo.Tp[0] * C)
+                          a0, geo.Tp[0] * C, bias=cbias[0])
             st["stats0"] = (fmean, frstd)
         else:
             stats = torch.empty(B * C * 2 + B * 128, dtype=torch.float64, device=dev)  # per-(b,c) sums + autocorrelation
@@ -377,7 +378,8 @@ class Engine:
             out = torch.empty(B, Tpi, C, dtype=BF, device=dev)
             if ln_mode:
                 y = torch.empty(B, Tpi, C, dtype=BF, device=dev)
-                ops.gemm_rows(a_prev, geo.Tp[i - 1] * C, s * C, Ti, B, k * C, self.wf[i], C, y, Tpi * C, C, None, valid=vrow(i))
+                epi = L.make_epilogue(bias=cbias[i]) if cbias[i] is not None else None  # bias before the LayerNorm
+                ops.gemm_rows(a_prev, geo.Tp[i - 1] * C, s * C, Ti, B, k * C, self.wf[i], C, y, Tpi * C, C, epi, valid=vrow(i))
                 ln = m.feature_extractor.conv_layers[i][2][1]
                 mean = torch.empty(B * Ti, dtype=torch.float32, device=dev)
                 rstd = torch.empty(B * Ti, dtype=torch.float32, device=dev)
@@ -385,7 +387,8 @@ class Engine:
                 st["y"].append(y); st["mean"].append(mean); st["rstd"].append(rstd)
             else:
                 y = torch.empty(B, Tpi, C, dtype=BF, device=dev) if save else None
-                epi = L.make_epilogue(gelu=2, out_pre=y, pre_bs=Tpi * C, pre_ld=C)  # y = gelu'(conv output), used by backward
+                # y = gelu'(conv output + bias), used by backward
+                epi = L.make_epilogue(bias=cbias[i], gelu=2, out_pre=y, pre_bs=Tpi * C, pre_ld=C)
                 ops.gemm_rows(a_prev, geo.Tp[i - 1] * C, s * C, Ti, B, k * C, self.wf[i], C, out, Tpi * C, C, epi, valid=vrow(i))
                 st["y"].append(y); st["mean"].append(None); st["rstd"].append(None)
             st["a"].append(out)
@@ -408,6 +411,9 @@ class Engine:
         dA = dfeat  # gradient w.r.t. a[i], no-lead layout [B, Tp_i, C]
         gpad = None
         cv = st.get("cv")
+        # conv_bias=True: d bias_i = column sum of dY_i (the gradient at the conv output, before GELU / LayerNorm), taken by
+        # whichever kernel produces dY_i (its rows of padding / skipped tiles are zero)
+        dcb = [self.g(blk[0].bias) if blk[0].bias is not None else None for blk in m.feature_extractor.conv_layers]
         for i in range(n - 1, 0, -1):
             _, k, s = convs[i]
             Ti, Tpi, lead, Tg = geo.T[i], geo.Tp[i], geo.lead[i], geo.Tg[i]
@@ -418,10 +424,10 @@ class Engine:
                 if ln_mode:
                     ln = m.feature_extractor.conv_layers[i][2][1]
                     ops.layer_norm_bwd(dA, Tpi * C, C, st["y"][i], Tpi * C, C, st["mean"][i], st["rstd"][i], ln.weight,
-                                       ln.bias, None, 0, 0, gv, Tg * C, C, self.g(ln.weight), self.g(ln.bias), None, Ti, B, C,
+                                       ln.bias, None, 0, 0, gv, Tg * C, C, self.g(ln.weight), self.g(ln.bias), dcb[i], Ti, B, C,
                                        gelu=True, valid=cv[i] if cv is not None else None)
                 else:
-                    ops.dgelu_mul(dA, Tpi * C, C, st["y"][i], Tpi * C, C, gv, Tg * C, C, Ti, B, C, None, pre_is_grad=True)
+                    ops.dgelu_mul(dA, Tpi * C, C, st["y"][i], Tpi * C, C, gv, Tg * C, C, Ti, B, C, dcb[i], pre_is_grad=True)
             gv = gpad[:, lead:]
             # ---- weight gradient: dW[co, (j,ci)] = sum dY[b,t,co] * a_{i-1}[b, s*t + j, ci]
             a_prev = st["a"][i - 1]
@@ -450,7 +456,9 @@ class Engine:
                 epi = None
                 if fuse_dgelu:
                     y_prev = st["y"][i - 1]
-                    epi = L.make_epilogue(dgelu=2, gelu_aux=y_prev.view(-1)[rho * C:], aux_bs=Tp_in * C, aux_ld=s * C)
+                    # (each phase stores its own rows of dY_{i-1}: the phases' column sums add up to d bias_{i-1})
+                    epi = L.make_epilogue(dgelu=2, gelu_aux=y_prev.view(-1)[rho * C:], aux_bs=Tp_in * C, aux_ld=s * C,
+                                          colsum=dcb[i - 1])
                 # rows u' of phase rho are input frames s*u' + rho: beyond the utterance's valid input frames the gradient is zero
                 pv = ((cv[i - 1] - rho + (s - 1)).clamp(min=0) // s).to(torch.int32) if cv is not None else None
                 ops.gemm_rows(a_view, Tg * C, C, n_u, B, nm * C, self.wd[i][rho], C, dst.view(-1)[dst_off + rho * C:], dst_bs,
@@ -462,7 +470,7 @@ class Engine:
                 ln = m.feature_extractor.conv_layers[i - 1][2][1]
                 ops.layer_norm_bwd(dAp, Tp_in * C, C, st["y"][i - 1], Tp_in * C, C, st["mean"][i - 1], st["rstd"][i - 1],
                                    ln.weight, ln.bias, None, 0, 0, gnext[:, lead_p:], Tg_p * C, C, self.g(ln.weight),
-                                   self.g(ln.bias), None, T_in, B, C, gelu=True, valid=cv[i - 1] if cv is not None else None)
+                                   self.g(ln.bias), dcb[i - 1], T_in, B, C, gelu=True, valid=cv[i - 1] if cv is not None else None)
                 gpad = gnext
                 dA = None
             else:
@@ -479,16 +487,16 @@ class Engine:
             ws = dA if (n > 1 and dA.dtype == BF and dA.is_contiguous() and k0 <= 10) else None
             ops.conv0_bwd(wav, L_, B, geo.T[0], C, k0, s0, blk0[0].weight, norm0.weight, norm0.bias, 1, None, None, fmean,
                           frstd, dA, geo.Tp[0] * C, self.g(blk0[0].weight), self.g(norm0.weight), self.g(norm0.bias),
-                          dconv_ws=ws, ws_bs=geo.Tp[0] * C)
+                          dconv_ws=ws, ws_bs=geo.Tp[0] * C, bias=blk0[0].bias, dbias=dcb[0])
         else:
             bstats = torch.empty(B, C, 12, dtype=torch.float32, device=dev)
             ops.conv0_bwd(wav, L_, B, geo.T[0], C, k0, s0, blk0[0].weight, norm0.weight, norm0.bias, 0, st["stats0"], bstats,
                           None, None, dA, geo.Tp[0] * C, self.g(blk0[0].weight), self.g(norm0.weight), self.g(norm0.bias))
 
     # ------------------------------------------------------------------------------------------------ LN + proj + mask
-    def project_forward(self, feats, T, mask_u8, pad_u8, save, want_features):
-        """transpose -> LayerNorm(C) -> post_extract_proj -> mask_emb / zero padded frames (WavLM/WavLM.py:341-357,574-575).
-        Writes into the zero-padded pos_conv input buffer."""
+    def project_forward(self, feats, T, mask_u8, pad_u8, save, want_features, chan_u8=None):
+        """transpose -> LayerNorm(C) -> post_extract_proj -> mask_emb / zero masked channels (`chan_u8`, uint8 [B, D] or None) /
+        zero padded frames (WavLM/WavLM.py:341-357,285-307,574-575).  Writes into the zero-padded pos_conv input buffer."""
         m, cfg = self.m, self.cfg
         B, Tp, C = feats.shape
         D = cfg.encoder_embed_dim
@@ -507,19 +515,20 @@ class Engine:
         if d is not None and d.p_input > 0:  # features = dropout_input(features), WavLM/WavLM.py:350
             ops.dropout_rows(xv, Tpad * D, D, None, 0, 0, xv, Tpad * D, D, T, B, D, d.p_input, d.key(DR.SITE_INPUT))
         features = xv[:, :T].clone() if want_features else None
-        ops.frame_mask_fwd(xv, Tpad * D, D, T, B, D, mask_u8, pad_u8, m.mask_emb)
+        ops.frame_mask_fwd(xv, Tpad * D, D, T, B, D, mask_u8, pad_u8, m.mask_emb, chan_u8)
         return dict(fn=fn, mean=mean, rstd=rstd, xpad=xpad, feats=feats if save else None, features=features, drop=d)
 
-    def project_backward(self, st, dxm, T, mask_u8, pad_u8, dfn_extra=None):
+    def project_backward(self, st, dxm, T, mask_u8, pad_u8, dfn_extra=None, chan_u8=None):
         """dxm: gradient w.r.t. the masked projection output, bf16 [B,T,D] (modified in place). Returns d(features) [B,Tp,C].
-        `dfn_extra` (bf16 [B,T,C]): gradient arriving at the LayerNorm output from a second consumer (wav2vec 2.0 quantizer)."""
+        `dfn_extra` (bf16 [B,T,C]): gradient arriving at the LayerNorm output from a second consumer (wav2vec 2.0 quantizer).
+        `chan_u8`: the channel mask of the forward pass."""
         m, cfg = self.m, self.cfg
         B = dxm.shape[0]
         D = cfg.encoder_embed_dim
         feats = st["feats"]
         Tp, C = feats.shape[1], feats.shape[2]
         dev = dxm.device
-        ops.frame_mask_bwd(dxm, T * D, D, T, B, D, mask_u8, pad_u8, self.g(m.mask_emb))
+        ops.frame_mask_bwd(dxm, T * D, D, T, B, D, mask_u8, pad_u8, self.g(m.mask_emb), chan_u8)
         d = st["drop"]
         if d is not None and d.p_input > 0:
             ops.dropout_rows(dxm, T * D, D, None, 0, 0, dxm, T * D, D, T, B, D, d.p_input, d.key(DR.SITE_INPUT))

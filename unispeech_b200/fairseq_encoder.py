@@ -8,7 +8,7 @@
   * `reorder_encoder_out`, `max_positions`, `set_num_updates`, `upgrade_state_dict_named`   fairseq_encoder.py:26-92
 
 Both keep the reference's freeze logic (`freeze_finetune_updates`: the encoder runs under no_grad until that many updates) and
-`apply_mask` (span masking only in training).  They are host glue around `unispeech_b200.wavlm.WavLM`: every tensor they return is a
+`apply_mask` (span masking, and channel masking when the model's `mask_channel_prob > 0`, in training only).  They are host glue around `unispeech_b200.wavlm.WavLM`: every tensor they return is a
 view of the kernels' output.  `final_dropout` and the output projection `proj` (CTC vocabulary / decoder width,
 hubert_asr.py:299-312,330-340) run on the same kernels as the encoder (`b200s_dropout_rows`, the wgmma GEMMs); `proj` keeps the
 reference's parameter names (`proj.weight [V, D]`, `proj.bias`) and initialiser (xavier_uniform / zeros, `Linear()` of

@@ -12,7 +12,8 @@ What makes the capture legal (and what it requires):
   * the batch shape and the set of executed layers are frozen: no padded samples (an all-False `padding_mask` is accepted and
     dropped, which is what the reference's own code path does with it), `encoder_layerdrop` must be 0, and the dropouts must be
     0 (their seeds are host-side kernel arguments);
-  * the span mask is DATA, not structure: it lives in a static device tensor that the graph reads (`mask_indices=`).
+  * the span mask is DATA, not structure: it lives in a static device tensor that the graph reads (`mask_indices=`); so does the
+    channel mask of models with `mask_channel_prob > 0` (`mask_channel_indices=`, drawn right after the span mask).
 
 `GraphedForwardBackward.step()` returns the static loss tensor of the replay; gradients are in `model.grad_buffer()` exactly as
 after an eager `loss.backward()`.  Data-parallel runs keep the eager path (the bucketed NCCL exchange is issued from Python
@@ -48,6 +49,11 @@ class GraphedForwardBackward:
         self.wav = torch.zeros(self.B, self.L, dtype=torch.float32, device=self.device)
         self.mask_dev = torch.zeros(self.B, self.T, dtype=torch.bool, device=self.device)
         self.mask_host = torch.zeros(self.B, self.T, dtype=torch.bool).pin_memory()
+        self.use_chan = self.use_mask and float(getattr(cfg, "mask_channel_prob", 0.0)) > 0.0
+        self.chan_dev, self.chan_host = None, None
+        if self.use_chan:
+            self.chan_dev = torch.zeros(self.B, cfg.encoder_embed_dim, dtype=torch.bool, device=self.device)
+            self.chan_host = torch.zeros(self.B, cfg.encoder_embed_dim, dtype=torch.bool).pin_memory()
         self.loss = torch.zeros((), dtype=torch.float32, device=self.device)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.capture_host_ms: Optional[float] = None
@@ -59,21 +65,25 @@ class GraphedForwardBackward:
             m.zero_grad_buffer()
             m._engine.prepared_version = None  # parameters change between steps: re-derive the bf16 operands
         x, _ = m.extract_features(self.wav, padding_mask=self.pad, mask=self.use_mask,
-                                  mask_indices=self.mask_dev if self.use_mask else None)
+                                  mask_indices=self.mask_dev if self.use_mask else None, mask_channel_indices=self.chan_dev)
         loss = self.loss_fn(x)
         loss.backward()
         self.loss.copy_(loss.detach().float().reshape(()))
 
     def sample_mask(self):
-        """Host-side span sampling of the reference into the pinned buffer, then one small async copy to the static device mask."""
+        """Host-side span (and channel) sampling of the reference into the pinned buffers, then small async copies to the static
+        device masks."""
         if not self.use_mask:
             return
-        idx = self.model.apply_mask(self.B, self.T, self.fpm_host)
+        idx, chan = self.model.sample_masks(self.B, self.T, self.fpm_host)
         if idx is None:
             self.mask_host.zero_()
         else:
             self.mask_host.copy_(idx)
         self.mask_dev.copy_(self.mask_host, non_blocking=True)
+        if self.use_chan:
+            self.chan_host.copy_(chan)
+            self.chan_dev.copy_(self.chan_host, non_blocking=True)
 
     def capture(self, warmup: int = 2):
         """Eager warm-up on a side stream (lazy initialisation: kernel attributes, engine scratch, the flat gradient buffer), then

@@ -81,9 +81,9 @@ class ILSHubertModel(WavLMForPretraining):
         self.label_embs_concat = None
 
     def forward(self, source, target_list=None, padding_mask=None, mask=True, features_only=False, output_layer=None,
-                mask_indices=None):
+                mask_indices=None, mask_channel_indices=None):
         out = super().forward(source, target_list=target_list, padding_mask=padding_mask, mask=mask, features_only=features_only,
-                              output_layer=output_layer, mask_indices=mask_indices)
+                              output_layer=output_layer, mask_indices=mask_indices, mask_channel_indices=mask_channel_indices)
         eng = self._engine
         if features_only:
             if self.layer_norm_first and output_layer is not None:   # ils_hubert.py:176-178

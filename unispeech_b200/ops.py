@@ -151,14 +151,15 @@ def dgelu_mul(dy, dy_bs, dy_rs, pre, pre_bs, pre_rs, out, out_bs, out_rs, rows_p
            i32(1 if pre_is_grad else 0), _s())
 
 
-def frame_mask_fwd(x, x_bs, x_rs, T, B, D, mask, pad, mask_emb):
+def frame_mask_fwd(x, x_bs, x_rs, T, B, D, mask, pad, mask_emb, chan_mask=None):
+    """`chan_mask` (uint8 [B, D] contiguous, device): channels zeroed in every frame of an utterance, or None."""
     _call("b200s_frame_mask_fwd", L.ptr(x), L.ll(x_bs), L.ll(x_rs), i32(T), i32(B), i32(D), L.ptr(mask), L.ptr(pad),
-           L.ptr(mask_emb), _s())
+           L.ptr(mask_emb), L.ptr(chan_mask), _s())
 
 
-def frame_mask_bwd(dx, x_bs, x_rs, T, B, D, mask, pad, dmask_emb):
+def frame_mask_bwd(dx, x_bs, x_rs, T, B, D, mask, pad, dmask_emb, chan_mask=None):
     _call("b200s_frame_mask_bwd", L.ptr(dx), L.ll(x_bs), L.ll(x_rs), i32(T), i32(B), i32(D), L.ptr(mask), L.ptr(pad),
-           L.ptr(dmask_emb), _s())
+           L.ptr(dmask_emb), L.ptr(chan_mask), _s())
 
 
 def gate_fwd(x, x_bs, x_rs, T, B, H, grep_w, grep_b, grep_a, gate):
@@ -185,22 +186,24 @@ def relpos_table_bwd(dtab, lut, n, H, demb):
 
 
 # ------------------------------------------------------------------------------------------------- conv layer 0
-def conv0_fwd(wav, L_, B, T, Cc, k, s, w, gamma, beta, mode, stats, fmean, frstd, out, out_bs):
+def conv0_fwd(wav, L_, B, T, Cc, k, s, w, gamma, beta, mode, stats, fmean, frstd, out, out_bs, bias=None):
+    """`bias` (fp32 [C], conv_bias=True): added before the LayerNorm (mode 1); cancelled exactly by the GroupNorm (mode 0)."""
     _call("b200s_conv0_fwd", L.ptr(wav), L.ll(L_), i32(B), i32(T), i32(Cc), i32(k), i32(s), L.ptr(w), L.ptr(gamma),
-           L.ptr(beta), i32(mode), L.ptr(stats), L.ptr(fmean), L.ptr(frstd), L.ptr(out), L.ll(out_bs), _s())
+           L.ptr(beta), i32(mode), L.ptr(stats), L.ptr(fmean), L.ptr(frstd), L.ptr(out), L.ll(out_bs), L.ptr(bias), _s())
 
 
 def conv0_bwd(wav, L_, B, T, Cc, k, s, w, gamma, beta, mode, stats, bstats, fmean, frstd, da, da_bs, dw, dgamma, dbeta,
-              dconv_ws=None, ws_bs=0):
-    """`dconv_ws` (LayerNorm mode): bf16 workspace for the gradient w.r.t. the raw convolution output; may be `da` itself."""
+              dconv_ws=None, ws_bs=0, bias=None, dbias=None):
+    """`dconv_ws` (LayerNorm mode): bf16 workspace for the gradient w.r.t. the raw convolution output; may be `da` itself.
+    `bias` / `dbias` (conv_bias=True): the forward's bias and its gradient (+=; untouched in GroupNorm mode, where it is zero)."""
     if dconv_ws is None:
         _call("b200s_conv0_bwd", L.ptr(wav), L.ll(L_), i32(B), i32(T), i32(Cc), i32(k), i32(s), L.ptr(w), L.ptr(gamma),
                L.ptr(beta), i32(mode), L.ptr(stats), L.ptr(bstats), L.ptr(fmean), L.ptr(frstd), L.ptr(da), L.ll(da_bs),
-               L.ptr(dw), L.ptr(dgamma), L.ptr(dbeta), _s())
+               L.ptr(dw), L.ptr(dgamma), L.ptr(dbeta), L.ptr(bias), L.ptr(dbias), _s())
     else:
         _call("b200s_conv0_bwd_ws", L.ptr(wav), L.ll(L_), i32(B), i32(T), i32(Cc), i32(k), i32(s), L.ptr(w), L.ptr(gamma),
                L.ptr(beta), i32(mode), L.ptr(stats), L.ptr(bstats), L.ptr(fmean), L.ptr(frstd), L.ptr(da), L.ll(da_bs),
-               L.ptr(dconv_ws), L.ll(ws_bs), L.ptr(dw), L.ptr(dgamma), L.ptr(dbeta), _s())
+               L.ptr(dconv_ws), L.ll(ws_bs), L.ptr(dw), L.ptr(dgamma), L.ptr(dbeta), L.ptr(bias), L.ptr(dbias), _s())
 
 
 # ------------------------------------------------------------------------------------------------- parameter prep

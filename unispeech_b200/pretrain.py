@@ -287,10 +287,11 @@ class WavLMForPretraining(WavLM):
         return [lg.new_zeros(lg.size(0), dtype=torch.long) for lg in self.get_logits(net_output, is_masked)]
 
     def forward(self, source, target_list=None, padding_mask=None, mask=True, features_only=False, output_layer=None,
-                mask_indices=None):
+                mask_indices=None, mask_channel_indices=None):
         """fairseq WavLMModel.forward.  With `features_only=False` the result carries everything the criterion needs
         (`x`, `padding_mask`, `mask_indices`, the frame-aligned `target_list`, `features_pen`); logits are never materialised."""
-        self.extract_features(source, padding_mask=padding_mask, mask=mask, output_layer=output_layer, mask_indices=mask_indices)
+        self.extract_features(source, padding_mask=padding_mask, mask=mask, output_layer=output_layer, mask_indices=mask_indices,
+                              mask_channel_indices=mask_channel_indices)
         res = self._last
         out = {"x": res["x"], "padding_mask": res["padding_mask"], "features": res["features"],
                "layer_results": res["layer_results"]}

@@ -306,7 +306,7 @@ class UniSpeechSATForPretraining(WavLMForPretraining):
         return dict(rows=pin(rows_h, torch.int32), inst=pin(inst_ns, torch.int32), same=pin(same, torch.uint8), S=S, N=N)
 
     def forward(self, source, target_list=None, padding_mask=None, mask=True, features_only=False, output_layer=None,
-                mask_indices=None):
+                mask_indices=None, mask_channel_indices=None):
         pre, fut, gen = None, None, None
         want_spk = not features_only and self.utterance_contrastive_loss and not self.skip_masked
         if want_spk and mask and (padding_mask is None or padding_mask.device.type == "cpu") and \
@@ -316,8 +316,9 @@ class UniSpeechSATForPretraining(WavLMForPretraining):
             B = source.shape[0]
             T = ConvGeom(self.conv_cfg, source.shape[1]).T[-1]
             pm_h = self.forward_padding_mask(T, padding_mask) if padding_mask is not None else torch.zeros(B, T, dtype=torch.bool)
-            if mask_indices is None:
-                mask_indices = self.apply_mask(B, T, pm_h if padding_mask is not None else None)
+            if mask_indices is None and mask_channel_indices is None:
+                # the channel draw follows the span draw immediately, as in the reference's apply_mask
+                mask_indices, mask_channel_indices = self.sample_masks(B, T, pm_h if padding_mask is not None else None)
             if mask_indices is not None:
                 # The helper thread draws from a COPY of the global CPU generator (the values the global one would have produced);
                 # the global state is moved to where that copy ended once the thread has been joined.
@@ -325,7 +326,7 @@ class UniSpeechSATForPretraining(WavLMForPretraining):
                 gen.set_state(torch.get_rng_state())
                 fut = _draw_pool().submit(self._draw_instances, mask_indices.bool(), pm_h, gen, source.device)
         out = super().forward(source, target_list=target_list, padding_mask=padding_mask, mask=mask, features_only=features_only,
-                              output_layer=output_layer, mask_indices=mask_indices)
+                              output_layer=output_layer, mask_indices=mask_indices, mask_channel_indices=mask_channel_indices)
         if fut is not None:
             pre = fut.result()
             torch.set_rng_state(gen.get_state())

@@ -236,14 +236,15 @@ class Wav2Vec2Model(WavLM):
             pen.append(net_output["features_pen"])
         return pen
 
-    def forward(self, source, padding_mask=None, mask=True, features_only=False, layer=None, mask_indices=None):
+    def forward(self, source, padding_mask=None, mask=True, features_only=False, layer=None, mask_indices=None,
+                mask_channel_indices=None):
         """Result keys of wav2vec2.py:633-723 except that `x` (the [N+1, B, T'] logits) is replaced by the fused loss:
         `loss_nce` (sum of cross entropies, device scalar), `sample_size`, `correct`, `count`."""
         if float(getattr(self.cfg, "dropout_features", 0.0)) > 0 and self.training and not features_only:
             raise NotImplementedError("dropout_features > 0 on the quantizer input is not implemented")
         # (`layer` is the 0-based index of the reference's TransformerEncoder.extract_features; extract_features here is 1-based)
         self.extract_features(source, padding_mask=padding_mask, mask=mask, output_layer=None if layer is None else layer + 1,
-                              mask_indices=mask_indices)
+                              mask_indices=mask_indices, mask_channel_indices=mask_channel_indices)
         res = self._last
         if features_only:
             return {"x": res["x"], "padding_mask": res["padding_mask"], "features": res["unmasked_features"],

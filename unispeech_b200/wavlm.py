@@ -75,10 +75,6 @@ def _check_supported(cfg):
     bad = []
     if cfg.activation_fn != "gelu":
         bad.append("activation_fn != gelu")
-    if cfg.conv_bias:
-        bad.append("conv_bias")
-    if cfg.mask_channel_prob > 0:
-        bad.append("mask_channel_prob > 0")
     if eval(cfg.conv_feature_layers)[-1][0] == cfg.encoder_embed_dim:
         bad.append("conv feature width == encoder_embed_dim (the reference then has no post_extract_proj; the projection kernels assume one)")
     return bad
@@ -147,11 +143,11 @@ class _ProjFn(torch.autograd.Function):
     projection's in the backward pass."""
 
     @staticmethod
-    def forward(ctx, feats, anchor, eng: Engine, T, mask_u8, pad_u8, want_features, want_fn=False):
+    def forward(ctx, feats, anchor, eng: Engine, T, mask_u8, pad_u8, want_features, want_fn=False, chan_u8=None):
         ctx.fwd_stream = torch.cuda.current_stream()
         save = bool(ctx.needs_input_grad[0] or ctx.needs_input_grad[1])
-        st = eng.project_forward(feats, T, mask_u8, pad_u8, save, want_features)
-        ctx.eng, ctx.st, ctx.T, ctx.mask, ctx.pad = eng, st, T, mask_u8, pad_u8
+        st = eng.project_forward(feats, T, mask_u8, pad_u8, save, want_features, chan_u8)
+        ctx.eng, ctx.st, ctx.T, ctx.mask, ctx.pad, ctx.chan = eng, st, T, mask_u8, pad_u8, chan_u8
         half = eng.cfg.conv_pos // 2
         eng._last_xpad = st["xpad"]  # the padded pos_conv input buffer the returned view lives in
         xv = st["xpad"][:, half:half + T]
@@ -163,10 +159,10 @@ class _ProjFn(torch.autograd.Function):
         if dfn_extra is not None:
             dfn_extra = dfn_extra if (dfn_extra.dtype == torch.bfloat16 and dfn_extra.is_contiguous()) else \
                 dfn_extra.to(torch.bfloat16).contiguous()
-        dfeat = ctx.eng.project_backward(ctx.st, dxv.contiguous(), ctx.T, ctx.mask, ctx.pad, dfn_extra)
+        dfeat = ctx.eng.project_backward(ctx.st, dxv.contiguous(), ctx.T, ctx.mask, ctx.pad, dfn_extra, ctx.chan)
         ctx.st = None  # (GradMultiply is applied where the gradient enters the extractor: _ConvFn.backward)
         ctx.eng.backward_stage_done("stem")
-        return dfeat, None, None, None, None, None, None, None
+        return dfeat, None, None, None, None, None, None, None, None
 
 
 class _StemFn(torch.autograd.Function):
@@ -496,6 +492,9 @@ class WavLM(nn.Module):
         self.post_extract_proj = nn.Linear(self.embed, cfg.encoder_embed_dim) if self.embed != cfg.encoder_embed_dim else None
         self.mask_prob, self.mask_selection, self.mask_other = cfg.mask_prob, cfg.mask_selection, cfg.mask_other
         self.mask_length, self.no_mask_overlap, self.mask_min_space = cfg.mask_length, cfg.no_mask_overlap, cfg.mask_min_space
+        self.mask_channel_prob, self.mask_channel_selection = cfg.mask_channel_prob, cfg.mask_channel_selection
+        self.mask_channel_other, self.mask_channel_length = cfg.mask_channel_other, cfg.mask_channel_length
+        self.no_mask_channel_overlap, self.mask_channel_min_space = cfg.no_mask_channel_overlap, cfg.mask_channel_min_space
         self.dropout_input = nn.Dropout(cfg.dropout_input)
         self.dropout_features = nn.Dropout(cfg.dropout_features)
         self.feature_grad_mult = cfg.feature_grad_mult
@@ -592,6 +591,22 @@ class WavLM(nn.Module):
             return torch.from_numpy(idx)
         return None
 
+    def apply_channel_mask(self, B):
+        """Host-side channel sampling identical to the reference (numpy RNG; WavLM/WavLM.py:288-307): spans over the
+        `encoder_embed_dim` channels, no padding mask, min_masks 0.  Returns bool [B, D] or None."""
+        if self.mask_channel_prob > 0:
+            idx = compute_mask_indices((B, self.cfg.encoder_embed_dim), None, self.mask_channel_prob, self.mask_channel_length,
+                                       self.mask_channel_selection, self.mask_channel_other, no_overlap=self.no_mask_channel_overlap,
+                                       min_space=self.mask_channel_min_space)
+            return torch.from_numpy(idx)
+        return None
+
+    def sample_masks(self, B, T, padding_mask):
+        """(span mask bool [B,T] or None, channel mask bool [B,D] or None), drawn from the numpy global RNG in the reference's
+        order: the span mask first, then the channel mask."""
+        mask_indices = self.apply_mask(B, T, padding_mask)
+        return mask_indices, self.apply_channel_mask(B)
+
     def forward_padding_mask(self, T: int, padding_mask: torch.Tensor) -> torch.Tensor:
         """Sample-level mask -> frame-level mask (WavLM/WavLM.py:311-321)."""
         extra = padding_mask.size(1) % T
@@ -601,9 +616,11 @@ class WavLM(nn.Module):
         return padding_mask.all(-1)
 
     def extract_features(self, source, padding_mask=None, mask=False, ret_conv=False, output_layer=None,
-                         ret_layer_results=False, mask_indices=None):
-        """Same contract as the reference.  `mask_indices` (bool [B,T], optional) lets a caller inject the masked frames instead
-        of sampling them (used by the parity tests; the reference's sampler is host numpy RNG)."""
+                         ret_layer_results=False, mask_indices=None, mask_channel_indices=None):
+        """Same contract as the reference.  `mask_indices` (bool [B,T], optional) and `mask_channel_indices` (bool [B,D],
+        optional) let a caller inject the masked frames and channels instead of sampling them (used by the parity tests and the
+        CUDA graph; the reference's sampler is host numpy RNG).  With `mask=True` both are sampled when neither is given;
+        once either is given, the other one given as None means no mask of that kind."""
         from .engine import ConvGeom
         T = ConvGeom(self.conv_cfg, source.shape[1]).T[-1]
         B = source.shape[0]
@@ -614,10 +631,13 @@ class WavLM(nn.Module):
         if fpm is not None and fpm.device.type == "cpu":
             fpm_host = fpm
             fpm = fpm.to(source.device, non_blocking=True)
-        if mask and mask_indices is None:
+        if mask and mask_indices is None and mask_channel_indices is None:
             if fpm is not None and fpm_host is None:
                 fpm_host = fpm.cpu()  # device-resident mask: one sync, exactly like the reference's `.item()` per row
-            mask_indices = self.apply_mask(B, T, fpm_host)
+            mask_indices, mask_channel_indices = self.sample_masks(B, T, fpm_host)
+        if mask_channel_indices is not None and tuple(mask_channel_indices.shape) != (B, self.cfg.encoder_embed_dim):
+            raise ValueError(f"mask_channel_indices must be [B, encoder_embed_dim] = [{B}, {self.cfg.encoder_embed_dim}]; "
+                             f"got {list(mask_channel_indices.shape)}")
         # ragged batch: frames of every utterance up to its last valid one (host arithmetic when the mask lives on the host; with
         # a device-only mask two tiny device ops, no synchronisation).  The layer GEMMs skip the padded tail of every utterance.
         # The tensor travels to the encoder as an attribute of the frame mask, so a stale one can never meet another batch.
@@ -638,9 +658,12 @@ class WavLM(nn.Module):
         self._last_conv = feats  # conv features [B, Tp, C] (valid rows T): `features_pen` of the pre-training criterion reads them
         eng = self._engine
         mask_u8 = mask_indices.to(device=source.device, dtype=torch.uint8).contiguous() if mask_indices is not None else None
+        chan_u8 = mask_channel_indices.to(device=source.device, dtype=torch.uint8).contiguous() \
+            if mask_channel_indices is not None else None
         pad_u8 = fpm.to(torch.uint8).contiguous() if fpm is not None else None
         want_fn = bool(getattr(self, "_want_unmasked_features", False))
-        xv, features, unmasked = _ProjFn.apply(feats, self.post_extract_proj.weight, eng, T, mask_u8, pad_u8, ret_conv, want_fn)
+        xv, features, unmasked = _ProjFn.apply(feats, self.post_extract_proj.weight, eng, T, mask_u8, pad_u8, ret_conv, want_fn,
+                                               chan_u8)
         xv._b200_xpad = eng._last_xpad
         el = getattr(self, "_extract_layer", None)  # UniSpeech-SAT: 0-based `utterance_contrastive_layer - 1` (unispeech_sat.py:640-645)
         pl = getattr(self, "_predict_layers", None)  # ILS-HuBERT: 1-based layers whose outputs feed intermediate heads (ils_hubert.py:167-171)
@@ -648,8 +671,8 @@ class WavLM(nn.Module):
         enc = self.encoder(xv, padding_mask=fpm, layer=lay, extract_layer=el)
         x, layer_results = enc[0], enc[1]
         res = {"x": x, "padding_mask": fpm, "features": features, "layer_results": layer_results,
-               "mask_indices": mask_indices, "padding_mask_host": fpm_host, "spk_x": enc[2] if el is not None else None,
-               "unmasked_features": unmasked}
+               "mask_indices": mask_indices, "mask_channel_indices": mask_channel_indices, "padding_mask_host": fpm_host,
+               "spk_x": enc[2] if el is not None else None, "unmasked_features": unmasked}
         self._last = res
         feature = res["features"] if ret_conv else res["x"]
         if ret_layer_results:
