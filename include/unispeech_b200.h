@@ -385,6 +385,39 @@ int b200s_vq_logits_bwd(const void* logits, long long logits_rs, int S, int G, i
 int b200s_vq_dvars(const void* dq, long long dq_rs, const int* codes, int S, int G, int V, int dv, float* dvars,
                    b200s_stream stream);
 
+/* ============================ CTC fine-tuning loss (csrc/ctc.cu) ============================ */
+/* log-softmax + connectionist temporal classification (Graves et al. 2006; the loss of the fairseq `ctc` criterion) on the bf16
+ * logits of the fine-tuning wrappers' `proj` head, without ever materialising log-probabilities: lp[t,c] = logit[t,c] - lse[t].
+ * logits: element (t, b, c) at logits[b * batch_stride + t * frame_stride + c] (strides in elements, unit class stride), so the
+ * T x B x V view of a [B*T, Vp] buffer is (frame_stride = Vp, batch_stride = T * Vp) and a contiguous T x B x V tensor is
+ * (B * V, V).  input_len: int32 [B] valid frames (clamped to [0, T]); frames t >= input_len[b] are NEVER read (they may hold
+ * anything) and get an exactly zero gradient.  targets: int32 [B, Smax] padded; target_len: int32 [B].  All device memory.
+ * Limits: 1 <= V <= 1024, 0 <= blank < V, Smax <= B200S_CTC_MAX_TARGET (one thread per position of the extended label
+ * sequence blank, l_1, blank, ..., l_S, blank); calls beyond them fail, nothing is truncated.
+ * An utterance is INFEASIBLE when input_len is too short for its target (with one blank per repeat), or when target_len is
+ * outside [0, Smax] or a label outside [0, V): nll = +inf and its whole gradient is written as zeros (with and without
+ * zero_infinity). */
+#define B200S_CTC_MAX_TARGET 511
+/* One warp per valid frame: lse[b*T + t] = logsumexp_c logit[t,b,c] (fp32), argmax[b*T + t] = first class with the largest
+ * logit (int32; NULL to skip).  Entries of padded frames are left untouched. */
+int b200s_ctc_stats(const void* logits, long long frame_stride, long long batch_stride, const int* input_len, int B, int T, int V,
+                    float* lse, int* argmax, b200s_stream stream);
+/* Alpha recursion, one CTA per utterance, fp32 log space.  log_alpha: fp32 [B, T, 2*Smax+1] workspace (written for valid frames
+ * and positions only; read back by b200s_ctc_beta_grad).  nll[b] = -log p(target_b | logits_b), +inf when infeasible.
+ * *loss_sum (fp64, may be NULL) += sum_b nll[b]; with zero_infinity the infeasible utterances are left out of that sum. */
+int b200s_ctc_alpha(const void* logits, long long frame_stride, long long batch_stride, const float* lse, const int* input_len,
+                    const int* targets, int Smax, const int* target_len, int B, int T, int V, int blank, int zero_infinity,
+                    float* log_alpha, float* nll, double* loss_sum, b200s_stream stream);
+/* Beta recursion with the gradient through CTC AND the log-softmax fused in (log_beta is never stored):
+ *   grad[t,b,c] = upstream[b] * (softmax(logit[t,b,:])_c - sum_{s: l'_s = c} gamma_t(s)),   gamma = exp(alpha + beta - lp + nll),
+ * as bf16 at grad[b * grad_batch_stride + t * grad_frame_stride + c] for c < Vpad (columns V..Vpad and every padded frame are
+ * zeros).  upstream: DEVICE fp32 [B] = d loss / d nll[b].  The per-class sums run over positions bucketed by class in a fixed
+ * order (no floating-point atomics): two calls give bit-identical gradients. */
+int b200s_ctc_beta_grad(const void* logits, long long frame_stride, long long batch_stride, const float* lse, const int* input_len,
+                        const int* targets, int Smax, const int* target_len, int B, int T, int V, int blank, const float* log_alpha,
+                        const float* nll, const float* upstream, void* grad, long long grad_frame_stride,
+                        long long grad_batch_stride, int Vpad, b200s_stream stream);
+
 /* ============================ on-device data path (csrc/datapath.cu) ============================ */
 /* Span masking of compute_mask_indices (WavLM/WavLM.py:35-159; static span length, overlapping spans) on the device, with the
  * library's counter-based RNG instead of numpy's (statistical parity): per row count = max(min_masks, floor(mask_prob sz / L + u)),

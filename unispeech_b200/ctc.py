@@ -1,0 +1,232 @@
+"""CTC fine-tuning on the library's own kernels (csrc/ctc.cu): the loss, the criterion and the model surface of the reference's
+ASR fine-tuning (src/fairseq/criterions/ctc.py, src/fairseq/models/hubert/hubert_asr.py `HubertCtc`,
+src/fairseq/models/wav2vec/wav2vec2_asr.py `Wav2VecCtc`).
+
+  * `ctc_loss(logits_tbv, input_len, targets, target_len, blank, reduction, zero_infinity)`: log-softmax + CTC on bf16 logits, one
+    autograd Function.  Forward = row statistics + alpha recursion (all an eval pass needs); backward = beta recursion with the
+    gradient through CTC and the log-softmax fused in.  The logits are read through their strides: the T x B x V view that the
+    fine-tuning wrappers return over their [B*T, Vp] buffer is consumed, and its gradient produced, without a copy.  The loss stays
+    on the device; nothing synchronises, so a fixed-shape fine-tuning step captures in a CUDA graph.
+  * `CtcCriterion`: `forward(model, sample) -> (loss, sample_size, logging_output)` with the reference's contract (below).
+  * `HubertCtc` / `Wav2VecCtc`: `w2v_encoder` = `HubertEncoder` / `Wav2VecEncoder`, `forward(**net_input)`, `get_logits`,
+    `get_normalized_probs`, `set_num_updates`; `state_dict` keys `w2v_encoder.w2v_model.*`, `w2v_encoder.proj.*`.
+
+Limits (the kernels fail beyond them, nothing is truncated): V <= 1024 classes, targets of at most `MAX_TARGET` labels.
+An infeasible utterance (input too short for its target with one blank per repeated label; a label outside [0, V)) has
+nll = +inf and an all-zero gradient, with and without `zero_infinity` (`torch.nn.functional.ctc_loss` leaves that gradient
+unspecified without it); `zero_infinity` additionally replaces its +inf by 0 in the returned loss.
+"""
+from __future__ import annotations
+
+from typing import List, Optional
+
+import torch
+import torch.nn as nn
+import torch.nn.functional as F
+
+from . import ops
+from .engine import BF
+from .fairseq_encoder import HubertEncoder, Wav2VecEncoder
+from .wavlm import _on_forward_stream
+
+MAX_TARGET = 511   # B200S_CTC_MAX_TARGET: one thread per position of the extended label sequence, 2 * 511 + 1 <= 1024
+MAX_CLASSES = 1024
+
+
+class _CtcFn(torch.autograd.Function):
+    """(nll [B] fp32, sum_b nll fp32 scalar, argmax [B, T] int32 or None) of bf16 logits T x B x V (unit class stride)."""
+
+    @staticmethod
+    def forward(ctx, logits, input_len, targets, target_len, blank, zero_infinity, want_argmax):
+        ctx.fwd_stream = torch.cuda.current_stream()
+        dev = logits.device
+        T, B, V = logits.shape
+        fs, bs = logits.stride(0), logits.stride(1)
+        Smax = targets.shape[1]
+        lse = torch.empty(B, T, dtype=torch.float32, device=dev)
+        # frames past input_len are not visited: they decode to blank
+        argmax = torch.full((B, T), blank, dtype=torch.int32, device=dev) if want_argmax else None
+        log_alpha = torch.empty(B, T, 2 * Smax + 1, dtype=torch.float32, device=dev)
+        nll = torch.empty(B, dtype=torch.float32, device=dev)
+        total = torch.zeros(1, dtype=torch.float64, device=dev)
+        ops.ctc_stats(logits, fs, bs, input_len, B, T, V, lse, argmax)
+        ops.ctc_alpha(logits, fs, bs, lse, input_len, targets, Smax, target_len, B, T, V, blank, zero_infinity, log_alpha, nll, total)
+        ctx.save_for_backward(logits, input_len, targets, target_len, lse, log_alpha, nll)
+        ctx.blank = blank
+        out = nll.masked_fill(nll == float("inf"), 0.0) if zero_infinity else nll.clone()
+        if argmax is not None:
+            ctx.mark_non_differentiable(argmax)
+        return out, total.float().reshape(()), argmax
+
+    @staticmethod
+    @_on_forward_stream
+    def backward(ctx, d_nll, d_total, _d_argmax=None):
+        logits, input_len, targets, target_len, lse, log_alpha, nll = ctx.saved_tensors
+        dev = logits.device
+        T, B, V = logits.shape
+        fs, bs = logits.stride(0), logits.stride(1)
+        up = torch.zeros(B, dtype=torch.float32, device=dev)   # d loss / d nll[b]
+        if d_nll is not None:
+            up += d_nll.float()
+        if d_total is not None:
+            up += d_total.float()
+        if bs == T * fs and fs >= V:
+            # rows view of a [B*T, Vp] buffer: the gradient gets the same layout, its padding columns written as zeros
+            buf = torch.empty(B * T, fs, dtype=BF, device=dev)
+            grad, vpad = buf[:, :V].reshape(B, T, V).transpose(0, 1), fs
+        else:
+            grad, vpad = torch.empty_strided(logits.shape, logits.stride(), dtype=BF, device=dev), V
+        ops.ctc_beta_grad(logits, fs, bs, lse, input_len, targets, targets.shape[1], target_len, B, T, V, ctx.blank, log_alpha, nll,
+                          up, grad, fs, bs, vpad)
+        return grad, None, None, None, None, None, None
+
+
+def _i32(t: torch.Tensor, dev) -> torch.Tensor:
+    return t.to(device=dev, dtype=torch.int32).contiguous()
+
+
+def ctc_loss(logits_tbv: torch.Tensor, input_len: torch.Tensor, targets: torch.Tensor, target_len: torch.Tensor, blank: int = 0,
+             reduction: str = "sum", zero_infinity: bool = False, return_argmax: bool = False):
+    """CTC loss of bf16 logits T x B x V (log-softmax included).  `targets` [B, Smax] padded, `input_len` / `target_len` [B].
+    reduction: "sum" (fp64 accumulation on the device), "mean" (F.ctc_loss's: nll / max(target_len, 1), averaged over the batch)
+    or "none" ([B]).  With `return_argmax` also returns the per-frame first-argmax class [B, T] int32 (blank past input_len)."""
+    if reduction not in ("sum", "mean", "none"):
+        raise ValueError(f"ctc_loss: reduction={reduction!r}")
+    if not logits_tbv.is_cuda or logits_tbv.dtype != BF or logits_tbv.dim() != 3:
+        raise ValueError("ctc_loss: logits must be a CUDA bf16 tensor T x B x V (there is no CPU or fp32 path)")
+    if logits_tbv.stride(2) != 1:
+        raise ValueError("ctc_loss: the class dimension of the logits must have unit stride")
+    if targets.dim() != 2 or targets.shape[0] != logits_tbv.shape[1]:
+        raise ValueError(f"ctc_loss: targets must be [B, Smax] padded, got {tuple(targets.shape)}")
+    dev = logits_tbv.device
+    target_len = _i32(target_len, dev)
+    nll, total, argmax = _CtcFn.apply(logits_tbv, _i32(input_len, dev), _i32(targets, dev), target_len, int(blank),
+                                      bool(zero_infinity), bool(return_argmax))
+    if reduction == "sum":
+        loss = total
+    elif reduction == "none":
+        loss = nll
+    else:
+        loss = (nll / target_len.clamp(min=1).float()).mean()
+    return (loss, argmax) if return_argmax else loss
+
+
+def prepare_targets(target: torch.Tensor, pad_idx: int, eos_idx: int, target_lengths: Optional[torch.Tensor] = None):
+    """`sample["target"]` [B, S] -> (int32 [B, S] with every pad / eos removed and the rest moved to the front in order, int32 [B]
+    lengths).  The reference packs the kept labels with `masked_select` (a device synchronisation); this is the same selection
+    kept per row, with device-side index arithmetic only."""
+    keep = (target != pad_idx) & (target != eos_idx)
+    B, S = target.shape
+    pos = keep.long().cumsum(1) - 1
+    out = torch.zeros(B, S + 1, dtype=target.dtype, device=target.device)
+    out.scatter_(1, torch.where(keep, pos, torch.full_like(pos, S)), target)   # dropped entries land in the spare column
+    lengths = keep.sum(-1) if target_lengths is None else target_lengths
+    return out[:, :S].to(torch.int32).contiguous(), lengths.to(torch.int32)
+
+
+def greedy_collapse(argmax: torch.Tensor, input_len, blank: int = 0) -> List[List[int]]:
+    """Best-path decoding of per-frame argmax classes [B, T] (host side): per utterance, the first input_len[b] frames with
+    consecutive duplicates merged and blanks removed."""
+    rows, lens = argmax.tolist(), [int(n) for n in input_len]
+    hyps = []
+    for row, n in zip(rows, lens):
+        out, prev = [], None
+        for c in row[:n]:
+            if c != prev and c != blank:
+                out.append(int(c))
+            prev = c
+        hyps.append(out)
+    return hyps
+
+
+class CtcCriterion(nn.Module):
+    """The reference's `ctc` criterion (src/fairseq/criterions/ctc.py) on `ctc_loss`.
+
+    `forward(model, sample)` -> `(loss, sample_size, logging_output)`:
+      * `net_output = model(**sample["net_input"])`, logits T x B x V from `model.get_logits(net_output)`;
+      * input lengths = `sample["net_input"]["src_lengths"]` if present, else the number of False entries per row of
+        `net_output["padding_mask"]` (all T when it is None);
+      * every `pad_idx` / `eos_idx` entry of `sample["target"]` is dropped; target lengths = `sample["target_lengths"]` if
+        present, else the number of kept labels;
+      * loss = sum over the batch of the CTC negative log-likelihood (`reduction="sum"`, `blank_idx`, `zero_infinity`);
+      * `sample_size` = number of sentences if `sentence_avg` else `ntokens` (`sample["ntokens"]`, else the sum of the target
+        lengths); `logging_output` = {"loss", "ntokens", "nsentences", "sample_size"}.
+    Where this differs: the reference packs the kept labels with `masked_select` and reads `ntokens` / the loss back with `.item()`;
+    here targets stay padded [B, S] with lengths and `logging_output` carries device tensors, so a training step never waits for
+    the device.  In eval mode `logging_output["hypotheses"]` holds the best path per utterance (per-frame argmax, consecutive
+    duplicates merged, blanks removed) as lists of class ids; scoring them against text (WER / CER) is left to the caller."""
+
+    def __init__(self, blank_idx: int = 0, pad_idx: int = 1, eos_idx: int = 2, zero_infinity: bool = False,
+                 sentence_avg: bool = False):
+        super().__init__()
+        self.blank_idx, self.pad_idx, self.eos_idx = blank_idx, pad_idx, eos_idx
+        self.zero_infinity, self.sentence_avg = zero_infinity, sentence_avg
+
+    def forward(self, model, sample, reduce: bool = True):
+        net_output = model(**sample["net_input"])
+        logits = model.get_logits(net_output)
+        T, B, _ = logits.shape
+        if "src_lengths" in sample["net_input"]:
+            input_lengths = sample["net_input"]["src_lengths"]
+        elif net_output["padding_mask"] is not None:
+            input_lengths = (~net_output["padding_mask"]).sum(-1)
+        else:
+            input_lengths = torch.full((B,), T, dtype=torch.int32, device=logits.device)
+        targets, target_lengths = prepare_targets(sample["target"].to(logits.device), self.pad_idx, self.eos_idx,
+                                                  sample.get("target_lengths"))
+        eval_mode = not model.training
+        res = ctc_loss(logits, input_lengths, targets, target_lengths, blank=self.blank_idx, reduction="sum",
+                       zero_infinity=self.zero_infinity, return_argmax=eval_mode)
+        loss, argmax = res if eval_mode else (res, None)
+        ntokens = sample["ntokens"] if "ntokens" in sample else target_lengths.sum()
+        sample_size = sample["target"].size(0) if self.sentence_avg else ntokens
+        logging_output = {"loss": loss.detach(), "ntokens": ntokens,
+                          "nsentences": sample["id"].numel() if "id" in sample else B, "sample_size": sample_size}
+        if eval_mode:
+            logging_output["hypotheses"] = greedy_collapse(argmax.cpu(), input_lengths.cpu(), self.blank_idx)
+        return loss, sample_size, logging_output
+
+
+class _CtcModel(nn.Module):
+    """`BaseFairseqModel` surface of the reference's CTC fine-tuning models around one `w2v_encoder`."""
+
+    def __init__(self, w2v_encoder):
+        super().__init__()
+        if w2v_encoder.proj is None:
+            raise ValueError("a CTC model needs the encoder's output projection: build the encoder with output_dim = vocabulary size")
+        self.w2v_encoder = w2v_encoder
+
+    def forward(self, **kwargs):
+        return self.w2v_encoder(**kwargs)
+
+    def get_logits(self, net_output):
+        """T x B x V bf16 logits.  The reference overwrites padded frames with (0, -inf, ...) here after a `padding_mask.any()`
+        read-back; `ctc_loss` never reads frames past the input length, so they are returned as they are."""
+        return net_output["encoder_out"]
+
+    def get_normalized_probs(self, net_output, log_probs: bool, sample=None):
+        """float (log-)softmax of `encoder_out` for callers that want probabilities; `CtcCriterion` does not go through it."""
+        logits = net_output["encoder_out"].float()
+        return F.log_softmax(logits, dim=-1) if log_probs else F.softmax(logits, dim=-1)
+
+    def set_num_updates(self, num_updates: int):
+        self.w2v_encoder.set_num_updates(num_updates)
+
+    def max_positions(self):
+        return self.w2v_encoder.max_positions()
+
+
+class HubertCtc(_CtcModel):
+    """hubert_asr.py `HubertCtc`: `w2v_encoder` is a `HubertEncoder` whose `proj` has the vocabulary's width."""
+
+    @classmethod
+    def build_model(cls, w2v_model, vocab_size: int, **encoder_kwargs):
+        return cls(HubertEncoder(w2v_model, output_dim=vocab_size, **encoder_kwargs))
+
+
+class Wav2VecCtc(_CtcModel):
+    """wav2vec2_asr.py `Wav2VecCtc`: `w2v_encoder` is a `Wav2VecEncoder` whose `proj` has the vocabulary's width."""
+
+    @classmethod
+    def build_model(cls, w2v_model, vocab_size: int, **encoder_kwargs):
+        return cls(Wav2VecEncoder(w2v_model, output_dim=vocab_size, **encoder_kwargs))

@@ -379,6 +379,26 @@ def vq_dvars(dq, dq_rs, codes, S, G, V, dv, dvars):
     _call("b200s_vq_dvars", L.ptr(dq), L.ll(dq_rs), L.ptr(codes), i32(S), i32(G), i32(V), i32(dv), L.ptr(dvars), _s())
 
 
+# ------------------------------------------------------------------------------------------------- CTC fine-tuning loss
+def ctc_stats(logits, frame_stride, batch_stride, input_len, B, T, V, lse, argmax):
+    _call("b200s_ctc_stats", L.ptr(logits), L.ll(frame_stride), L.ll(batch_stride), L.ptr(input_len), i32(B), i32(T), i32(V),
+          L.ptr(lse), L.ptr(argmax), _s())
+
+
+def ctc_alpha(logits, frame_stride, batch_stride, lse, input_len, targets, Smax, target_len, B, T, V, blank, zero_infinity,
+              log_alpha, nll, loss_sum):
+    _call("b200s_ctc_alpha", L.ptr(logits), L.ll(frame_stride), L.ll(batch_stride), L.ptr(lse), L.ptr(input_len), L.ptr(targets),
+          i32(Smax), L.ptr(target_len), i32(B), i32(T), i32(V), i32(blank), i32(1 if zero_infinity else 0), L.ptr(log_alpha),
+          L.ptr(nll), L.ptr(loss_sum), _s())
+
+
+def ctc_beta_grad(logits, frame_stride, batch_stride, lse, input_len, targets, Smax, target_len, B, T, V, blank, log_alpha, nll,
+                  upstream, grad, grad_frame_stride, grad_batch_stride, Vpad):
+    _call("b200s_ctc_beta_grad", L.ptr(logits), L.ll(frame_stride), L.ll(batch_stride), L.ptr(lse), L.ptr(input_len),
+          L.ptr(targets), i32(Smax), L.ptr(target_len), i32(B), i32(T), i32(V), i32(blank), L.ptr(log_alpha), L.ptr(nll),
+          L.ptr(upstream), L.ptr(grad), L.ll(grad_frame_stride), L.ll(grad_batch_stride), i32(Vpad), _s())
+
+
 # ------------------------------------------------------------------------------------------------- on-device data path
 def span_mask(valid_len, B, T, mask_prob, mask_length, min_masks, key, mask, counts):
     _call("b200s_span_mask", L.ptr(valid_len), i32(B), i32(T), f32(mask_prob), i32(mask_length), i32(min_masks), u32(key[0]),
