@@ -418,6 +418,39 @@ int b200s_ctc_beta_grad(const void* logits, long long frame_stride, long long ba
                         const float* nll, const float* upstream, void* grad, long long grad_frame_stride,
                         long long grad_batch_stride, int Vpad, b200s_stream stream);
 
+/* ============================ k-means pseudo-labels (csrc/kmeans.cu) ============================ */
+/* Nearest-centroid labels, Lloyd updates and k-means++ seeding over bf16 features (the label stage of HuBERT-style pre-training).
+ * Centres: fp32 master [K, D]; the bf16 copy the assignment multiplies, [Kp, D] with Kp = K rounded up to a multiple of 256 (rows
+ * K..Kp are zeros); cnorm fp32 [Kp] = |bf16 copy|^2.  Limits, checked before any launch: 1 <= K <= B200S_KMEANS_MAX_K, D a
+ * positive multiple of 64 (zero-pad narrower features: distances do not change).  No floating-point atomics: every result is
+ * bit-identical from call to call.  All pointers are device memory. */
+#define B200S_KMEANS_MAX_K 1024
+/* labels[b*rows + t] = argmin_k (cnorm[k] - 2 x[b,t] . c_k) (ties to the lowest k), score[...] = that minimum (fp32, NULL to
+ * skip), for t < valid[b] (valid: int32 [batches] or NULL = all rows); rows t >= valid[b] get label -1 and no score, and a
+ * 128-row band that starts at or past valid[b] is not read.  x: bf16, element (b, t, d) at x[b*x_bs + t*x_rs + d] (x_bs, x_rs
+ * multiples of 8, 16-byte aligned base).  prev_labels / changed (both or neither): *changed += number of valid rows whose label
+ * differs from prev_labels (int32 atomics; the caller zeroes it). */
+int b200s_kmeans_assign(const void* x, long long x_bs, long long x_rs, int rows, int batches, int D, const int* valid,
+                        const void* centers, const float* cnorm, int K, int* labels, float* score, const int* prev_labels,
+                        int* changed, b200s_stream stream);
+/* Bytes of workspace b200s_kmeans_update needs (-1 for bad sizes). */
+long long b200s_kmeans_update_workspace(long long n, int K, int D);
+/* Per-cluster statistics of n labelled rows (x: bf16 [n, D], row stride x_rs; labels outside [0, K) are skipped):
+ * counts[k] (int32), sums[k, :] (fp32, summed in fp64 across fixed pieces), *inertia = sum over labelled rows of |x|^2 + score
+ * (fp64; with the scores of b200s_kmeans_assign that is the sum of squared distances to the assigned centres). */
+int b200s_kmeans_update(const void* x, long long x_rs, int n, int D, const int* labels, const float* score, int K, void* workspace,
+                        long long workspace_bytes, int* counts, float* sums, double* inertia, b200s_stream stream);
+/* centers[k] = sums[k] / counts[k] where counts[k] > 0; an empty cluster keeps its centre (sums = counts = NULL: no update).
+ * Then writes the bf16 copy centers_bf16 [Kp, D] and cnorm [Kp]. */
+int b200s_kmeans_centers(const float* sums, const int* counts, int K, int D, float* centers, void* centers_bf16, float* cnorm,
+                         b200s_stream stream);
+/* k-means++ seeding over n rows (x: bf16 [n, D], row stride x_rs): centre 0 uniform, centre j drawn with probability
+ * d2[i] / sum d2 (fp64 prefix sums, counter-based hash keyed by (seed0, seed1)), d2[i] = min over chosen centres of
+ * |x_i - c|^2 (fp32 workspace [n]).  centers: fp32 [K, D] out (copies of the chosen bf16 rows).  *inertia (fp64, may be NULL) =
+ * sum d2 with all K centres chosen.  2K + 1 launches, no read-back. */
+int b200s_kmeanspp_init(const void* x, long long x_rs, int n, int D, int K, uint32_t seed0, uint32_t seed1, float* d2,
+                        float* centers, double* inertia, b200s_stream stream);
+
 /* ============================ on-device data path (csrc/datapath.cu) ============================ */
 /* Span masking of compute_mask_indices (WavLM/WavLM.py:35-159; static span length, overlapping spans) on the device, with the
  * library's counter-based RNG instead of numpy's (statistical parity): per row count = max(min_masks, floor(mask_prob sz / L + u)),

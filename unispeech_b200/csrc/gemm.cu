@@ -116,6 +116,13 @@ int make_qkv_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int
   return make_tmap(out, v);
 }
 
+// [batches, rows, cols] bf16 with arbitrary row / batch strides (elements): box = 64 columns x box_rows rows (k-means operands)
+int make_rows_tmap(CUtensorMap* out, const void* ptr, long long cols, long long rows, long long batches, long long row_stride,
+                   long long batch_stride, int box_rows) {
+  ViewSpec v{ptr, {cols, rows, batches, 1}, {row_stride, batches > 1 ? batch_stride : 0, 0}, {64, box_rows, 1, 1}};
+  return make_tmap(out, v);
+}
+
 // [B, T, cols] fp32 row-major (the attention backward's dQ accumulator): rank 3 (cols, T, B), so a box clips at T inside each
 // utterance; box = 32 columns (one 128-byte swizzle row) x box_rows rows.  Used as the destination of TMA reductions.
 int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_rows) {

@@ -399,6 +399,33 @@ def ctc_beta_grad(logits, frame_stride, batch_stride, lse, input_len, targets, S
           L.ptr(upstream), L.ptr(grad), L.ll(grad_frame_stride), L.ll(grad_batch_stride), i32(Vpad), _s())
 
 
+# ------------------------------------------------------------------------------------------------- k-means pseudo-labels
+def kmeans_assign(x, x_bs, x_rs, rows, batches, D, valid, centers_bf16, cnorm, K, labels, score=None, prev_labels=None,
+                  changed=None):
+    _call("b200s_kmeans_assign", L.ptr(x), L.ll(x_bs), L.ll(x_rs), i32(rows), i32(batches), i32(D), L.ptr(valid),
+          L.ptr(centers_bf16), L.ptr(cnorm), i32(K), L.ptr(labels), L.ptr(score), L.ptr(prev_labels), L.ptr(changed), _s(),
+          flops=2.0 * rows * batches * K * D)
+
+
+def kmeans_update_workspace(n, K, D) -> int:
+    return int(L.load().b200s_kmeans_update_workspace(L.ll(n), i32(K), i32(D)))
+
+
+def kmeans_update(x, x_rs, n, D, labels, score, K, workspace, counts, sums, inertia):
+    _call("b200s_kmeans_update", L.ptr(x), L.ll(x_rs), i32(n), i32(D), L.ptr(labels), L.ptr(score), i32(K), L.ptr(workspace),
+          L.ll(workspace.numel()), L.ptr(counts), L.ptr(sums), L.ptr(inertia), _s(), nbytes=2.0 * n * D)
+
+
+def kmeans_centers(sums, counts, K, D, centers, centers_bf16, cnorm):
+    _call("b200s_kmeans_centers", L.ptr(sums), L.ptr(counts), i32(K), i32(D), L.ptr(centers), L.ptr(centers_bf16), L.ptr(cnorm),
+          _s())
+
+
+def kmeanspp_init(x, x_rs, n, D, K, seed, d2, centers, inertia=None):
+    _call("b200s_kmeanspp_init", L.ptr(x), L.ll(x_rs), i32(n), i32(D), i32(K), u32(seed[0]), u32(seed[1]), L.ptr(d2),
+          L.ptr(centers), L.ptr(inertia), _s())
+
+
 # ------------------------------------------------------------------------------------------------- on-device data path
 def span_mask(valid_len, B, T, mask_prob, mask_length, min_masks, key, mask, counts):
     _call("b200s_span_mask", L.ptr(valid_len), i32(B), i32(T), f32(mask_prob), i32(mask_length), i32(min_masks), u32(key[0]),
