@@ -135,7 +135,7 @@ def test_sat_kernel_matches_reference_fixture(cuda_device):
     import numpy as np
     import torch.nn.functional as F
     from unispeech_b200 import ops
-    from unispeech_b200.unispeech_sat import sample_instances
+    from unispeech_b200.heads import sample_instances
     dev = cuda_device
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", "sat_heads.npz"))
     B, T, C, Dp, temp = 3, 14, 16, 8, 0.1

@@ -22,8 +22,8 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from . import _lib as L
 from . import dropout as DR
+from . import heads as H
 from . import ops
 from .engine import BF
 from .wavlm import WavLM, _on_forward_stream
@@ -46,16 +46,14 @@ class _OutputProjFn(torch.autograd.Function):
         Vp = (V + 63) // 64 * 64
         wpad = torch.zeros(Vp, D, dtype=torch.float32, device=dev)
         wpad[:V] = w
-        wp, wpT = torch.empty(Vp, D, dtype=BF, device=dev), torch.empty(D, Vp, dtype=BF, device=dev)
-        ops.prep_linear(wpad, Vp, D, 1.0, wp, D, wpT, Vp)
+        wp, wpT = H.linear_operands(wpad)
         bpad = torch.zeros(Vp, dtype=torch.float32, device=dev)
         bpad[:V] = b
         xd = x2d
         if p_drop > 0:
             xd = torch.empty_like(x2d)
             ops.dropout_rows(x2d, 0, D, None, 0, 0, xd, 0, D, R, 1, D, p_drop, key)
-        y = torch.empty(R, Vp, dtype=BF, device=dev)
-        ops.gemm_rows(xd, 0, D, R, 1, D, wp, Vp, y, 0, Vp, L.make_epilogue(bias=bpad))
+        y = H.linear_rows(xd, wp, bpad)
         ctx.xd, ctx.wpT, ctx.dims, ctx.drop = xd, wpT, (R, D, V, Vp), (p_drop, key)
         return y[:, :V]
 
@@ -67,11 +65,8 @@ class _OutputProjFn(torch.autograd.Function):
         dyp = torch.zeros(R, Vp, dtype=BF, device=dev)
         dyp[:, :V] = dy
         db = torch.zeros(Vp, dtype=torch.float32, device=dev)
-        ops.colsum(dyp, 0, Vp, R, 1, Vp, db)
         dw = torch.zeros(Vp, D, dtype=torch.float32, device=dev)
-        ops.gemm_wgrad(dyp, 0, Vp, ctx.xd, 0, D, R, 1, Vp, D, dw, D)
-        dx = torch.empty(R, D, dtype=BF, device=dev)
-        ops.gemm_rows(dyp, 0, Vp, R, 1, Vp, ctx.wpT, D, dx, 0, D, None)
+        dx = H.linear_rows_backward(dyp, ctx.xd, ctx.wpT, dw, db)
         p_drop, key = ctx.drop
         if p_drop > 0:
             ops.dropout_rows(dx, 0, D, None, 0, 0, dx, 0, D, R, 1, D, p_drop, key)
@@ -130,9 +125,7 @@ class _EncoderBase(nn.Module):
         if self.proj is None and p == 0.0:
             return x_btc.transpose(0, 1) if tbc else x_btc
         B, T, D = x_btc.shape
-        x2d = x_btc.reshape(B * T, D)
-        if x2d.dtype != BF or not x2d.is_contiguous():
-            x2d = x2d.to(BF).contiguous()
+        x2d = H.bf16(x_btc.reshape(B * T, D))
         seed = self.dropout_seed if self.dropout_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
         key = DR.site_key(seed, _SITE_FINAL)
         if self.proj is None:

@@ -16,9 +16,10 @@ from typing import Dict, List, Optional
 import torch
 import torch.nn as nn
 
-from . import _lib as L
+from . import heads as H
 from . import ops
 from .engine import BF
+from .heads import _rows
 from .wavlm import WavLM, WavLMConfig, _on_forward_stream
 
 
@@ -37,24 +38,17 @@ class WavLMPretrainConfig(WavLMConfig):
         super().__init__(cfg)
 
 
-def _rows(n, C, dtype, dev):
-    return torch.empty(n, C, dtype=dtype, device=dev)
-
-
 def _head_forward(model, x2d, w, b, label_embs, idx):
     """Shared front of the masked-prediction head: gather the selected frames, final_proj, and per label set the GEMM against the
     row-normalised label embeddings.  Returns the state both the fused criterion and the materialising logits path build on."""
     dev = x2d.device
-    S, D = idx.numel(), x2d.shape[1]
+    S = idx.numel()
     Dp = model.final_dim
     Dt = w.shape[0]
     untie = model.untie_final_proj
-    wp, wpT = torch.empty(Dt, D, dtype=BF, device=dev), torch.empty(D, Dt, dtype=BF, device=dev)
-    ops.prep_linear(w, Dt, D, 1.0, wp, D, wpT, Dt)
-    xs = _rows(S, D, BF, dev)
-    ops.gather_rows(x2d, D, idx, S, D, xs, D)
-    proj = _rows(S, Dt, BF, dev)
-    ops.gemm_rows(xs, 0, D, S, 1, D, wp, Dt, proj, 0, Dt, L.make_epilogue(bias=b))
+    wp, wpT = H.linear_operands(w)
+    xs = H.gather(x2d, idx)
+    proj = H.linear_rows(xs, wp, b)
     sets, off = [], 0
     for i, C in enumerate(model.num_classes):
         Cpad = (C + 63) // 64 * 64
@@ -67,18 +61,16 @@ def _head_forward(model, x2d, w, b, label_embs, idx):
         ops.gemm_rows(proj_i, 0, Dt, S, 1, Dp, en, Cpad, zraw, 0, Cpad, None)
         sets.append(dict(off=off, C=C, Cpad=Cpad, en_t=en_t, invn=invn, zraw=zraw))
         off += C
-    return dict(xs=xs, proj=proj, wpT=wpT, sets=sets, shape=(x2d.shape[0], D, S, Dp, Dt, untie))
+    return dict(xs=xs, proj=proj, wpT=wpT, sets=sets, shape=(x2d.shape[0], S, Dp, Dt, untie))
 
 
-def _head_backward(model, eng, st, label_embs, idx, Gs, pns, rvecs, grads=None):
+def _head_backward(st, label_embs, idx, Gs, pns, rvecs, grads):
     """Shared back of the head.  Gs[i] = d loss / d (proj . En^T) (bf16 [S, Cpad]), rvecs[i] = sum_c G_sc cos_sc, pns[i] = 1/|proj_s|:
     d proj = G En - rvec pn proj,  d En = G^T proj,  then final_proj's weight / bias / input gradients and the scatter back.
-    `grads` = (d label_embs [sum C, Dp], d final_proj.weight, d final_proj.bias) fp32 views to accumulate into; default: the
-    flat-buffer views of `model.label_embs_concat` / `model.final_proj` (models with one head per layer pass their own)."""
-    rows, D, S, Dp, Dt, untie = st["shape"]
+    `grads` = (d label_embs [sum C, Dp], d final_proj.weight, d final_proj.bias): fp32 views to accumulate into."""
+    rows, S, Dp, Dt, untie = st["shape"]
     dev = st["xs"].device
-    g = eng.g
-    g_emb, g_w, g_b = grads if grads is not None else (g(model.label_embs_concat), g(model.final_proj.weight), g(model.final_proj.bias))
+    g_emb, g_w, g_b = grads
     dproj = _rows(S, Dt, BF, dev)
     for i, se in enumerate(st["sets"]):
         off, C, Cpad = se["off"], se["C"], se["Cpad"]
@@ -92,20 +84,14 @@ def _head_backward(model, eng, st, label_embs, idx, Gs, pns, rvecs, grads=None):
         d_en = torch.zeros(Cpad, Dp, dtype=torch.float32, device=dev)
         ops.gemm_wgrad(Gs[i], 0, Cpad, proj_i, 0, Dt, S, 1, Cpad, Dp, d_en, Dp)                          # G^T proj
         ops.nce_dlabel(d_en, label_embs[off:off + C], se["invn"], C, Dp, g_emb[off:off + C])
-    ops.colsum(dproj, 0, Dt, S, 1, Dt, g_b)
-    ops.gemm_wgrad(dproj, 0, Dt, st["xs"], 0, D, S, 1, Dt, D, g_w, D)
-    dxs = _rows(S, D, BF, dev)
-    ops.gemm_rows(dproj, 0, Dt, S, 1, Dt, st["wpT"], D, dxs, 0, D, None)
-    dx = torch.zeros(rows, D, dtype=BF, device=dev)
-    ops.scatter_add_rows(dxs, D, idx, S, D, dx, D)
-    return dx
+    return H.scatter(H.linear_rows_backward(dproj, st["xs"], st["wpT"], g_w, g_b), idx, rows)
 
 
 class _MaskedPredictionFn(torch.autograd.Function):
     """loss = sum over label sets of weight * CE(cos(final_proj(x[idx]), label_embs) / temp, target).  x: bf16 [B*T, D]."""
 
     @staticmethod
-    def forward(ctx, x2d, w, b, label_embs, model, idx, targets, weight, stats, grads=None):
+    def forward(ctx, x2d, w, b, label_embs, model, idx, targets, weight, stats, grads):
         ctx.fwd_stream = torch.cuda.current_stream()
         ctx.grad_views = grads
         dev = x2d.device
@@ -126,7 +112,7 @@ class _MaskedPredictionFn(torch.autograd.Function):
             stats.append(dict(loss=part, correct=correct, count=S))
             se["zraw"] = None
             Gs.append(G); pns.append(pn); rvecs.append(rvec)
-        ctx.model, ctx.eng, ctx.idx, ctx.st, ctx.grads = model, model._engine, idx, st, (Gs, pns, rvecs)
+        ctx.idx, ctx.st, ctx.grads = idx, st, (Gs, pns, rvecs)
         ctx.save_for_backward(w, b, label_embs)
         return loss_sum.float().reshape(())
 
@@ -139,7 +125,7 @@ class _MaskedPredictionFn(torch.autograd.Function):
         for G, rvec in zip(Gs, rvecs):
             G.mul_(scale_bf)     # upstream gradient of the scalar loss (device scalar, no sync): everything below is linear in G
             rvec.mul_(scale_f)
-        dx = _head_backward(ctx.model, ctx.eng, ctx.st, label_embs, ctx.idx, Gs, pns, rvecs, ctx.grad_views)
+        dx = _head_backward(ctx.st, label_embs, ctx.idx, Gs, pns, rvecs, ctx.grad_views)
         ctx.st = ctx.grads = None
         return dx, None, None, None, None, None, None, None, None, None
 
@@ -151,7 +137,7 @@ class _LogitsFn(torch.autograd.Function):
     model through `get_logits` / `get_targets`.  Same GEMMs as the fused criterion; the logits are assembled from their outputs."""
 
     @staticmethod
-    def forward(ctx, x2d, w, b, label_embs, model, idx, targets, grads=None):
+    def forward(ctx, x2d, w, b, label_embs, model, idx, targets, grads):
         ctx.fwd_stream = torch.cuda.current_stream()
         ctx.grad_views = grads
         st = _head_forward(model, x2d, w, b, label_embs, idx)
@@ -166,7 +152,7 @@ class _LogitsFn(torch.autograd.Function):
             pos = z.gather(1, t)
             outs.append(torch.cat([pos, z.scatter(1, t, float("-inf"))], dim=1))
             pns.append(pn)
-        ctx.model, ctx.eng, ctx.idx, ctx.st, ctx.pns, ctx.targets = model, model._engine, idx, st, pns, targets
+        ctx.model, ctx.idx, ctx.st, ctx.pns, ctx.targets = model, idx, st, pns, targets
         ctx.save_for_backward(w, b, label_embs)
         return tuple(outs)
 
@@ -191,7 +177,7 @@ class _LogitsFn(torch.autograd.Function):
             G = torch.zeros(S, Cpad, dtype=BF, device=dev)
             G[:, :C] = Gf.to(BF)
             Gs.append(G)
-        dx = _head_backward(model, ctx.eng, st, label_embs, ctx.idx, Gs, ctx.pns, rvecs, ctx.grad_views)
+        dx = _head_backward(st, label_embs, ctx.idx, Gs, ctx.pns, rvecs, ctx.grad_views)
         ctx.st = None
         return dx, None, None, None, None, None, None, None
 
@@ -246,40 +232,59 @@ class WavLMForPretraining(WavLM):
             names.append("features_pen")
         return extra_losses, names
 
-    def _selection(self, net_output, masked: bool):
-        """Host-side frame selection of the criterion: flat indices of the masked (or unmasked) unpadded frames + their labels."""
-        x = net_output["x"]
-        B, T, D = x.shape
-        dev = x.device
-        mi, pm, targets = net_output["mask_indices"], net_output["padding_mask"], net_output["target_list"]
-        assert mi is not None and targets is not None, "forward(..., target_list=..., mask=True) must run first"
-        mi_h = mi.cpu() if mi.device.type != "cpu" else mi
-        pm_h = net_output.get("padding_mask_host")
+    # ---- frame selection (host), shared by the criterion and the materialising logits path
+    @staticmethod
+    def _host_masks(out):
+        """Host copies of the span mask and the frame padding mask of a forward result.  Frames are selected on the host, like
+        the reference's collater-side masks: with a host padding mask there is no device round trip at all (a device-only mask
+        costs one synchronising copy here)."""
+        mi_h = out["mask_indices"].cpu()
+        pm, pm_h = out["padding_mask"], out.get("padding_mask_host")
         if pm_h is None:
-            pm_h = torch.zeros(B, T, dtype=torch.bool) if pm is None else (pm.cpu() if pm.device.type != "cpu" else pm)
-        sel = torch.logical_and(~pm_h, mi_h if masked else ~mi_h)
+            pm_h = torch.zeros(mi_h.shape, dtype=torch.bool) if pm is None else pm.cpu()
+        return mi_h, pm_h
+
+    def _plans(self, net_output, pred_masked_weight, pred_nomask_weight):
+        """(tag, host frame selection, weight) of the masked ("m") and unmasked ("u") terms that are switched on."""
+        assert net_output["mask_indices"] is not None and net_output["target_list"] is not None, \
+            "forward(..., target_list=..., mask=True) must run first"
+        mi_h, pm_h = self._host_masks(net_output)
+        plans = []
+        if not self.skip_masked and pred_masked_weight > 0:
+            plans.append(("m", torch.logical_and(~pm_h, mi_h), pred_masked_weight))
+        if not self.skip_nomask and pred_nomask_weight > 0:
+            plans.append(("u", torch.logical_and(~pm_h, ~mi_h), pred_nomask_weight))
+        return plans
+
+    @staticmethod
+    def _select(sel, targets, dev):
+        """Flat indices of the selected frames (host, and int32 on the device) and their labels (int32, device)."""
         idx_h = torch.nonzero(sel.reshape(-1), as_tuple=False).squeeze(1)
         idx = idx_h.to(torch.int32).to(dev, non_blocking=True)
         tg = [t.reshape(-1).to(dev)[idx.long()].to(torch.int32).contiguous() if t.device.type != "cpu"
               else t.reshape(-1)[idx_h].to(torch.int32).to(dev, non_blocking=True) for t in targets]
         return idx_h, idx, tg
 
+    def _heads(self, net_output):
+        """Each masked-prediction head: (bf16 [B*T, D] rows it reads, final_proj weight, bias, label embeddings, the fp32 gradient
+        views of those three, weight of its loss or None).  One head here, on the encoder output."""
+        g = self._engine.g
+        fp, emb = self.final_proj, self.label_embs_concat
+        x = net_output["x"]
+        yield H.bf16(x.reshape(-1, x.shape[-1])), fp.weight, fp.bias, emb, (g(emb), g(fp.weight), g(fp.bias)), None
+
     def get_logits(self, net_output, is_masked=True):
-        """`[S, C+1]` float logit list of the reference (wavlm.py:599-607), one per label set, positives in column 0.  Opt-in
-        materialising path (the fused `criterion` never builds these); differentiable, cached in `net_output`."""
+        """`[S, C+1]` float logit list of the reference (wavlm.py:599-607), one per head and label set (head-major), positives in
+        column 0.  Opt-in materialising path (the fused `criterion` never builds these); differentiable, cached in `net_output`."""
         key = "logit_m_list" if is_masked else "logit_u_list"
         if net_output.get(key) is None:
-            skip = self.skip_masked if is_masked else self.skip_nomask
-            idx_h, idx, tg = self._selection(net_output, is_masked)
-            if skip or idx_h.numel() == 0:
-                net_output[key] = [None for _ in self.num_classes]
-            else:
-                x = net_output["x"]
-                x2d = x.reshape(-1, x.shape[-1])
-                if x2d.dtype != BF or not x2d.is_contiguous():
-                    x2d = x2d.to(BF).contiguous()
-                net_output[key] = list(_LogitsFn.apply(x2d, self.final_proj.weight, self.final_proj.bias, self.label_embs_concat,
-                                                       self, idx, tg))
+            plans = self._plans(net_output, float(is_masked), float(not is_masked))
+            idx_h, idx, tg = self._select(plans[0][1], net_output["target_list"], net_output["x"].device) if plans else (None,) * 3
+            lst = []
+            for x2d, w, b, emb, grads, _ in self._heads(net_output):
+                lst += (_LogitsFn.apply(x2d, w, b, emb, self, idx, tg, grads) if idx_h is not None and idx_h.numel()
+                        else [None] * len(self.num_classes))
+            net_output[key] = lst
         return [lg.float() for lg in net_output[key] if lg is not None]
 
     def get_targets(self, net_output, is_masked=True):
@@ -306,55 +311,33 @@ class WavLMForPretraining(WavLM):
 
     def criterion(self, net_output: Dict, pred_masked_weight: float = 1.0, pred_nomask_weight: float = 0.0,
                   loss_weights: Optional[List[float]] = None):
-        """WavLMCriterion.get_loss (wavlm_criterion.py:52-138): returns (loss, sample_size, logging_output) with `loss` a
-        device scalar; logging values stay device tensors (call `.item()` when you log)."""
+        """WavLMCriterion.get_loss (wavlm_criterion.py:52-138; for several heads HubertCriterion.get_loss over the head-major list,
+        hubert_criterion.py:52-110): returns (loss, sample_size, logging_output) with `loss` a device scalar; logging values stay
+        device tensors (call `.item()` when you log)."""
         x = net_output["x"]
-        B, T, D = x.shape
-        dev = x.device
-        mi, pm, targets = net_output["mask_indices"], net_output["padding_mask"], net_output["target_list"]
-        assert mi is not None and targets is not None, "forward(..., target_list=..., mask=True) must run first"
-        mi_h = mi.cpu() if mi.device.type != "cpu" else mi
-        # frame selection happens on the host, like the reference's collater-side masks: with a host padding mask there is no
-        # device round trip at all (a device-only mask costs one synchronising copy here)
-        pm_h = net_output.get("padding_mask_host")
-        if pm_h is None:
-            pm_h = torch.zeros(B, T, dtype=torch.bool) if pm is None else (pm.cpu() if pm.device.type != "cpu" else pm)
-        x2d = x.reshape(B * T, D)
-        if x2d.dtype != BF or not x2d.is_contiguous():
-            x2d = x2d.to(BF).contiguous()
         loss, sample_size, log = 0.0, 0, {}
-        plans = []
-        if not self.skip_masked and pred_masked_weight > 0:
-            plans.append(("m", torch.logical_and(~pm_h, mi_h), pred_masked_weight))
-        if not self.skip_nomask and pred_nomask_weight > 0:
-            plans.append(("u", torch.logical_and(~pm_h, ~mi_h), pred_nomask_weight))
+        plans = self._plans(net_output, pred_masked_weight, pred_nomask_weight)
+        heads = list(self._heads(net_output))
         for tag, sel, wgt in plans:
-            idx_h = torch.nonzero(sel.reshape(-1), as_tuple=False).squeeze(1)
+            idx_h, idx, tg = self._select(sel, net_output["target_list"], x.device)
             if idx_h.numel() == 0:
                 continue
-            idx = idx_h.to(torch.int32).to(dev, non_blocking=True)
-            tg = [t.reshape(-1).to(dev)[idx.long()].to(torch.int32).contiguous() if t.device.type != "cpu"
-                  else t.reshape(-1)[idx_h].to(torch.int32).to(dev, non_blocking=True) for t in targets]
-            stats = []
-            part = _MaskedPredictionFn.apply(x2d, self.final_proj.weight, self.final_proj.bias, self.label_embs_concat, self, idx,
-                                             tg, float(wgt), stats)
-            loss = loss + part
-            sample_size += idx_h.numel()
-            for i, st in enumerate(stats):
-                log[f"loss_{tag}_{i}"] = st["loss"] / wgt
-                log[f"correct_{tag}_{i}"] = st["correct"]
-                log[f"count_{tag}_{i}"] = st["count"]
-        if loss_weights is not None:  # wavlm_criterion.py:89-103: every extra loss the model reports, weight x value x sample_size
+            k = 0
+            for x2d, w, b, emb, grads, lw in heads:
+                stats = []
+                part = _MaskedPredictionFn.apply(x2d, w, b, emb, self, idx, tg, float(wgt), stats, grads)
+                loss = loss + (part if lw is None else lw * part)
+                for st in stats:
+                    log[f"loss_{tag}_{k}"] = st["loss"] / wgt
+                    log[f"correct_{tag}_{k}"] = st["correct"]
+                    log[f"count_{tag}_{k}"] = st["count"]
+                    k += 1
+            sample_size += idx_h.numel()   # once per plan, whatever the number of heads (hubert_criterion.py:75, 91)
+        if loss_weights is not None:  # every extra loss the model reports, weight x value x sample_size
             extra_losses, names = self.get_extra_losses(net_output)
-            lw = list(loss_weights)
-            if len(lw) == 1 and len(extra_losses) != 1:
-                lw = [lw[0]] * len(extra_losses)
-            assert len(extra_losses) == len(lw), f"{len(extra_losses)}, {len(lw)}"
-            for p, n, coef in zip(extra_losses, names, lw):
-                if coef != 0 and p is not None:
-                    p = coef * p.float() * sample_size
-                    loss = loss + p
-                    log[f"loss_{n}"] = p.detach()
-        log.update(ntokens=sample_size, sample_size=sample_size, nsentences=B)
+            for i, p in H.weighted_extra_losses(extra_losses, loss_weights, sample_size):
+                loss = loss + p
+                log[f"loss_{names[i]}"] = p.detach()
+        log.update(ntokens=sample_size, sample_size=sample_size, nsentences=x.shape[0])
         log["loss"] = loss.detach() if torch.is_tensor(loss) else loss
         return loss, sample_size, log

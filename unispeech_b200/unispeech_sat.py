@@ -7,7 +7,8 @@ Mirrors src/fairseq/models/unispeech_sat/unispeech_sat.py: constructor tail :383
 `mean_targets`, `contrastive_acc`, `loss_spk_u`, `prob_perplexity`, `code_perplexity`, `num_vars`, `temp`), `sample_instances`
 :487-543 (host `torch.randint`, same call order: reproducible under `torch.manual_seed`), `compute_nce` :545-557,
 `get_extra_losses` :795-820, `remove_pretraining_modules` :822-834, and `GumbelVectorQuantizer`
-(src/fairseq/modules/gumbel_vector_quantizer.py:13-201: `set_num_updates` temperature schedule :85-88, forward :141-201).
+(src/fairseq/modules/gumbel_vector_quantizer.py:13-201: `set_num_updates` temperature schedule :85-88, forward :141-201); the
+last two live in heads.py, shared with wav2vec 2.0.
 Training-mode Gumbel noise comes from the library's counter-based hash (the reference's Philox stream cannot be reproduced;
 the CPU checker restates this generator, as for dropout).
 """
@@ -18,11 +19,12 @@ from typing import Dict, List, Optional
 import torch
 import torch.nn as nn
 
-from . import _lib as L
 from . import dropout as DR
+from . import heads as H
 from . import ops
 from .engine import BF
-from .pretrain import WavLMForPretraining, WavLMPretrainConfig, _rows
+from .heads import GumbelVectorQuantizer, _rows, sample_instances
+from .pretrain import WavLMForPretraining, WavLMPretrainConfig
 from .wavlm import _on_forward_stream
 
 _SITE_GUMBEL = 0x7F000002  # noise site of the quantizer (distinct from every dropout site)
@@ -45,48 +47,6 @@ class UniSpeechSATConfig(WavLMPretrainConfig):
         super().__init__(cfg)
 
 
-class GumbelVectorQuantizer(nn.Module):
-    """Parameter container + temperature schedule of the reference module (time_first, combine_groups=False, weight_proj_depth=1)."""
-
-    def __init__(self, dim, num_vars, temp, groups, vq_dim):
-        super().__init__()
-        assert vq_dim % groups == 0
-        self.groups, self.num_vars, self.input_dim = groups, num_vars, dim
-        self.vars = nn.Parameter(torch.FloatTensor(1, groups * num_vars, vq_dim // groups))
-        nn.init.uniform_(self.vars)
-        self.weight_proj = nn.Linear(dim, groups * num_vars)
-        nn.init.normal_(self.weight_proj.weight, mean=0, std=1)
-        nn.init.zeros_(self.weight_proj.bias)
-        self.max_temp, self.min_temp, self.temp_decay = temp
-        self.curr_temp = self.max_temp
-
-    def set_num_updates(self, num_updates):
-        self.curr_temp = max(self.max_temp * self.temp_decay ** num_updates, self.min_temp)
-
-
-def sample_instances(bsz: int, num: int, n_instances: int, cross_sample_instances: int, generator=None) -> torch.Tensor:
-    """Flat row indices [bsz, (n + c) * num] into y.view(-1, C) drawn exactly like unispeech_sat.py:487-533 (host RNG: the same
-    `torch.randint` calls in the same order; `idx[idx >= tszs] += 1` is written as `idx += (idx >= tszs)`, which is the same
-    update without the boolean gather / scatter -- half of the reference formulation's host time)."""
-    cross_high, high = num * bsz, num
-    assert high > 1, (bsz, num)
-    if n_instances > 0:
-        tszs = torch.arange(num).unsqueeze(-1).expand(-1, n_instances).flatten()
-        instance_idxs = torch.randint(low=0, high=high - 1, size=(bsz, n_instances * num), generator=generator)
-        instance_idxs += (instance_idxs >= tszs)
-    if cross_sample_instances > 0:
-        tszs = torch.arange(num).unsqueeze(-1).expand(-1, cross_sample_instances).flatten()
-        cross_instance_idxs = torch.randint(low=0, high=cross_high - 1, size=(bsz, cross_sample_instances * num), generator=generator)
-        cross_instance_idxs += (cross_instance_idxs >= tszs)
-    if n_instances > 0:
-        instance_idxs += (torch.arange(bsz) * high).unsqueeze(1)
-    else:
-        instance_idxs = cross_instance_idxs
-    if cross_sample_instances > 0 and n_instances > 0:
-        instance_idxs = torch.cat([instance_idxs, cross_instance_idxs], dim=1)
-    return instance_idxs
-
-
 _DRAW_POOL = None
 
 
@@ -106,44 +66,17 @@ class _SpkNceFn(torch.autograd.Function):
     def forward(ctx, spk2d, anchor, model, rows_idx, inst_idx, same, S, N, gum_key, stats_out):
         ctx.fwd_stream = torch.cuda.current_stream()
         dev = spk2d.device
-        D = spk2d.shape[1]
         Dp = model.final_dim
-        sp, qz = model.spk_proj, model.quantizer
-        xs = _rows(S, D, BF, dev)
-        ops.gather_rows(spk2d, D, rows_idx, S, D, xs, D)
-        wsp, wspT = torch.empty(Dp, D, dtype=BF, device=dev), torch.empty(D, Dp, dtype=BF, device=dev)
-        ops.prep_linear(sp.weight, Dp, D, 1.0, wsp, D, wspT, Dp)
-        proj = _rows(S, Dp, BF, dev)
-        ops.gemm_rows(xs, 0, D, S, 1, D, wsp, Dp, proj, 0, Dp, L.make_epilogue(bias=sp.bias))
-        st = dict(xs=xs, proj=proj, wspT=wspT, quant=None)
-        y = proj
+        sp, qz, pq = model.spk_proj, model.quantizer, model.project_q
+        xs = H.gather(spk2d, rows_idx)
+        wsp, wspT = H.linear_operands(sp.weight)
+        proj = H.linear_rows(xs, wsp, sp.bias)
+        y, qs = proj, None
         if qz is not None:
-            G, V = qz.groups, qz.num_vars
-            dv = qz.vars.shape[-1]
-            GV, vq_dim = G * V, G * dv
-            wq, wqT = torch.empty(GV, D, dtype=BF, device=dev), torch.empty(D, GV, dtype=BF, device=dev)
-            ops.prep_linear(qz.weight_proj.weight, GV, D, 1.0, wq, D, wqT, GV)
-            logits = _rows(S, GV, BF, dev)
-            ops.gemm_rows(xs, 0, D, S, 1, D, wq, GV, logits, 0, GV, L.make_epilogue(bias=qz.weight_proj.bias))
-            codes = torch.empty(S * G, dtype=torch.int32, device=dev)
-            q = _rows(S, vq_dim, BF, dev)
-            counts = torch.zeros(GV, dtype=torch.float32, device=dev)
-            probs = torch.zeros(GV, dtype=torch.float32, device=dev)
-            training = model.training
-            ops.vq_hard(logits, GV, qz.vars, S, G, V, dv, codes, q, vq_dim, counts, probs, gumbel=training, key=gum_key)
-            pq = model.project_q
-            wpq, wpqT = torch.empty(Dp, vq_dim, dtype=BF, device=dev), torch.empty(vq_dim, Dp, dtype=BF, device=dev)
-            ops.prep_linear(pq.weight, Dp, vq_dim, 1.0, wpq, vq_dim, wpqT, Dp)
-            y = _rows(S, Dp, BF, dev)
-            ops.gemm_rows(q, 0, vq_dim, S, 1, vq_dim, wpq, Dp, y, 0, Dp, L.make_epilogue(bias=pq.bias))
-            # perplexities (gumbel_vector_quantizer.py:152-170): tiny [G, V] reductions of the kernel's accumulators
-            hard_probs = (counts / S).view(G, V)
-            avg_probs = (probs / S).view(G, V).detach().requires_grad_(False)
-            stats_out["code_perplexity"] = torch.exp(-torch.sum(hard_probs * torch.log(hard_probs + 1e-7), dim=-1)).sum()
-            stats_out["num_vars"] = V * G
-            stats_out["temp"] = qz.curr_temp
-            st["quant"] = dict(G=G, V=V, dv=dv, logits=logits, codes=codes, q=q, wqT=wqT, wpqT=wpqT, avg_probs=avg_probs,
-                               training=training, tau=float(qz.curr_temp))
+            q, qs = qz.forward_rows(xs, gum_key, stats_out)
+            wpq, wpqT = H.linear_operands(pq.weight)
+            y = H.linear_rows(q, wpq, pq.bias)
+            qs.update(q=q, wpqT=wpqT)
         g = torch.empty(S, N + 1, dtype=torch.float32, device=dev)
         loss64 = torch.zeros(1, dtype=torch.float64, device=dev)
         stats = torch.zeros(2, dtype=torch.int32, device=dev)
@@ -151,12 +84,11 @@ class _SpkNceFn(torch.autograd.Function):
         tot = float(S * (N + 1))
         stats_out["contrastive_acc"] = stats[0].float() / tot
         stats_out["mean_targets"] = stats[1].float() / tot
-        st.update(y=y, g=g)
-        ctx.model, ctx.st, ctx.sel, ctx.dims, ctx.key = model, st, (rows_idx, inst_idx), (spk2d.shape[0], D, S, N, Dp), gum_key
+        ctx.model, ctx.sel, ctx.rows = model, (rows_idx, inst_idx), spk2d.shape[0]
+        ctx.st = dict(xs=xs, proj=proj, wspT=wspT, y=y, g=g, quant=qs)
         outs = [loss64.float().reshape(())]
         if qz is not None:
-            ap = st["quant"]["avg_probs"]
-            outs.append(torch.exp(-torch.sum(ap * torch.log(ap + 1e-7), dim=-1)).sum())  # prob_perplexity (differentiable below)
+            outs.append(H.perplexity(qs["avg_probs"]).sum())  # prob_perplexity (differentiable below)
         return tuple(outs)
 
     @staticmethod
@@ -164,10 +96,10 @@ class _SpkNceFn(torch.autograd.Function):
     def backward(ctx, dloss, dppl=None):
         model, st = ctx.model, ctx.st
         rows_idx, inst_idx = ctx.sel
-        rows, D, S, N, Dp = ctx.dims
+        S, Dp = st["proj"].shape
+        N = st["g"].shape[1] - 1
         dev = st["xs"].device
-        eng = model._engine
-        g_ = eng.g
+        g_ = model._engine.g
         qs = st["quant"]
         up = (dloss if dloss is not None else torch.zeros((), device=dev)).float().reshape(1).contiguous()
         dacc_p = torch.zeros(S, Dp, dtype=torch.float32, device=dev)
@@ -175,51 +107,18 @@ class _SpkNceFn(torch.autograd.Function):
         ops.sat_nce_bwd(st["proj"], Dp, st["y"], Dp, inst_idx, S, N, Dp, model.logit_temp, st["g"], up, dacc_p, dacc_y)
         dproj = _rows(S, Dp, BF, dev)
         ops.f32_to_bf16_rows(dacc_p, Dp, dproj, Dp, S, Dp)
-        sp = model.spk_proj
-        ops.colsum(dproj, 0, Dp, S, 1, Dp, g_(sp.bias))
-        ops.gemm_wgrad(dproj, 0, Dp, st["xs"], 0, D, S, 1, Dp, D, g_(sp.weight), D)
-        dxs = _rows(S, D, BF, dev)
-        dlogits = None
+        dxq = None
         if qs is not None:
-            G, V, dv = qs["G"], qs["V"], qs["dv"]
-            GV, vq_dim = G * V, G * dv
-            qz, pq = model.quantizer, model.project_q
+            pq = model.project_q
             dy = _rows(S, Dp, BF, dev)
             ops.f32_to_bf16_rows(dacc_y, Dp, dy, Dp, S, Dp)
-            ops.colsum(dy, 0, Dp, S, 1, Dp, g_(pq.bias))
-            ops.gemm_wgrad(dy, 0, Dp, qs["q"], 0, vq_dim, S, 1, Dp, vq_dim, g_(pq.weight), vq_dim)
-            dq = _rows(S, vq_dim, BF, dev)
-            ops.gemm_rows(dy, 0, Dp, S, 1, Dp, qs["wpqT"], vq_dim, dq, 0, vq_dim, None)
-            ops.vq_dvars(dq, vq_dim, qs["codes"], S, G, V, dv, g_(qz.vars).view(GV, dv))
-            # gradient of the logits: diversity term (through avg_probs) and, in training mode, the straight-through estimator
-            c = None
-            if dppl is not None:
-                ap = qs["avg_probs"]
-                ppl_g = torch.exp(-torch.sum(ap * torch.log(ap + 1e-7), dim=-1, keepdim=True))   # [G, 1]
-                c = (dppl.float() * ppl_g * (-torch.log(ap + 1e-7) - ap / (ap + 1e-7))).reshape(-1).contiguous()
-            h = None
-            if qs["training"]:
-                vb, vbT = torch.empty(GV, dv, dtype=BF, device=dev), torch.empty(dv, GV, dtype=BF, device=dev)
-                ops.prep_linear(qz.vars.view(GV, dv), GV, dv, 1.0, vb, dv, vbT, GV)
-                h = _rows(S, GV, BF, dev)
-                for grp in range(G):   # h[s, g, v] = dq[s, g, :] . vars[g, v, :]
-                    ops.gemm_rows(dq.view(-1)[grp * dv:], 0, vq_dim, S, 1, dv, vb[grp * V:(grp + 1) * V], V, h.view(-1)[grp * V:], 0,
-                                  GV, None)
-            if c is not None or h is not None:
-                dlogits = _rows(S, GV, BF, dev)
-                ops.vq_logits_bwd(qs["logits"], GV, S, G, V, c, h, GV, qs["tau"], ctx.key, dlogits, GV)
-                ops.colsum(dlogits, 0, GV, S, 1, GV, g_(qz.weight_proj.bias))
-                ops.gemm_wgrad(dlogits, 0, GV, st["xs"], 0, D, S, 1, GV, D, g_(qz.weight_proj.weight), D)
-        if dlogits is not None:
-            dxs2 = _rows(S, D, BF, dev)
-            ops.gemm_rows(dlogits, 0, dlogits.shape[1], S, 1, dlogits.shape[1], qs["wqT"], D, dxs2, 0, D, None)
-            ops.gemm_rows(dproj, 0, Dp, S, 1, Dp, st["wspT"], D, dxs, 0, D, L.make_epilogue(res1=dxs2, res1_ld=D))
-        else:
-            ops.gemm_rows(dproj, 0, Dp, S, 1, Dp, st["wspT"], D, dxs, 0, D, None)
-        dx = torch.zeros(rows, D, dtype=BF, device=dev)
-        ops.scatter_add_rows(dxs, D, rows_idx, S, D, dx, D)
+            dq = H.linear_rows_backward(dy, qs["q"], qs["wpqT"], g_(pq.weight), g_(pq.bias))
+            dxq = model.quantizer.backward_rows(qs, dq, dppl, g_)
+        # spk_proj's gradients come last: the quantizer's input gradient is added in the epilogue of spk_proj's input GEMM
+        sp = model.spk_proj
+        dxs = H.linear_rows_backward(dproj, st["xs"], st["wspT"], g_(sp.weight), g_(sp.bias), res=dxq)
         ctx.st = None
-        return dx, None, None, None, None, None, None, None, None, None
+        return H.scatter(dxs, rows_idx, ctx.rows), None, None, None, None, None, None, None, None, None
 
 
 class UniSpeechSATForPretraining(WavLMForPretraining):
@@ -341,18 +240,12 @@ class UniSpeechSATForPretraining(WavLMForPretraining):
             out.update(loss_spk_m=None, mean_targets=None, contrastive_acc=None)
             return out
         if pre is None:   # device-resident masks: the frame selection needs them on the host first
-            mi, pm = res["mask_indices"], res["padding_mask"]
-            assert mi is not None, "the utterance-contrastive loss needs mask=True"
-            mi_h = mi.cpu() if mi.device.type != "cpu" else mi
-            pm_h = res.get("padding_mask_host")
-            if pm_h is None:
-                pm_h = torch.zeros(B, T, dtype=torch.bool) if pm is None else (pm.cpu() if pm.device.type != "cpu" else pm)
+            assert res["mask_indices"] is not None, "the utterance-contrastive loss needs mask=True"
+            mi_h, pm_h = self._host_masks(res)
             pre = self._draw_instances(mi_h.bool(), pm_h, None, dev)
         S, N = pre["S"], pre["N"]
         up = lambda t: t.to(dev, non_blocking=True)
-        spk2d = spk_x.reshape(B * T, D)
-        if spk2d.dtype != BF or not spk2d.is_contiguous():
-            spk2d = spk2d.to(BF).contiguous()
+        spk2d = H.bf16(spk_x.reshape(B * T, D))
         seed = self.noise_seed if self.noise_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
         stats: Dict = {}
         outs = _SpkNceFn.apply(spk2d, self.spk_proj.weight, self, up(pre["rows"]), up(pre["inst"]), up(pre["same"]), S, N,

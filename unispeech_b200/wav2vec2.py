@@ -20,12 +20,11 @@ from typing import Dict, List, Optional
 import torch
 import torch.nn as nn
 
-from . import _lib as L
 from . import dropout as DR
+from . import heads as H
 from . import ops
 from .engine import BF
-from .pretrain import _rows
-from .unispeech_sat import GumbelVectorQuantizer, sample_instances
+from .heads import GumbelVectorQuantizer, _rows, sample_instances
 from .wavlm import WavLM, WavLMConfig, _on_forward_stream
 
 _SITE_GUMBEL_W2V = 0x7F000003  # noise site of this model's quantizer
@@ -62,57 +61,27 @@ class _W2vNceFn(torch.autograd.Function):
     def forward(ctx, x2d, f2d, anchor, model, rows_idx, neg_idx, S, N, gum_key, stats_out):
         ctx.fwd_stream = torch.cuda.current_stream()
         dev = x2d.device
-        D, C, Dp = x2d.shape[1], f2d.shape[1], model.final_dim
+        Dp = model.final_dim
         fp, qz, pq = model.final_proj, model.quantizer, model.project_q
-        xs, ys = _rows(S, D, BF, dev), _rows(S, C, BF, dev)
-        ops.gather_rows(x2d, D, rows_idx, S, D, xs, D)
-        ops.gather_rows(f2d, C, rows_idx, S, C, ys, C)
-        wfp, wfpT = torch.empty(Dp, D, dtype=BF, device=dev), torch.empty(D, Dp, dtype=BF, device=dev)
-        ops.prep_linear(fp.weight, Dp, D, 1.0, wfp, D, wfpT, Dp)
-        proj = _rows(S, Dp, BF, dev)
-        ops.gemm_rows(xs, 0, D, S, 1, D, wfp, Dp, proj, 0, Dp, L.make_epilogue(bias=fp.bias))
-        st = dict(xs=xs, ys=ys, proj=proj, wfpT=wfpT, quant=None)
-        Kq = pq.weight.shape[1]
-        wpq, wpqT = torch.empty(Dp, Kq, dtype=BF, device=dev), torch.empty(Kq, Dp, dtype=BF, device=dev)
-        ops.prep_linear(pq.weight, Dp, Kq, 1.0, wpq, Kq, wpqT, Dp)
-        st["wpqT"] = wpqT
-        y = _rows(S, Dp, BF, dev)
+        xs, ys = H.gather(x2d, rows_idx), H.gather(f2d, rows_idx)
+        wfp, wfpT = H.linear_operands(fp.weight)
+        proj = H.linear_rows(xs, wfp, fp.bias)
+        wpq, wpqT = H.linear_operands(pq.weight)
+        yin, qs = ys, None                        # project_q's input: the features, or their quantized codes
         if qz is not None:
-            G, V = qz.groups, qz.num_vars
-            dv = qz.vars.shape[-1]
-            GV, vq_dim = G * V, G * dv
-            wq, wqT = torch.empty(GV, C, dtype=BF, device=dev), torch.empty(C, GV, dtype=BF, device=dev)
-            ops.prep_linear(qz.weight_proj.weight, GV, C, 1.0, wq, C, wqT, GV)
-            logits = _rows(S, GV, BF, dev)
-            ops.gemm_rows(ys, 0, C, S, 1, C, wq, GV, logits, 0, GV, L.make_epilogue(bias=qz.weight_proj.bias))
-            codes = torch.empty(S * G, dtype=torch.int32, device=dev)
-            q = _rows(S, vq_dim, BF, dev)
-            counts = torch.zeros(GV, dtype=torch.float32, device=dev)
-            probs = torch.zeros(GV, dtype=torch.float32, device=dev)
-            training = model.training
-            ops.vq_hard(logits, GV, qz.vars, S, G, V, dv, codes, q, vq_dim, counts, probs, gumbel=training, key=gum_key)
-            ops.gemm_rows(q, 0, vq_dim, S, 1, vq_dim, wpq, Dp, y, 0, Dp, L.make_epilogue(bias=pq.bias))
-            hard_probs = (counts / S).view(G, V)
-            avg_probs = (probs / S).view(G, V).detach().requires_grad_(False)
-            stats_out["code_perplexity"] = torch.exp(-torch.sum(hard_probs * torch.log(hard_probs + 1e-7), dim=-1)).sum()
-            stats_out["num_vars"] = V * G
-            stats_out["temp"] = qz.curr_temp
-            stats_out["codes"] = codes.view(S, G)   # selected code per (frame, group): `targets` of the reference's produce_targets
-            st["quant"] = dict(G=G, V=V, dv=dv, logits=logits, codes=codes, q=q, wqT=wqT, avg_probs=avg_probs, training=training,
-                               tau=float(qz.curr_temp))
-        else:
-            ops.gemm_rows(ys, 0, C, S, 1, C, wpq, Dp, y, 0, Dp, L.make_epilogue(bias=pq.bias))
+            yin, qs = qz.forward_rows(ys, gum_key, stats_out)
+            stats_out["codes"] = qs["codes"].view(S, qz.groups)   # `targets` of the reference's produce_targets
+        y = H.linear_rows(yin, wpq, pq.bias)
         g = torch.empty(S, N + 1, dtype=torch.float32, device=dev)
         loss64 = torch.zeros(1, dtype=torch.float64, device=dev)
         stats = torch.zeros(2, dtype=torch.int32, device=dev)
         ops.w2v_nce_fwd(proj, Dp, y, Dp, neg_idx, S, N, Dp, model.logit_temp, g, loss64, stats)
         stats_out["correct"], stats_out["count"] = stats[0], stats[1]
-        st.update(y=y, g=g)
-        ctx.model, ctx.st, ctx.sel, ctx.dims, ctx.key = model, st, (rows_idx, neg_idx), (x2d.shape[0], D, C, S, N, Dp), gum_key
+        ctx.model, ctx.sel, ctx.rows = model, (rows_idx, neg_idx), x2d.shape[0]
+        ctx.st = dict(xs=xs, proj=proj, wfpT=wfpT, yin=yin, wpqT=wpqT, y=y, g=g, quant=qs)
         outs = [loss64.float().reshape(())]
         if qz is not None:
-            ap = st["quant"]["avg_probs"]
-            outs.append(torch.exp(-torch.sum(ap * torch.log(ap + 1e-7), dim=-1)).sum())  # prob_perplexity (differentiable below)
+            outs.append(H.perplexity(qs["avg_probs"]).sum())  # prob_perplexity (differentiable below)
         return tuple(outs)
 
     @staticmethod
@@ -120,11 +89,12 @@ class _W2vNceFn(torch.autograd.Function):
     def backward(ctx, dloss, dppl=None):
         model, st = ctx.model, ctx.st
         rows_idx, neg_idx = ctx.sel
-        rows, D, C, S, N, Dp = ctx.dims
+        S, Dp = st["proj"].shape
+        N = st["g"].shape[1] - 1
         dev = st["xs"].device
         g_ = model._engine.g
         qs = st["quant"]
-        fp, qz, pq = model.final_proj, model.quantizer, model.project_q
+        fp, pq = model.final_proj, model.project_q
         up = (dloss if dloss is not None else torch.zeros((), device=dev)).float().reshape(1).contiguous()
         dacc_p = torch.zeros(S, Dp, dtype=torch.float32, device=dev)
         dacc_y = torch.zeros(S, Dp, dtype=torch.float32, device=dev)
@@ -132,52 +102,14 @@ class _W2vNceFn(torch.autograd.Function):
         # ---- x branch: final_proj
         dproj = _rows(S, Dp, BF, dev)
         ops.f32_to_bf16_rows(dacc_p, Dp, dproj, Dp, S, Dp)
-        ops.colsum(dproj, 0, Dp, S, 1, Dp, g_(fp.bias))
-        ops.gemm_wgrad(dproj, 0, Dp, st["xs"], 0, D, S, 1, Dp, D, g_(fp.weight), D)
-        dxs = _rows(S, D, BF, dev)
-        ops.gemm_rows(dproj, 0, Dp, S, 1, Dp, st["wfpT"], D, dxs, 0, D, None)
-        dx = torch.zeros(rows, D, dtype=BF, device=dev)
-        ops.scatter_add_rows(dxs, D, rows_idx, S, D, dx, D)
+        dx = H.scatter(H.linear_rows_backward(dproj, st["xs"], st["wfpT"], g_(fp.weight), g_(fp.bias)), rows_idx, ctx.rows)
         # ---- y branch: project_q (+ quantizer)
         dy = _rows(S, Dp, BF, dev)
         ops.f32_to_bf16_rows(dacc_y, Dp, dy, Dp, S, Dp)
-        ops.colsum(dy, 0, Dp, S, 1, Dp, g_(pq.bias))
-        dys = None
-        if qs is None:
-            ops.gemm_wgrad(dy, 0, Dp, st["ys"], 0, C, S, 1, Dp, C, g_(pq.weight), C)
-            dys = _rows(S, C, BF, dev)
-            ops.gemm_rows(dy, 0, Dp, S, 1, Dp, st["wpqT"], C, dys, 0, C, None)
-        else:
-            G, V, dv = qs["G"], qs["V"], qs["dv"]
-            GV, vq_dim = G * V, G * dv
-            ops.gemm_wgrad(dy, 0, Dp, qs["q"], 0, vq_dim, S, 1, Dp, vq_dim, g_(pq.weight), vq_dim)
-            dq = _rows(S, vq_dim, BF, dev)
-            ops.gemm_rows(dy, 0, Dp, S, 1, Dp, st["wpqT"], vq_dim, dq, 0, vq_dim, None)
-            ops.vq_dvars(dq, vq_dim, qs["codes"], S, G, V, dv, g_(qz.vars).view(GV, dv))
-            c = None
-            if dppl is not None:   # diversity term through avg_probs
-                ap = qs["avg_probs"]
-                ppl_g = torch.exp(-torch.sum(ap * torch.log(ap + 1e-7), dim=-1, keepdim=True))
-                c = (dppl.float() * ppl_g * (-torch.log(ap + 1e-7) - ap / (ap + 1e-7))).reshape(-1).contiguous()
-            h = None
-            if qs["training"]:     # straight-through estimator of F.gumbel_softmax(hard=True)
-                vb, vbT = torch.empty(GV, dv, dtype=BF, device=dev), torch.empty(dv, GV, dtype=BF, device=dev)
-                ops.prep_linear(qz.vars.view(GV, dv), GV, dv, 1.0, vb, dv, vbT, GV)
-                h = _rows(S, GV, BF, dev)
-                for grp in range(G):
-                    ops.gemm_rows(dq.view(-1)[grp * dv:], 0, vq_dim, S, 1, dv, vb[grp * V:(grp + 1) * V], V, h.view(-1)[grp * V:], 0,
-                                  GV, None)
-            if c is not None or h is not None:
-                dlogits = _rows(S, GV, BF, dev)
-                ops.vq_logits_bwd(qs["logits"], GV, S, G, V, c, h, GV, qs["tau"], ctx.key, dlogits, GV)
-                ops.colsum(dlogits, 0, GV, S, 1, GV, g_(qz.weight_proj.bias))
-                ops.gemm_wgrad(dlogits, 0, GV, st["ys"], 0, C, S, 1, GV, C, g_(qz.weight_proj.weight), C)
-                dys = _rows(S, C, BF, dev)
-                ops.gemm_rows(dlogits, 0, GV, S, 1, GV, qs["wqT"], C, dys, 0, C, None)
-        df = None
-        if dys is not None:
-            df = torch.zeros(rows, C, dtype=BF, device=dev)
-            ops.scatter_add_rows(dys, C, rows_idx, S, C, df, C)
+        dys = H.linear_rows_backward(dy, st["yin"], st["wpqT"], g_(pq.weight), g_(pq.bias))
+        if qs is not None:
+            dys = model.quantizer.backward_rows(qs, dys, dppl, g_)
+        df = None if dys is None else H.scatter(dys, rows_idx, ctx.rows)
         ctx.st = None
         return dx, df, None, None, None, None, None, None, None, None
 
@@ -253,7 +185,7 @@ class Wav2Vec2Model(WavLM):
         assert mi is not None, "the contrastive loss needs mask=True"
         B, T, D = x.shape
         dev = x.device
-        mi_h = (mi.cpu() if mi.device.type != "cpu" else mi).bool()
+        mi_h = mi.cpu().bool()
         counts = mi_h.sum(1)
         num = int(counts[0])
         if not bool((counts == num).all()):
@@ -265,9 +197,7 @@ class Wav2Vec2Model(WavLM):
         negs = sample_instances(B, num, self.n_negatives, self.cross_sample_negatives)      # [B, N * num], wav2vec2.py:488-523
         neg_ns = negs.to(torch.int32).view(B, num, N).permute(2, 0, 1).reshape(N, S)          # frame-major list -> [N, S] (:525-531)
         up = lambda t: t.contiguous().pin_memory().to(dev, non_blocking=True)
-        x2d = x.reshape(B * T, D)
-        if x2d.dtype != BF or not x2d.is_contiguous():
-            x2d = x2d.to(BF).contiguous()
+        x2d = H.bf16(x.reshape(B * T, D))
         f2d = unm.reshape(B * T, unm.shape[-1])
         seed = self.noise_seed if self.noise_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
         stats: Dict = {}
@@ -285,16 +215,9 @@ class Wav2Vec2Model(WavLM):
         loss, ssz = net_output["loss_nce"], net_output["sample_size"]
         log = {"loss_0": loss.detach()}
         if loss_weights is not None:
-            extra = self.get_extra_losses(net_output)
-            lw = list(loss_weights)
-            if len(lw) == 1 and len(extra) != 1:
-                lw = [lw[0]] * len(extra)
-            assert len(extra) == len(lw), f"{len(extra)}, {len(lw)}"
-            for i, (p, coef) in enumerate(zip(extra, lw)):
-                if coef != 0 and p is not None:
-                    p = coef * p.float() * ssz
-                    loss = loss + p
-                    log[f"loss_{i + 1}"] = p.detach()
+            for i, p in H.weighted_extra_losses(self.get_extra_losses(net_output), loss_weights, ssz):
+                loss = loss + p
+                log[f"loss_{i + 1}"] = p.detach()
         log.update(loss=loss.detach(), ntokens=ssz, sample_size=ssz, correct=net_output["correct"], count=net_output["count"])
         for k in ("prob_perplexity", "code_perplexity", "temp"):
             if k in net_output:
