@@ -6,7 +6,7 @@
 // The [B*H,T,T] bias of the reference is never materialised: it is Toeplitz, so a (query tile, key tile) pair reads only 255
 // consecutive entries of the per-head table.  Each kernel stages that window per tile in shared memory (the forward one key tile
 // ahead, the backward 128 new entries per query tile) and adds gate_i * tab[j-i] inside the softmax loop, so shared memory is
-// constant in T: 160,032 bytes for the forward, 176,128 for the backward.
+// constant in T: 88,352 bytes for the forward, 176,128 for the backward.
 // Layout: q/k/v are column slices of the fused projection output qkv[B, T, 3D] (head h of q at columns h*64.., k at
 // D + h*64.., v at 2D + h*64..), read by TMA with a strided 3-D tensor map; no head-major reshuffle exists.
 #pragma once

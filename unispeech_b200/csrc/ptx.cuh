@@ -63,6 +63,23 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// arrive on hardware barrier `id` without waiting (the barrier completes once `count` threads have arrived or synced)
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+// barrier over `count` threads on hardware barrier `id` that also returns whether `pred` holds for any of them
+__device__ __forceinline__ bool named_bar_any(int id, int count, bool pred) {
+  uint32_t any;
+  asm volatile(
+      "{\n\t.reg .pred p, q;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "bar.red.or.pred q, %2, %3, p;\n\t"
+      "selp.u32 %0, 1, 0, q;\n\t}"
+      : "=r"(any)
+      : "r"(static_cast<uint32_t>(pred)), "r"(id), "r"(count)
+      : "memory");
+  return any != 0;
+}
 
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
