@@ -88,42 +88,45 @@ int b200s_gemm_wgrad_ragged(const void* y, long long y_bs, long long y_rs, const
 
 /* Grouped positional convolution as an implicit GEMM (TransformerEncoder.pos_conv, WavLM/WavLM.py:514-527,577-579;
  * SamePad WavLM/modules.py:72-83), also used for its input gradient with flipped/transposed taps:
- *   out[b,t,g*Cg+n] = epilogue( sum_{j<taps} sum_{c<Cg} xpad[b, t+j, g*Cg+c] * wp[g*64+n, j*64+c] )
+ *   out[b,t,g*Cg+n] = epilogue( sum_{j<taps} sum_{c<Cg} xpad[b, t+j, g*Cg+c] * wp[g*Cgp+n, j*Cgp+c] )
  * xpad: [B, Tpad, D] bf16 (row stride D) with zero rows around the T valid frames, pointer offset so that tap j of
- * output frame t reads row t+j;  wp: [G*64, taps*64] bf16 zero padded (b200s_posconv_prep). Cg = D/G <= 64. */
+ * output frame t reads row t+j;  wp: [G*Cgp, taps*Cgp] bf16 zero padded (b200s_posconv_prep).  Cg = D/G <= 128, a multiple
+ * of 8; Cgp = 64 if Cg <= 64, else 128 (then taps <= 129). */
 int b200s_posconv_gemm(const void* xpad, long long xpad_bs, int T, int B, int D, int G, int taps,
                        const void* wp, void* out, long long out_bs, long long out_ld,
                        const b200s_epilogue* epi, b200s_stream stream);
 
-/* dwp[g, n, j, c] (+=) sum_{b,t} dy[b,t,g*Cg+n] * xpad[b,t+j,g*Cg+c];  dwp fp32 [G, Cg, taps, 64], only c < Cg is
+/* dwp[g, n, j, c] (+=) sum_{b,t} dy[b,t,g*Cg+n] * xpad[b,t+j,g*Cg+c];  dwp fp32 [G, Cg, taps, Cgp], only c < Cg is
  * meaningful. */
 int b200s_posconv_wgrad(const void* dy, long long dy_bs, long long dy_rs, const void* xpad, long long xpad_bs,
                         int T, int B, int D, int G, int taps, float* dwp, b200s_stream stream);
 
 /* ============================ attention (csrc/attn_fwd.cu, attn_bwd2.cu) =========================== */
 
-/* out[b,t,h*64+d] = sum_j softmax_j(scale q_i.k_j + gate[b,h,i]*tab[h,j-i+T-1], -inf at padded keys) v_j
+/* out[b,t,h*HD+d] = sum_j softmax_j(scale q_i.k_j + gate[b,h,i]*tab[h,j-i+T-1], -inf at padded keys) v_j
  * Replaces compute_bias + gate multiply + F.multi_head_attention_forward (WavLM/modules.py:417-455,504-563); the
  * [B*H,T,T] bias is never materialised (it is Toeplitz).  qkv: bf16 [B,T,3D] fused projection output; gate: fp32
  * [B,H,T] or NULL (=1); tab: fp32 [H,2T-1] or NULL (no bias); key_pad: uint8 [B,T] or NULL; out: bf16 [B,T,D];
- * lse: fp32 [B,H,T] log2-domain log-sum-exp (saved for backward).  head_dim = 64; any T >= 1 with B*H*T < 2^32 (the
- * kernel stages the bias window and key mask per key tile: its shared memory does not depend on T). */
+ * lse: fp32 [B,H,T] log2-domain log-sum-exp (saved for backward).  head_dim HD = 64, or 80 with tab = NULL (D = H * HD;
+ * any other value is an error); any T >= 1 with B*H*T < 2^32 (the kernel stages the bias window and key mask per key tile:
+ * its shared memory does not depend on T).  The same head_dim argument ends every attention entry point below. */
 int b200s_attn_fwd(const void* qkv, const float* gate, const float* tab, const uint8_t* key_pad, void* out,
-                   float* lse, int B, int T, int H, float scale, b200s_stream stream);
+                   float* lse, int B, int T, int H, float scale, int head_dim, b200s_stream stream);
 
 /* Backward of b200s_attn_fwd (autograd of the same lines).  delta: fp32 [B,H,T] workspace; dqkv: bf16 [B,T,3D];
  * dgate: fp32 [B,H,T] (written); dtab: fp32 [H,2T-1] (+=, shared by all layers: WavLM/WavLM.py:549,594-599).  Any T >= 1;
  * runs the fused kernel below with an fp32 dQ buffer allocated on the stream for the call. */
 int b200s_attn_bwd(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                    const uint8_t* key_pad, const float* lse, float* delta, void* dqkv, float* dgate, float* dtab,
-                   int B, int T, int H, float scale, b200s_stream stream);
+                   int B, int T, int H, float scale, int head_dim, b200s_stream stream);
 
 /* Same contract as b200s_attn_bwd, computed by ONE fused tensor-core kernel (csrc/attn_bwd2.cu: probabilities recomputed
  * once, dK/dV accumulated in registers, dQ reduced across key tiles in fp32).  dq_acc: fp32 [B,T,D] workspace that must be ZERO
  * on entry and is zero again on return.  Any T >= 1 (constant shared memory). */
 int b200s_attn_bwd_fused(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                          const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv,
-                         float* dgate, float* dtab, int B, int T, int H, float scale, b200s_stream stream);
+                         float* dgate, float* dtab, int B, int T, int H, float scale, int head_dim,
+                         b200s_stream stream);
 
 /* Attention with dropout on the probabilities (attention_dropout; the dropout_p argument of
  * F.multi_head_attention_forward, WavLM/modules.py:551): O = (softmax(..) o M) V / (1 - p).  M comes from the counter-based
@@ -133,11 +136,11 @@ int b200s_attn_bwd_fused(const void* qkv, const void* out, const void* dout, con
  * counter of the hash); the mask takes B*H*T^2/8 bytes (134 MB per layer for one utterance of T = 8192 with 16 heads). */
 int b200s_attn_fwd_dropout(const void* qkv, const float* gate, const float* tab, const uint8_t* key_pad, void* out,
                            float* lse, int B, int T, int H, float scale, float drop_p, uint32_t key0, uint32_t key1,
-                           uint32_t* drop_mask, b200s_stream stream);
+                           uint32_t* drop_mask, int head_dim, b200s_stream stream);
 int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* dout, const float* gate,
                                  const float* tab, const uint8_t* key_pad, const float* lse, float* delta,
                                  float* dq_acc, void* dqkv, float* dgate, float* dtab, int B, int T, int H, float scale,
-                                 float drop_p, const uint32_t* drop_mask, b200s_stream stream);
+                                 float drop_p, const uint32_t* drop_mask, int head_dim, b200s_stream stream);
 long long b200s_attn_dropout_mask_words(int B, int T, int H);
 
 /* Deprecated, kept for callers of the earlier ABI: validates 0 <= sms < SM count and has no effect.  It reserved SMs of the persistent
@@ -286,7 +289,8 @@ int b200s_prep_linear_batched(const void* descs, int n_descs, int total_tiles, b
 int b200s_prep_conv_fwd(const float* src, int Co, int Ci, int k, void* dst, b200s_stream stream);
 int b200s_prep_conv_dgrad(const float* src, int Co, int Ci, int k, int s, int rho, void* dst, b200s_stream stream);
 int b200s_unprep_conv_wgrad(const float* dwk, int Co, int Ci, int k, float* dw, b200s_stream stream);
-/* weight_norm(dim=2) of pos_conv (WavLM/WavLM.py:526) -> padded per-group operands; and its backward.  Workspaces (8-byte aligned,
+/* weight_norm(dim=2) of pos_conv (WavLM/WavLM.py:526) -> padded per-group operands wp_fwd / wp_dgrad bf16 [G, Cgp, taps, Cgp]
+ * (Cgp as for b200s_posconv_gemm); and its backward from dwp [G, Cg, taps, Cgp].  Workspaces (8-byte aligned,
  * zeroed inside): norm2 = 2 * taps floats, work = 4 * taps floats -- the per-tap sums are accumulated in fp64 so that the norm, and
  * with it every bf16 pos_conv weight, is the same value on every run (the forward pass is bit-reproducible). */
 int b200s_posconv_prep(const float* weight_v, const float* weight_g, int D, int G, int taps, float* norm2,

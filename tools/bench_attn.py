@@ -1,5 +1,7 @@
 """Micro-benchmark of the attention kernels at the WavLM-Base (16 x 749, 12 heads) and -Large (8 x 999, 16 heads) shapes.
-    python tools/bench_attn.py [--reps 10] [--only base|large|long] [--dropout 0.1]
+    python tools/bench_attn.py [--reps 10] [--only base|large|long|wide] [--dropout 0.1]
+`--only wide` times the forward, the forward with dropout (--dropout, else 0.1) and the fused backward without the bias at
+8 x 999 with 16 heads at head width 80 (the 1280-wide encoders) next to head width 64 at the same shape; it runs only when asked.
 `--only long` times one utterance with 16 heads at T = 8192 (164 s: the forward and both backward entry points) and
 T = 16384 (the forward), and checks every call once against the fp32 reference one head at a time (one [T, T] fp32
 matrix is 1 GB at T = 16384).
@@ -207,5 +209,45 @@ for name, B, T, H in (("base", 16, 749, 12), ("large", 8, 999, 16)):
             all_ok &= check_bwd(k, fn, qkv, gate if bias else None, tab if bias else None, dout, dqkv, dgate, dtab if bias else None,
                                 B, T, H, keep, args.dropout)
             del keep
+# 1280-wide encoders (XLS-R 1B, MMS-1B, HuBERT X-Large): head width 80, no relative-position bias, beside head width 64 at the same
+# B, T, H.  Algorithmic FLOPs scale with the head width.
+if args.only == "wide":
+    B, T, H = 8, 999, 16
+    p_w = args.dropout if args.dropout > 0 else 0.1
+    for hd in (64, 80):
+        D = H * hd
+        torch.manual_seed(0)
+        qkv = torch.randn(B, T, 3 * D, device=dev).to(torch.bfloat16)
+        out = torch.empty(B, T, D, device=dev, dtype=torch.bfloat16)
+        lse = torch.empty(B, H, T, device=dev)
+        dout = torch.randn(B, T, D, device=dev).to(torch.bfloat16)
+        delta = torch.empty(B, H, T, device=dev)
+        dqkv = torch.zeros(B, T, 3 * D, device=dev, dtype=torch.bfloat16)
+        dq_acc = torch.zeros(B, T, D, device=dev)
+        words = torch.empty(ops.attn_dropout_mask_words(B, T, H), dtype=torch.int32, device=dev)
+        sc = hd ** -0.5
+        fns = {
+            "fwd": lambda: ops.attn_fwd(qkv, None, None, None, out, lse, B, T, H, sc, head_dim=hd),
+            "fwd_dropout": lambda: ops.attn_fwd_dropout(qkv, None, None, None, out, lse, B, T, H, sc, p_w, (123, 456), words,
+                                                        head_dim=hd),
+            "bwd_fused": lambda: ops.attn_bwd_fused(qkv, out, dout, None, None, None, lse, delta, dq_acc, dqkv, None, None, B, T,
+                                                    H, sc, head_dim=hd),
+        }
+        fl = 4.0 * B * H * T * T * hd
+        for k, fn in fns.items():
+            for _ in range(2):
+                fn()
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(args.reps):
+                fn()
+            e1.record()
+            torch.cuda.synchronize()
+            ms = e0.elapsed_time(e1) / args.reps
+            tf = fl * (1.0 if k.startswith("fwd") else 2.5) / ms / 1e9
+            print(f"wide   hd={hd} {k:13s} {ms*1e3:9.1f} us   {tf:8.1f} TFLOP/s (algorithmic)  {tf / peak:6.3f} of peak", flush=True)
+        del qkv, out, lse, dout, delta, dqkv, dq_acc, words, fns
+        torch.cuda.empty_cache()
 if not all_ok:
     sys.exit(1)

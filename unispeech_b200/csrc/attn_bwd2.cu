@@ -45,6 +45,11 @@
 // Dropout: the keep bit of (query i, key j) is bit i & 31 of word drop_mask[block(i), j], written by the forward kernel.
 // Padding: a CTA whose 128 keys are all padded writes zero dK / dV rows and exits; query tiles that are fully padded at the end
 // of the utterance are not visited (their probabilities are zero: the forward leaves lse = +inf there).
+// Head width 80 (no bias; tiles and MMAs as in attn_common.cuh): dK / dV take 80 accumulator registers instead of 64, which
+// the 128-query tiling above cannot afford, so the query tile is 64 rows: S^T / dP^T are m64n64 (32 registers each), the dS^T
+// tile is one [128 keys][64 queries] block, and dQ = dS K is split over the keys instead of the queries: each warpgroup
+// reduces its 64 keys' share of the tile's 64 x 80 dQ (TMA reductions of 32 + 32 + 16 columns).  The dropout mask words are
+// the same (a tile covers two 32-query blocks instead of four).
 #include "../../include/unispeech_b200.h"
 #include "attn_common.cuh"
 #include "common.h"
@@ -61,30 +66,45 @@ __device__ __forceinline__ float ex2f(float x) {
   return y;
 }
 
-// shared-memory map (bytes from the 1024-aligned base)
-constexpr int kFK = 0;             // K tile          16 KB
-constexpr int kFV = 16384;         // V tile          16 KB
-constexpr int kFQ = 32768;         // Q tiles, 2 stages x 16 KB
-constexpr int kFDO = 65536;        // dO tiles, 2 stages x 16 KB
-constexpr int kFDS = 98304;        // dS^T: [2 query blocks][128 keys][64 queries] bf16, 32 KB
-constexpr int kFW = 131072;        // gate*dS staging for the diagonal sums: [128 keys][kWStride] bf16 (33280 B) ...
-constexpr int kWStride = 130;      // bf16 per staged row (65 words: conflict-free diagonal reads)
-constexpr int kFDQ1 = 17408;       // ... aliased by the dQ staging of WG 0 at kFW and of WG 1 at kFW + kFDQ1 (16 KB each:
-                                   // two [64 queries][32] fp32 SWIZZLE_128B boxes), inside each WG's own staged rows
-constexpr int kFWBytes = kFDQ1 + 16384;          // 33792
-constexpr int kFScal = kFW + kFWBytes;           // 164864: per stage lse, Delta*scale, gate*log2e, gate/scale [4][128] fp32
-constexpr int kFDg = kFScal + 2 * 4 * 512;       // 168960: d gate partial column sums [8 warps][128] fp32
-constexpr int kFSmem = kFDg + 8 * 512 + 1024;    // 174080 bytes with the alignment slack, for every T (+ 2 KB static: bias
-                                                 // window and d tab blocks)
-constexpr int kFThreads = 256;                   // two warpgroups
+constexpr int kWStride = 130;      // bf16 per staged row of the gate*dS tile (65 words: conflict-free diagonal reads)
+constexpr int kFThreads = 256;     // two warpgroups
+
+// shared-memory map of head width HD (bytes from the 1024-aligned base); at HD = 64:
+//   K 0, V 16384 (16 KB tiles); Q 32768, dO 65536 (2 stages x 16 KB); dS^T 98304 ([2 query blocks][128 keys][64 queries] bf16,
+//   32 KB); at 131072 the gate*dS staging for the diagonal sums ([128 keys][kWStride] bf16, 33280 B), aliased by the dQ
+//   staging of WG 0 at kFW and of WG 1 at kFW + kFDQ1 (16 KB each: two [64 queries][32] fp32 SWIZZLE_128B boxes, inside each
+//   WG's own staged rows); per stage lse, Delta*scale, gate*log2e, gate/scale [4][128] fp32 at 164864; d gate partial column
+//   sums [8 warps][128] fp32 at 168960; 174080 bytes with the alignment slack (+ 2 KB static: bias window and d tab blocks).
+// At HD = 80: 20 KB K / V tiles, 10 KB Q / dO stages (64 queries), one 16 KB dS^T block, and 20 KB of dQ staging per WG
+// (two [64][32] SWIZZLE_128B boxes and one [64][16] fp32 box): 148480 bytes.  Both are the same for every T.
+template <int HD>
+struct BwdMap {
+  static constexpr int kQT = HD == 64 ? kAttnTile : 64;  // queries per tile
+  static constexpr int kKV = kAttnTile * HD * 2;           // one K or V tile
+  static constexpr int kQS = kQT * HD * 2;                 // one Q or dO stage
+  static constexpr int kFK = 0, kFV = kKV, kFQ = 2 * kKV, kFDO = kFQ + 2 * kQS, kFDS = kFDO + 2 * kQS;
+  static constexpr int kFW = kFDS + kAttnTile * kQT * 2;
+  static constexpr int kFDQ1 = HD == 64 ? 17408 : 64 * HD * 4;
+  static constexpr int kFWBytes = kFDQ1 + (HD == 64 ? 16384 : 64 * HD * 4);
+  static constexpr int kFScal = kFW + kFWBytes;
+  static constexpr int kFDg = kFScal + 2 * 4 * 512;
+  static constexpr int kFSmem = kFDg + 8 * 512 + 1024;
+};
+static_assert(BwdMap<64>::kFDS == 98304 && BwdMap<64>::kFScal == 164864 && BwdMap<64>::kFSmem == 174080, "HD 64 map");
 
 }  // namespace
 
-template <bool HAS_BIAS, bool DROP>
+template <int HD, bool HAS_BIAS, bool DROP>
 __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tm_qkv,
                                                                       const __grid_constant__ CUtensorMap tm_do,
                                                                       const __grid_constant__ CUtensorMap tm_dq,
+                                                                      const __grid_constant__ CUtensorMap tm_qkv16,
+                                                                      const __grid_constant__ CUtensorMap tm_do16,
+                                                                      const __grid_constant__ CUtensorMap tm_dq16,
                                                                       const __grid_constant__ AttnParams p) {
+  static_assert(HD == 64 || (HD == 80 && !HAS_BIAS), "head width 64, or 80 without the relative-position bias");
+  using M = BwdMap<HD>;
+  constexpr int QT = M::kQT, kFDS = M::kFDS, kFW = M::kFW, kFDQ1 = M::kFDQ1;
   pdl_grid_sync();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int k0 = blockIdx.x * kAttnTile, h = blockIdx.y, b = blockIdx.z;
@@ -93,13 +113,13 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, still a __shared__ pointer (LDS/STS, not generic)
-  uint8_t* sK = smem + kFK;
-  uint8_t* sV = smem + kFV;
-  uint8_t* sQ = smem + kFQ;
-  uint8_t* sDO = smem + kFDO;
+  uint8_t* sK = smem + M::kFK;
+  uint8_t* sV = smem + M::kFV;
+  uint8_t* sQ = smem + M::kFQ;
+  uint8_t* sDO = smem + M::kFDO;
   uint8_t* sDS = smem + kFDS;
-  float* scal = reinterpret_cast<float*>(smem + kFScal);
-  float* dgp = reinterpret_cast<float*>(smem + kFDg);
+  float* scal = reinterpret_cast<float*>(smem + M::kFScal);
+  float* dgp = reinterpret_cast<float*>(smem + M::kFDg);
   // static, not in the dynamic map: addressed by immediates, which keeps the bias variants within their register budget
   __shared__ __align__(16) float win_s[2 * kAttnTile];    // bias window of the current query tile, by m
   __shared__ float dtab_acc[2 * kAttnTile];                // d tab blocks: lower (m < 128), upper
@@ -111,7 +131,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
   // utterance's pad bytes (every thread takes a few), one block-wide reduction: the prologue pays a single global-load latency.
   __shared__ int nq_s;
   if (tid == 0) nq_s = 1;
-  int NQ = N;  // query tiles to visit
+  int NQ = QT == kAttnTile ? N : (T + QT - 1) / QT;  // query tiles to visit
   {
     bool masked = false;
     if (tid < kAttnTile) {
@@ -129,9 +149,9 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     if (n_masked == kAttnTile) {
       // nothing attends to these keys: dK = dV = 0
       if (tid < kAttnTile && k0 + tid < T) {
-        __nv_bfloat16* dst = p.dqkv + (static_cast<long long>(b) * T + k0 + tid) * (3 * D) + D + h * kHeadDim;
+        __nv_bfloat16* dst = p.dqkv + (static_cast<long long>(b) * T + k0 + tid) * (3 * D) + D + h * HD;
 #pragma unroll
-        for (int g = 0; g < 8; ++g) {
+        for (int g = 0; g < HD / 8; ++g) {
           *reinterpret_cast<uint4*>(dst + g * 8) = make_uint4(0u, 0u, 0u, 0u);
           *reinterpret_cast<uint4*>(dst + D + g * 8) = make_uint4(0u, 0u, 0u, 0u);
         }
@@ -139,7 +159,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       return;
     }
     if (p.key_pad != nullptr) {
-      if (last_live >= 0) atomicMax(&nq_s, last_live / kAttnTile + 1);
+      if (last_live >= 0) atomicMax(&nq_s, last_live / QT + 1);
       __syncthreads();
       NQ = nq_s;
     }
@@ -151,16 +171,21 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     tma_prefetch_desc(&tm_qkv);
     tma_prefetch_desc(&tm_do);
     tma_prefetch_desc(&tm_dq);
+    if (HD == 80) {
+      tma_prefetch_desc(&tm_qkv16);
+      tma_prefetch_desc(&tm_do16);
+      tma_prefetch_desc(&tm_dq16);
+    }
     mbar_init(&kv_full, 1);
     for (int i = 0; i < 2; ++i) mbar_init(&qdo_full[i], 1);
     fence_mbar_init();
-    mbar_expect_tx(&kv_full, 32768);
-    tma_load_4d(sK, &tm_qkv, &kv_full, D + h * kHeadDim, k0, b, 0);
-    tma_load_4d(sV, &tm_qkv, &kv_full, 2 * D + h * kHeadDim, k0, b, 0);
+    mbar_expect_tx(&kv_full, 2 * M::kKV);
+    tma_load_head<HD, kAttnTile, QT>(sK, &tm_qkv, &tm_qkv16, &kv_full, D + h * HD, k0, b);
+    tma_load_head<HD, kAttnTile, QT>(sV, &tm_qkv, &tm_qkv16, &kv_full, 2 * D + h * HD, k0, b);
     for (int qi = 0; qi < 2 && qi < NQ; ++qi) {
-      mbar_expect_tx(&qdo_full[qi], 32768);
-      tma_load_4d(sQ + qi * 16384, &tm_qkv, &qdo_full[qi], h * kHeadDim, qi * kAttnTile, b, 0);
-      tma_load_4d(sDO + qi * 16384, &tm_do, &qdo_full[qi], h * kHeadDim, qi * kAttnTile, b, 0);
+      mbar_expect_tx(&qdo_full[qi], 2 * M::kQS);
+      tma_load_head<HD, QT, QT>(sQ + qi * M::kQS, &tm_qkv, &tm_qkv16, &qdo_full[qi], h * HD, qi * QT, b);
+      tma_load_head<HD, QT, QT>(sDO + qi * M::kQS, &tm_do, &tm_do16, &qdo_full[qi], h * HD, qi * QT, b);
     }
   }
 
@@ -175,7 +200,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
   // gate/scale of query tid & 127 (lse = +inf marks out-of-range queries: p = exp2(-inf) = 0)
   const float inv_scale = 1.0f / p.scale;
   auto load_terms = [&](int qi, float& t0, float& t1) {
-    const int i = qi * kAttnTile + (tid & 127);
+    const int i = qi * QT + (tid & 127);
     t0 = tid < kAttnTile ? INFINITY : 0.f;
     t1 = 0.f;
     if (i < T) {
@@ -216,6 +241,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     uint32_t* wtile = reinterpret_cast<uint32_t*>(smem + kFW);
 
     float dv_acc[32], dk_acc[32];  // written by the first tile's MMAs (scale_d = 0)
+    float dv16[8], dk16[8];        // their columns 64..79 (HD = 80 only)
 
     // diagonal sums of the staged gate*dS tile of query tile qi.  Task (e, s): elements (key (ii + e) & 127, query ii) for
     // ii = 16 s .. 16 s + 15: diagonal key - query = e (not wrapped, ii + e < 128) or e - 128 (wrapped).  The wrap point is a
@@ -242,27 +268,32 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     for (int qi = 0; qi < NQ; ++qi) {
       const int st = qi & 1;
       mbar_wait(&qdo_full[st], (qi >> 1) & 1);
-      const uint32_t bq = smem_u32(sQ + st * 16384), bdo = smem_u32(sDO + st * 16384);
-      float s_acc[64], d_acc[64];
+      const uint32_t bq = smem_u32(sQ + st * M::kQS), bdo = smem_u32(sDO + st * M::kQS);
+      float s_acc[QT / 2], d_acc[QT / 2];
+      // S^T = K_w Q^T and dP^T = V_w dO^T over the head width (at HD = 80 the fifth k16 step reads the 32-byte blocks)
+      auto scores = [&](float* acc, uint32_t a, uint32_t bt) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t da = make_smem_desc_sw128(a + k * 32, 16, 1024), db = make_smem_desc_sw128(bt + k * 32, 16, 1024);
+          if (QT == 128) wgmma_m64n128k16<0, 0>(acc, da, db, k > 0 ? 1u : 0u);
+          else wgmma_m64n64k16<0, 0>(acc, da, db, k > 0 ? 1u : 0u);
+        }
+        if (HD == 80)
+          wgmma_m64n64k16<0, 0>(acc, make_smem_desc_sw32(a - w * 8192 + kAttnTile * 128 + w * 2048),
+                                make_smem_desc_sw32(bt + QT * 128), 1u);
+        wgmma_commit();
+      };
       wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_m64n128k16<0, 0>(s_acc, make_smem_desc_sw128(ak + k * 32, 16, 1024), make_smem_desc_sw128(bq + k * 32, 16, 1024),
-                               k > 0 ? 1u : 0u);
-      wgmma_commit();
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_m64n128k16<0, 0>(d_acc, make_smem_desc_sw128(av + k * 32, 16, 1024), make_smem_desc_sw128(bdo + k * 32, 16, 1024),
-                               k > 0 ? 1u : 0u);
-      wgmma_commit();
-      // dropout keep words of this thread's two key rows for the tile's four 32-query blocks
-      uint32_t kw[2][4];
+      scores(s_acc, ak, bq);
+      scores(d_acc, av, bdo);
+      // dropout keep words of this thread's two key rows for the tile's 32-query blocks
+      uint32_t kw[2][QT / 32];
       if (DROP) {
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
-          for (int blk = 0; blk < 4; ++blk)
-            kw[rr][blk] = p.drop_mask[(bh * (4 * N) + qi * 4 + blk) * (N * kAttnTile) + k0 + kr + 8 * rr];
+          for (int blk = 0; blk < QT / 32; ++blk)
+            kw[rr][blk] = p.drop_mask[(bh * (4 * N) + qi * (QT / 32) + blk) * (N * kAttnTile) + k0 + kr + 8 * rr];
       }
       // the previous tile's dQ reduction has read this WG's staging buffer before the buffer is written again
       if (qi > 0) {
@@ -275,7 +306,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       // P^T on the S^T fragments while the dP^T chain runs (fp32, in place)
       wgmma_wait<1>();
 #pragma unroll
-      for (int g = 0; g < 16; ++g) {
+      for (int g = 0; g < QT / 8; ++g) {
         const float2 lse = *reinterpret_cast<const float2*>(ts + 8 * g + fc);
         float2 gl = make_float2(0.f, 0.f);
         if (HAS_BIAS) gl = *reinterpret_cast<const float2*>(ts + 2 * kAttnTile + 8 * g + fc);
@@ -294,9 +325,9 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
 
       // dS^T after dP^T lands; bf16 operands for dV / dK, the dS^T tile and the staging tile; d gate column partials
       wgmma_wait<0>();
-      uint32_t p16[32];
+      uint32_t p16[QT / 4];
 #pragma unroll
-      for (int hq = 0; hq < 2; ++hq) {   // query halves: 16 d gate partials live at a time
+      for (int hq = 0; hq < QT / 64; ++hq) {   // query halves: 16 d gate partials live at a time
       float dg[16];
 #pragma unroll
       for (int g = 8 * hq; g < 8 * hq + 8; ++g) {
@@ -357,8 +388,11 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       // ---- dV += P^T dO (this WG's 64 keys; A = P^T from registers)
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 8; ++k)  // K = 128 queries, 16 per step
+      for (int k = 0; k < QT / 16; ++k) {  // K = the tile's queries, 16 per step
         wgmma_m64n64k16_rs<1>(dv_acc, p16 + 4 * k, make_smem_desc_sw128(bdo + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+        if (HD == 80)
+          wgmma_m64n16k16_rs<1>(dv16, p16 + 4 * k, make_smem_desc_sw32(bdo + QT * 128 + k * 512), (qi > 0 || k > 0) ? 1u : 0u);
+      }
       wgmma_commit();
       fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
       named_bar_sync(1, kFThreads);
@@ -366,15 +400,24 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       // ---- dK += dS^T Q (this WG's 64 keys; A = its rows of the dS^T tile, K-major).  From shared memory rather than registers:
       // 32 more live registers through the dS^T pass would spill.
 #pragma unroll
-      for (int k = 0; k < 8; ++k)
-        wgmma_m64n64k16<0, 1>(dk_acc, make_smem_desc_sw128(smem_u32(sDS) + (k >> 2) * 16384 + w * 8192 + (k & 3) * 32, 16, 1024),
-                              make_smem_desc_sw128(bq + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
-      // ---- dQ = dS K (this WG's 64 queries; A = the dS^T tile read MN-major, K = 128 keys, 16 per step)
-      float dq[32];
+      for (int k = 0; k < QT / 16; ++k) {
+        const uint64_t da = make_smem_desc_sw128(smem_u32(sDS) + (k >> 2) * 16384 + w * 8192 + (k & 3) * 32, 16, 1024);
+        wgmma_m64n64k16<0, 1>(dk_acc, da, make_smem_desc_sw128(bq + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+        if (HD == 80) wgmma_m64n16k16<0, 1>(dk16, da, make_smem_desc_sw32(bq + QT * 128 + k * 512), (qi > 0 || k > 0) ? 1u : 0u);
+      }
+      // ---- dQ = dS K.  HD 64: this WG's 64 queries, K = 128 keys.  HD 80: the tile's 64 queries, K = this WG's 64 keys (the two
+      // WGs' shares are added by the reductions).  A = the dS^T tile read MN-major, 16 keys per step.
+      float dq[32], dq16[8];
+      constexpr int kDqSteps = QT == kAttnTile ? 8 : 4;
+      const uint32_t dq_a = smem_u32(sDS) + (QT == kAttnTile ? w * 16384 : w * 8192);
+      const uint32_t dq_b = smem_u32(sK) + (QT == kAttnTile ? 0 : w * 8192);
 #pragma unroll
-      for (int k = 0; k < 8; ++k)
-        wgmma_m64n64k16<1, 1>(dq, make_smem_desc_sw128(smem_u32(sDS) + w * 16384 + k * 2048, 16384, 1024),
-                              make_smem_desc_sw128(smem_u32(sK) + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+      for (int k = 0; k < kDqSteps; ++k) {
+        const uint64_t da = make_smem_desc_sw128(dq_a + k * 2048, 16384, 1024);
+        wgmma_m64n64k16<1, 1>(dq, da, make_smem_desc_sw128(dq_b + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+        if (HD == 80)
+          wgmma_m64n16k16<1, 1>(dq16, da, make_smem_desc_sw32(smem_u32(sK) + kAttnTile * 128 + w * 2048 + k * 512), k > 0 ? 1u : 0u);
+      }
       wgmma_commit();
       // the next tile's per-query terms: loaded while the MMAs run, stored once this tile's have been read (not earlier: live
       // across the exp2 pass they would push that pass over the register budget)
@@ -409,13 +452,13 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       }
       named_bar_sync(1, kFThreads);  // the Q / dO stage, the staging, dS^T and d gate tiles of this query tile are consumed
       if (tid == 0 && qi + 2 < NQ) {
-        mbar_expect_tx(&qdo_full[st], 32768);
-        tma_load_4d(sQ + st * 16384, &tm_qkv, &qdo_full[st], h * kHeadDim, (qi + 2) * kAttnTile, b, 0);
-        tma_load_4d(sDO + st * 16384, &tm_do, &qdo_full[st], h * kHeadDim, (qi + 2) * kAttnTile, b, 0);
+        mbar_expect_tx(&qdo_full[st], 2 * M::kQS);
+        tma_load_head<HD, QT, QT>(sQ + st * M::kQS, &tm_qkv, &tm_qkv16, &qdo_full[st], h * HD, (qi + 2) * QT, b);
+        tma_load_head<HD, QT, QT>(sDO + st * M::kQS, &tm_do, &tm_do16, &qdo_full[st], h * HD, (qi + 2) * QT, b);
       }
 
-      // dQ rows of this WG -> the staging boxes ([64 queries][32 fp32], SWIZZLE_128B; the staged dS already carries the
-      // softmax scale) -> TMA reductions into dq_acc[b, q, h*64 + col]
+      // dQ rows of this WG -> the staging boxes ([64 queries][32 fp32], SWIZZLE_128B, and at HD = 80 [64][16] fp32 behind
+      // them; the staged dS already carries the softmax scale) -> TMA reductions into dq_acc[b, q, h*HD + col]
       {
         const int r0 = 16 * wq + (lane >> 2);
 #pragma unroll
@@ -426,12 +469,22 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
             *reinterpret_cast<float2*>(dq_stage + (col >> 5) * 8192 + r * 128 + ((((col & 31) >> 2) ^ (r & 7)) << 4) + (col & 3) * 4) =
                 make_float2(dq[4 * g + 2 * rr], dq[4 * g + 2 * rr + 1]);
           }
+        if (HD == 80) {
+#pragma unroll
+          for (int g = 0; g < 2; ++g)
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr)
+              *reinterpret_cast<float2*>(dq_stage + 16384 + (r0 + 8 * rr) * 64 + (8 * g + fc) * 4) =
+                  make_float2(dq16[4 * g + 2 * rr], dq16[4 * g + 2 * rr + 1]);
+        }
       }
       fence_proxy_async_smem();
       named_bar_sync(2 + w, 128);
-      if (flusher && qi * kAttnTile + 64 * w < T) {
-        tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage), h * kHeadDim, qi * kAttnTile + 64 * w, b);
-        tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage) + 8192, h * kHeadDim + 32, qi * kAttnTile + 64 * w, b);
+      const int dq_row = QT == kAttnTile ? qi * kAttnTile + 64 * w : qi * QT;
+      if (flusher && dq_row < T) {
+        tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage), h * HD, dq_row, b);
+        tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage) + 8192, h * HD + 32, dq_row, b);
+        if (HD == 80) tma_reduce_add_3d(&tm_dq16, smem_u32(dq_stage) + 16384, h * HD + 64, dq_row, b);
         bulk_commit();
       }
       if (HAS_BIAS && tid >= kAttnTile) {
@@ -451,12 +504,19 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     for (int rr = 0; rr < 2; ++rr) {
       const int key = k0 + kr + 8 * rr;
       if (key < T) {
-        __nv_bfloat16* dst = p.dqkv + (static_cast<long long>(b) * T + key) * (3 * D) + h * kHeadDim + fc;
+        __nv_bfloat16* dst = p.dqkv + (static_cast<long long>(b) * T + key) * (3 * D) + h * HD + fc;
+        const float rp = DROP ? p.drop_rp : 1.0f;   // dV = (P o M)^T dO / (1-p)
 #pragma unroll
         for (int g = 0; g < 8; ++g) {
-          const float rp = DROP ? p.drop_rp : 1.0f;   // dV = (P o M)^T dO / (1-p)
           *reinterpret_cast<uint32_t*>(dst + 2 * D + 8 * g) = pack_bf16x2(dv_acc[4 * g + 2 * rr] * rp, dv_acc[4 * g + 2 * rr + 1] * rp);
           *reinterpret_cast<uint32_t*>(dst + D + 8 * g) = pack_bf16x2(dk_acc[4 * g + 2 * rr], dk_acc[4 * g + 2 * rr + 1]);
+        }
+        if (HD == 80) {
+#pragma unroll
+          for (int g = 0; g < 2; ++g) {
+            *reinterpret_cast<uint32_t*>(dst + 2 * D + 64 + 8 * g) = pack_bf16x2(dv16[4 * g + 2 * rr] * rp, dv16[4 * g + 2 * rr + 1] * rp);
+            *reinterpret_cast<uint32_t*>(dst + D + 64 + 8 * g) = pack_bf16x2(dk16[4 * g + 2 * rr], dk16[4 * g + 2 * rr + 1]);
+          }
         }
       }
     }
@@ -472,6 +532,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
 }
 
 // Delta_i = sum_d dO_id O_id (fp32 [B,H,T]); also clears d gate, which the fused kernel accumulates with atomics.
+template <int HD>
 __global__ void __launch_bounds__(256) attn_delta2_kernel(const __nv_bfloat16* __restrict__ o,
                                                           const __nv_bfloat16* __restrict__ dout, int B, int T, int H,
                                                           float* __restrict__ delta, float* __restrict__ dgate) {
@@ -479,12 +540,17 @@ __global__ void __launch_bounds__(256) attn_delta2_kernel(const __nv_bfloat16* _
   const int lane = threadIdx.x & 31;
   const long long row = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   if (row >= static_cast<long long>(B) * T) return;
-  const int D = H * kHeadDim;
+  const int D = H * HD;
   const long long b = row / T, t = row % T;
   for (int h = 0; h < H; ++h) {
-    const float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(o + row * D + h * kHeadDim + lane * 2));
-    const float2 g = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dout + row * D + h * kHeadDim + lane * 2));
-    const float s = warp_sum(a.x * g.x + a.y * g.y);
+    float part = 0.f;
+#pragma unroll
+    for (int c = 2 * lane; c < HD; c += 64) {  // column pairs: one per lane, and at HD 80 a second one for lanes 0..7
+      const float2 a = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(o + row * D + h * HD + c));
+      const float2 g = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(dout + row * D + h * HD + c));
+      part += a.x * g.x + a.y * g.y;
+    }
+    const float s = warp_sum(part);
     if (lane == 0) {
       delta[(b * H + h) * T + t] = s;
       if (dgate != nullptr) dgate[(b * H + h) * T + t] = 0.f;
@@ -513,26 +579,36 @@ __global__ void __launch_bounds__(256) attn_dq_convert_kernel(float* __restrict_
   }
 }
 
-int make_qkv_tmap(CUtensorMap* out, const void* qkv, int T, int B, int D3, int box_rows);
-int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_rows);
+int make_qkv_tmap(CUtensorMap* out, const void* qkv, int T, int B, int D3, int box_cols, int box_rows);
+int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_cols, int box_rows);
 
 
 // Delta pre-kernel, the fused kernel and the dQ conversion on one stream (see the entry points below for the contract).
 static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                            const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv, float* dgate,
                            float* dtab, int B, int T, int H, float scale, float drop_p, const uint32_t* drop_mask,
-                           cudaStream_t st) {
-  const int D = H * kHeadDim;
+                           int head_dim, cudaStream_t st) {
+  const int D = H * head_dim;
   const long long rows = static_cast<long long>(B) * T;
-  B200_CHECK_CUDA(launch_pdl(attn_delta2_kernel, dim3(static_cast<unsigned>(ceil_div_ll(rows * 32, 256))), dim3(256), 0, st,
+  B200_CHECK_CUDA(launch_pdl(head_dim == 80 ? attn_delta2_kernel<80> : attn_delta2_kernel<64>, dim3(static_cast<unsigned>(ceil_div_ll(rows * 32, 256))), dim3(256), 0, st,
       static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), B, T, H, delta,
       tab != nullptr ? dgate : nullptr));
   B200_CHECK_LAUNCH();
 
-  CUtensorMap tm_qkv, tm_do, tm_dq;
-  if (make_qkv_tmap(&tm_qkv, qkv, T, B, 3 * D, kAttnTile)) return -3;
-  if (make_qkv_tmap(&tm_do, dout, T, B, D, kAttnTile)) return -3;
-  if (make_f32_rows_tmap(&tm_dq, dq_acc, T, B, D, 64)) return -3;
+  CUtensorMap tm_qkv, tm_do, tm_dq, tm_qkv16, tm_do16, tm_dq16;
+  const int box_rows = head_dim == 64 ? kAttnTile : BwdMap<80>::kQT;
+  if (make_qkv_tmap(&tm_qkv, qkv, T, B, 3 * D, 64, box_rows)) return -3;
+  if (make_qkv_tmap(&tm_do, dout, T, B, D, 64, box_rows)) return -3;
+  if (make_f32_rows_tmap(&tm_dq, dq_acc, T, B, D, 32, 64)) return -3;
+  if (head_dim == 80) {
+    if (make_qkv_tmap(&tm_qkv16, qkv, T, B, 3 * D, 16, box_rows)) return -3;
+    if (make_qkv_tmap(&tm_do16, dout, T, B, D, 16, box_rows)) return -3;
+    if (make_f32_rows_tmap(&tm_dq16, dq_acc, T, B, D, 16, 64)) return -3;
+  } else {  // not read
+    tm_qkv16 = tm_qkv;
+    tm_do16 = tm_do;
+    tm_dq16 = tm_dq;
+  }
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.T = T; p.H = H; p.B = B; p.D = D;
@@ -549,13 +625,15 @@ static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, c
   p.drop_mask = const_cast<uint32_t*>(drop_mask);
   p.drop_rp = 1.0f / (1.0f - drop_p);
   const int N = p.n_tiles;
-  const int smem = kFSmem;
+  const int smem = head_dim == 64 ? BwdMap<64>::kFSmem : BwdMap<80>::kFSmem;
   dim3 grid(N, H, B);
-  void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnParams) =
-      tab != nullptr ? (drop ? attn_bwd_fused_kernel<true, true> : attn_bwd_fused_kernel<true, false>)
-                     : (drop ? attn_bwd_fused_kernel<false, true> : attn_bwd_fused_kernel<false, false>);
+  void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+               const AttnParams) =
+      head_dim == 80 ? (drop ? attn_bwd_fused_kernel<80, false, true> : attn_bwd_fused_kernel<80, false, false>)
+      : tab != nullptr ? (drop ? attn_bwd_fused_kernel<64, true, true> : attn_bwd_fused_kernel<64, true, false>)
+                       : (drop ? attn_bwd_fused_kernel<64, false, true> : attn_bwd_fused_kernel<64, false, false>);
   B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFThreads), smem, st, tm_qkv, tm_do, tm_dq, p));
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFThreads), smem, st, tm_qkv, tm_do, tm_dq, tm_qkv16, tm_do16, tm_dq16, p));
   B200_CHECK_LAUNCH();
   const long long nvec = rows * (D / 8);
   const int blocks = static_cast<int>(std::min<long long>(ceil_div_ll(nvec, 256), static_cast<long long>(sm_count()) * 16));
@@ -576,17 +654,19 @@ extern "C" {
 // The fp32 dQ reduction buffer is allocated on the stream for the call (b200s_attn_bwd_fused takes it from the caller).
 int b200s_attn_bwd(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                    const uint8_t* key_pad, const float* lse, float* delta, void* dqkv, float* dgate, float* dtab, int B,
-                   int T, int H, float scale, b200s_stream stream) {
+                   int T, int H, float scale, int head_dim, b200s_stream stream) {
   B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv, "attn_bwd: null pointer");
+  B200_CHECK_ARG(head_dim == 64 || head_dim == 80, "attn_bwd: head_dim=%d is not supported (64 or 80)", head_dim);
+  B200_CHECK_ARG(head_dim == 64 || tab == nullptr, "attn_bwd: the relative-position bias needs head_dim 64 (got %d)", head_dim);
   B200_CHECK_ARG(T >= 1, "attn_bwd: T=%d out of range", T);
   B200_CHECK_ARG(!tab || (dgate && dtab), "attn_bwd: bias given but dgate/dtab missing");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t bytes = sizeof(float) * static_cast<size_t>(B) * T * H * kHeadDim;
+  const size_t bytes = sizeof(float) * static_cast<size_t>(B) * T * H * head_dim;
   void* dq_acc = nullptr;
   B200_CHECK_CUDA(cudaMallocAsync(&dq_acc, bytes, st));
   B200_CHECK_CUDA(cudaMemsetAsync(dq_acc, 0, bytes, st));
   const int rc = attn_bwd_launch(qkv, out, dout, gate, tab, key_pad, lse, delta, static_cast<float*>(dq_acc), dqkv, dgate, dtab, B,
-                                 T, H, scale, 0.f, nullptr, st);
+                                 T, H, scale, 0.f, nullptr, head_dim, st);
   B200_CHECK_CUDA(cudaFreeAsync(dq_acc, st));
   return rc;
 }
@@ -596,21 +676,24 @@ int b200s_attn_bwd(const void* qkv, const void* out, const void* dout, const flo
 int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                                  const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv,
                                  float* dgate, float* dtab, int B, int T, int H, float scale, float drop_p,
-                                 const uint32_t* drop_mask, b200s_stream stream) {
+                                 const uint32_t* drop_mask, int head_dim, b200s_stream stream) {
   B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv && dq_acc, "attn_bwd_fused: null pointer");
+  B200_CHECK_ARG(head_dim == 64 || head_dim == 80, "attn_bwd_fused: head_dim=%d is not supported (64 or 80)", head_dim);
+  B200_CHECK_ARG(head_dim == 64 || tab == nullptr, "attn_bwd_fused: the relative-position bias needs head_dim 64 (got %d)",
+                 head_dim);
   B200_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f, "attn_bwd_fused: dropout p=%f out of range [0,1)", static_cast<double>(drop_p));
   B200_CHECK_ARG(drop_p == 0.f || drop_mask != nullptr, "attn_bwd_fused: dropout needs the mask written by b200s_attn_fwd_dropout");
   B200_CHECK_ARG(T >= 1, "attn_bwd_fused: T=%d out of range", T);
   B200_CHECK_ARG(!tab || (dgate && dtab), "attn_bwd_fused: bias given but dgate/dtab missing");
   return attn_bwd_launch(qkv, out, dout, gate, tab, key_pad, lse, delta, dq_acc, dqkv, dgate, dtab, B, T, H, scale, drop_p,
-                         drop_mask, static_cast<cudaStream_t>(stream));
+                         drop_mask, head_dim, static_cast<cudaStream_t>(stream));
 }
 
 int b200s_attn_bwd_fused(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                          const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv, float* dgate,
-                         float* dtab, int B, int T, int H, float scale, b200s_stream stream) {
+                         float* dtab, int B, int T, int H, float scale, int head_dim, b200s_stream stream) {
   return b200s_attn_bwd_fused_dropout(qkv, out, dout, gate, tab, key_pad, lse, delta, dq_acc, dqkv, dgate, dtab, B, T, H, scale,
-                                      0.f, nullptr, stream);
+                                      0.f, nullptr, head_dim, stream);
 }
 
 }  // extern "C"

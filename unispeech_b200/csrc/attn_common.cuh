@@ -7,8 +7,12 @@
 // consecutive entries of the per-head table.  Each kernel stages that window per tile in shared memory (the forward one key tile
 // ahead, the backward 128 new entries per query tile) and adds gate_i * tab[j-i] inside the softmax loop, so shared memory is
 // constant in T: 88,352 bytes for the forward, 176,128 for the backward.
-// Layout: q/k/v are column slices of the fused projection output qkv[B, T, 3D] (head h of q at columns h*64.., k at
-// D + h*64.., v at 2D + h*64..), read by TMA with a strided 3-D tensor map; no head-major reshuffle exists.
+// Layout: q/k/v are column slices of the fused projection output qkv[B, T, 3D] (head h of q at columns h*HD.., k at
+// D + h*HD.., v at 2D + h*HD..), read by TMA with a strided 3-D tensor map; no head-major reshuffle exists.
+// Head width HD is 64 or 80 (a template parameter of the kernels).  A [rows][HD] tile is one 64-column SWIZZLE_128B block
+// ([rows][128 B]) and, at HD = 80, a 16-column SWIZZLE_32B block ([rows][32 B]) right behind it: a 160-byte row is wider than
+// the 128-byte swizzle span, and the two boxes load exactly the head's columns.  K = 80 products are four k16 steps on the
+// first block and one on the second; N = 80 products are an n64 and an n16 wgmma on the same A operand.
 #pragma once
 #include "dropout.cuh"
 #include "ptx.cuh"
@@ -16,11 +20,22 @@
 namespace b200 {
 
 constexpr int kAttnTile = 128;  // queries per CTA tile == keys per tile
-constexpr int kHeadDim = 64;
 constexpr float kLog2e = 1.4426950408889634f;
 
+// one [ROWS][HD] bf16 tile of a [B, T, cols] tensor (columns c0 .., rows row0 ..) into `dst` in the layout above, as boxes of
+// BOX_ROWS rows: m64 holds the 64-column SWIZZLE_128B map, m16 the 16-column SWIZZLE_32B map (read only at HD = 80)
+template <int HD, int ROWS, int BOX_ROWS>
+__device__ __forceinline__ void tma_load_head(uint8_t* dst, const CUtensorMap* m64, const CUtensorMap* m16, uint64_t* bar,
+                                              int c0, int row0, int b) {
+#pragma unroll
+  for (int r = 0; r < ROWS; r += BOX_ROWS) {
+    tma_load_4d(dst + r * 128, m64, bar, c0, row0 + r, b, 0);
+    if (HD == 80) tma_load_4d(dst + ROWS * 128 + r * 32, m16, bar, c0 + 64, row0 + r, b, 0);
+  }
+}
+
 struct AttnParams {
-  int T, H, B, D;          // D = H * 64
+  int T, H, B, D;          // D = H * head width
   int n_tiles;             // ceil(T / 128)
   float scale;             // head_dim^-0.5
   const float* gate;       // [B,H,T] or null (=1)

@@ -28,7 +28,10 @@
 // few MB and stays in L2.
 // Dropout: the keep bits of a column pair are one hash word; a warp holds 16 consecutive query rows, i.e. one 16-bit half of
 // each mask word, which it assembles from ballots and stores as u16 (no cross-warp merge).
-// Shared memory: 81920 B of Q / K / V rings + 2 x 2704 B of stages + 1024 B alignment = 88352 B for every T.
+// Head width HD = 64 or 80 (attn_common.cuh): at 80 a tile is 20 KB instead of 16, S = Q K^T takes a fifth k16 step on the
+// SWIZZLE_32B blocks and O += P V an n16 wgmma next to the n64 one, so O is 40 fp32 registers per thread instead of 32.
+// Shared memory: 5 tiles of Q / K / V rings (81920 B at HD 64, 102400 B at 80) + 2 x 2704 B of stages + 1024 B alignment
+// = 88352 B (HD 64) or 108832 B (HD 80) for every T.
 #include "../../include/unispeech_b200.h"
 #include "attn_common.cuh"
 #include "common.h"
@@ -49,22 +52,28 @@ __device__ __forceinline__ uint32_t gather_every4th_bit(uint32_t x) {
   return (x | (x >> 12)) & 0xFFu;
 }
 
-constexpr int kFwdQ = 0;                        // 16 KB: rows of consumer c at 8192 c
-constexpr int kFwdK = 16384;                    // 2 x 16 KB ring
-constexpr int kFwdV = 49152;                    // 2 x 16 KB ring
-constexpr int kFwdStage = 81920;                // two per-key-tile stages (bias copies, key mask, flag)
 constexpr int kFwdThreads = 288;                // two consumer warpgroups + one producer warp
 // floats of ONE bias-window copy: 256 entries + 16, so that the two copies sit 16 banks apart (a warp's 8-byte loads touch 14
 // consecutive floats of each copy: no bank conflict)
 constexpr int kTabStride = 2 * kAttnTile + 16;
 constexpr int kMaskOff = 2 * kTabStride;        // the key mask, then the flag
 constexpr int kStageFloats = kMaskOff + kAttnTile + 4;
-constexpr int kFwdSmem = kFwdStage + 2 * kStageFloats * 4 + 1024;   // 88352 (+ 1024 for the alignment of the base)
+// shared-memory map of head width HD: Q tile (rows of consumer c at 8192 c, and 2048 c in the 32-byte block), 2-stage K and V
+// rings, then the two per-key-tile stages (bias copies, key mask, flag)
+template <int HD>
+struct FwdMap {
+  static constexpr int kTile = kAttnTile * HD * 2;  // one [128][HD] bf16 tile
+  static constexpr int kQ = 0, kK = kTile, kV = 3 * kTile, kStage = 5 * kTile;
+  static constexpr int kSmem = kStage + 2 * kStageFloats * 4 + 1024;  // (+ 1024 for the alignment of the base)
+};
 constexpr float kRebase = 1.2089258e24f;        // 2^80: a tile whose row sum reaches this is re-based on its own maximum
 
-template <bool HAS_BIAS, bool DROP>
+template <int HD, bool HAS_BIAS, bool DROP>
 __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_constant__ CUtensorMap tm,
+                                                                 const __grid_constant__ CUtensorMap tm16,
                                                                  const __grid_constant__ AttnParams p) {
+  static_assert(HD == 64 || (HD == 80 && !HAS_BIAS), "head width 64, or 80 without the relative-position bias");
+  using M = FwdMap<HD>;
   pdl_grid_sync();
   const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
   const int q0 = blockIdx.x * kAttnTile, h = blockIdx.y, b = blockIdx.z;
@@ -72,8 +81,8 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, still a __shared__ pointer (LDS/STS, not generic)
-  uint8_t* sQ = smem + kFwdQ;
-  float* stage = reinterpret_cast<float*>(smem + kFwdStage);
+  uint8_t* sQ = smem + M::kQ;
+  float* stage = reinterpret_cast<float*>(smem + M::kStage);
 
   __shared__ uint64_t q_full, k_full[2], k_empty[2], v_full[2], v_empty[2], stage_full[2];
 
@@ -100,9 +109,9 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
   // ---- a CTA whose query rows are all padded (or beyond T) has nothing to compute
   if (p.key_pad != nullptr && live_s == 0) {
     if (tid < kAttnTile && q0 + tid < T) {
-      uint4* dst = reinterpret_cast<uint4*>(p.out + (static_cast<long long>(b) * T + q0 + tid) * D + h * kHeadDim);
+      uint4* dst = reinterpret_cast<uint4*>(p.out + (static_cast<long long>(b) * T + q0 + tid) * D + h * HD);
 #pragma unroll
-      for (int g = 0; g < 8; ++g) dst[g] = make_uint4(0u, 0u, 0u, 0u);
+      for (int g = 0; g < HD / 8; ++g) dst[g] = make_uint4(0u, 0u, 0u, 0u);
       if (p.lse != nullptr) p.lse[(static_cast<long long>(b) * p.H + h) * T + q0 + tid] = INFINITY;
     }
     return;
@@ -110,18 +119,19 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
 
   auto load_k = [&](int n) {
     const int s = n & 1;
-    mbar_expect_tx(&k_full[s], 16384);
-    tma_load_4d(smem + kFwdK + s * 16384, &tm, &k_full[s], D + h * kHeadDim, n * kAttnTile, b, 0);
+    mbar_expect_tx(&k_full[s], M::kTile);
+    tma_load_head<HD, kAttnTile, kAttnTile>(smem + M::kK + s * M::kTile, &tm, &tm16, &k_full[s], D + h * HD, n * kAttnTile, b);
   };
   auto load_v = [&](int n) {
     const int s = n & 1;
-    mbar_expect_tx(&v_full[s], 16384);
-    tma_load_4d(smem + kFwdV + s * 16384, &tm, &v_full[s], 2 * D + h * kHeadDim, n * kAttnTile, b, 0);
+    mbar_expect_tx(&v_full[s], M::kTile);
+    tma_load_head<HD, kAttnTile, kAttnTile>(smem + M::kV + s * M::kTile, &tm, &tm16, &v_full[s], 2 * D + h * HD, n * kAttnTile, b);
   };
   if (tid == 0) {
     // the TMA thread initialises the barriers and puts Q and the first two K / V tiles in flight right away (the other warps
     // see the barriers after the __syncthreads below)
     tma_prefetch_desc(&tm);
+    if (HD == 80) tma_prefetch_desc(&tm16);
     mbar_init(&q_full, 1);
 #pragma unroll
     for (int s = 0; s < 2; ++s) {
@@ -132,8 +142,8 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
       mbar_init(&stage_full[s], 32);  // one arrival per lane of the stage warp once its part of the stage is stored
     }
     fence_mbar_init();
-    mbar_expect_tx(&q_full, 16384);
-    tma_load_4d(sQ, &tm, &q_full, h * kHeadDim, q0, b, 0);
+    mbar_expect_tx(&q_full, M::kTile);
+    tma_load_head<HD, kAttnTile, kAttnTile>(sQ, &tm, &tm16, &q_full, h * HD, q0, b);
     for (int n = 0; n < 2 && n < n_eff; ++n) {
       load_k(n);
       load_v(n);
@@ -222,9 +232,12 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
                                                            (N * kAttnTile)) + ((row16 >> 4) & 1);
   }
 
-  float o[32];  // O rows r0, r0 + 8 x 64 columns, fragment layout
+  float o[32];   // O rows r0, r0 + 8 x columns 0..63, fragment layout
+  float o16[8];  // ... x columns 64..79 (HD = 80 only)
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) o16[i] = 0.f;
   float m_ref[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   const uint32_t aQ = smem_u32(sQ) + 8192 * c;
 
@@ -239,13 +252,16 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
     uint32_t pk[32];  // P: bf16 pairs in the register-A layout (pk[i / 2] = columns of acc[i], acc[i + 1])
     mbar_wait(&k_full[s], (n >> 1) & 1);
     named_bar_sync(1 + c, 2 * 128);
-    const uint32_t bK = smem_u32(smem + kFwdK + s * 16384);
+    const uint32_t bK = smem_u32(smem + M::kK + s * M::kTile);
     auto qk = [&]() {  // S = Q K_n^T
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < 4; ++k)
         wgmma_m64n128k16<0, 0>(acc, make_smem_desc_sw128(aQ + k * 32, 16, 1024), make_smem_desc_sw128(bK + k * 32, 16, 1024),
                                k > 0 ? 1u : 0u);
+      if (HD == 80)  // columns 64..79: the 32-byte blocks behind the 128-row tiles
+        wgmma_m64n128k16<0, 0>(acc, make_smem_desc_sw32(smem_u32(sQ) + kAttnTile * 128 + 2048 * c),
+                               make_smem_desc_sw32(bK + kAttnTile * 128), 1u);
       wgmma_commit();
     };
     qk();
@@ -363,6 +379,11 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
           o[4 * g + 2 * rr] *= factor;
           o[4 * g + 2 * rr + 1] *= factor;
         }
+#pragma unroll
+        for (int g = 0; g < 2; ++g) {
+          o16[4 * g + 2 * rr] *= factor;
+          o16[4 * g + 2 * rr + 1] *= factor;
+        }
       }
     }
     if (lane == 0) mbar_arrive(&k_empty[s]);
@@ -371,10 +392,13 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
 
     // ---- O += P V_n: P as the register A operand
     mbar_wait(&v_full[s], (n >> 1) & 1);
-    const uint32_t bV = smem_u32(smem + kFwdV + s * 16384);
+    const uint32_t bV = smem_u32(smem + M::kV + s * M::kTile);
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 8; ++k) wgmma_m64n64k16_rs<1>(o, pk + 4 * k, make_smem_desc_sw128(bV + k * 2048, 8192, 1024), 1u);
+    for (int k = 0; k < 8; ++k) {
+      wgmma_m64n64k16_rs<1>(o, pk + 4 * k, make_smem_desc_sw128(bV + k * 2048, 8192, 1024), 1u);
+      if (HD == 80) wgmma_m64n16k16_rs<1>(o16, pk + 4 * k, make_smem_desc_sw32(bV + kAttnTile * 128 + k * 512), 1u);
+    }
     wgmma_commit();
     wgmma_wait<0>();
     if (lane == 0) mbar_arrive(&v_empty[s]);
@@ -391,15 +415,20 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
       if (p.lse != nullptr && quad == 0)
         p.lse[(static_cast<long long>(b) * p.H + h) * T + row] = (l > 0.f) ? (m_ref[rr] + log2f(l)) : INFINITY;
       const float inv = l > 0.f ? (DROP ? p.drop_rp : 1.0f) / l : 0.f;
-      __nv_bfloat16* dst = p.out + (static_cast<long long>(b) * T + row) * D + h * kHeadDim + 2 * quad;
+      __nv_bfloat16* dst = p.out + (static_cast<long long>(b) * T + row) * D + h * HD + 2 * quad;
 #pragma unroll
       for (int g = 0; g < 8; ++g)
         *reinterpret_cast<uint32_t*>(dst + 8 * g) = pack_bf16x2(o[4 * g + 2 * rr] * inv, o[4 * g + 2 * rr + 1] * inv);
+      if (HD == 80) {
+#pragma unroll
+        for (int g = 0; g < 2; ++g)
+          *reinterpret_cast<uint32_t*>(dst + 64 + 8 * g) = pack_bf16x2(o16[4 * g + 2 * rr] * inv, o16[4 * g + 2 * rr + 1] * inv);
+      }
     }
   }
 }
 
-int make_qkv_tmap(CUtensorMap* out, const void* qkv, int T, int B, int D3, int box_rows);
+int make_qkv_tmap(CUtensorMap* out, const void* qkv, int T, int B, int D3, int box_cols, int box_rows);
 
 }  // namespace b200
 
@@ -407,26 +436,34 @@ using namespace b200;
 
 extern "C" {
 
-// out[b,t,h*64+d] = softmax_j(scale q.k + gate*tab[j-i], key padding) v     (WavLM/modules.py:540-563 replaced)
+// out[b,t,h*HD+d] = softmax_j(scale q.k + gate*tab[j-i], key padding) v     (WavLM/modules.py:540-563 replaced)
 // qkv: bf16 [B,T,3D] fused projection output; gate: fp32 [B,H,T] or NULL; tab: fp32 [H,2T-1] or NULL (no bias);
 // key_pad: uint8 [B,T] or NULL; out: bf16 [B,T,D]; lse: fp32 [B,H,T] (log2-domain log-sum-exp, saved for backward).
-// Rows of `out` at padded query frames are unspecified-but-finite (zeros where a whole 128-row block is padded).
+// head_dim HD: 64, or 80 without the bias.  Rows of `out` at padded query frames are unspecified-but-finite (zeros where a
+// whole 128-row block is padded).
 int b200s_attn_fwd_dropout(const void* qkv, const float* gate, const float* tab, const uint8_t* key_pad, void* out, float* lse,
                            int B, int T, int H, float scale, float drop_p, uint32_t key0, uint32_t key1, uint32_t* drop_mask,
-                           b200s_stream stream) {
+                           int head_dim, b200s_stream stream) {
   B200_CHECK_ARG(qkv && out, "attn_fwd: null pointer");
+  B200_CHECK_ARG(head_dim == 64 || head_dim == 80, "attn_fwd: head_dim=%d is not supported (64 or 80)", head_dim);
+  B200_CHECK_ARG(head_dim == 64 || tab == nullptr, "attn_fwd: the relative-position bias needs head_dim 64 (got %d)", head_dim);
   B200_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f, "attn_fwd: dropout p=%f out of range [0,1)", static_cast<double>(drop_p));
   B200_CHECK_ARG(drop_p == 0.f || drop_mask != nullptr, "attn_fwd: dropout needs the mask buffer (b200s_attn_dropout_mask_words)");
   B200_CHECK_ARG(static_cast<long long>(B) * H * T < (1LL << 32), "attn_fwd: B*H*T exceeds the 32-bit dropout row counter");
-  const int D = H * kHeadDim;
-  CUtensorMap tm;
+  const int D = H * head_dim;
+  CUtensorMap tm, tm16;
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.T = T; p.H = H; p.B = B; p.D = D;
   p.n_tiles = ceil_div(T, kAttnTile);
   B200_CHECK_ARG(T >= 1, "attn_fwd: T=%d out of range", T);
-  const int smem = kFwdSmem;
-  if (make_qkv_tmap(&tm, qkv, T, B, 3 * D, kAttnTile)) return -3;
+  const int smem = head_dim == 64 ? FwdMap<64>::kSmem : FwdMap<80>::kSmem;
+  if (make_qkv_tmap(&tm, qkv, T, B, 3 * D, 64, kAttnTile)) return -3;
+  if (head_dim == 80) {
+    if (make_qkv_tmap(&tm16, qkv, T, B, 3 * D, 16, kAttnTile)) return -3;
+  } else {
+    tm16 = tm;  // not read
+  }
   p.scale = scale;
   p.gate = gate; p.tab = tab; p.key_pad = key_pad;
   p.out = static_cast<__nv_bfloat16*>(out);
@@ -438,18 +475,19 @@ int b200s_attn_fwd_dropout(const void* qkv, const float* gate, const float* tab,
   p.drop_rp = 1.0f / (1.0f - drop_p);
   dim3 grid(ceil_div(T, kAttnTile), H, B);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  void (*kern)(const CUtensorMap, const AttnParams) =
-      tab != nullptr ? (drop ? attn_fwd_kernel<true, true> : attn_fwd_kernel<true, false>)
-                     : (drop ? attn_fwd_kernel<false, true> : attn_fwd_kernel<false, false>);
+  void (*kern)(const CUtensorMap, const CUtensorMap, const AttnParams) =
+      head_dim == 80 ? (drop ? attn_fwd_kernel<80, false, true> : attn_fwd_kernel<80, false, false>)
+      : tab != nullptr ? (drop ? attn_fwd_kernel<64, true, true> : attn_fwd_kernel<64, true, false>)
+                       : (drop ? attn_fwd_kernel<64, false, true> : attn_fwd_kernel<64, false, false>);
   B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFwdThreads), smem, st, tm, p));
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFwdThreads), smem, st, tm, tm16, p));
   B200_CHECK_LAUNCH();
   return 0;
 }
 
 int b200s_attn_fwd(const void* qkv, const float* gate, const float* tab, const uint8_t* key_pad, void* out, float* lse,
-                   int B, int T, int H, float scale, b200s_stream stream) {
-  return b200s_attn_fwd_dropout(qkv, gate, tab, key_pad, out, lse, B, T, H, scale, 0.f, 0u, 0u, nullptr, stream);
+                   int B, int T, int H, float scale, int head_dim, b200s_stream stream) {
+  return b200s_attn_fwd_dropout(qkv, gate, tab, key_pad, out, lse, B, T, H, scale, 0.f, 0u, 0u, nullptr, head_dim, stream);
 }
 
 long long b200s_attn_dropout_mask_words(int B, int T, int H) { return attn_drop_mask_words(B, H, T); }

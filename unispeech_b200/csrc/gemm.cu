@@ -64,7 +64,8 @@ struct ViewSpec {
   int box[4];
 };
 
-// bf16, 128B swizzle, zero OOB fill.  Returns 0 on success.
+// bf16, zero OOB fill; 128B swizzle, or 32B for a box of 16 columns (the last 16 columns of an 80-wide attention head).
+// Returns 0 on success.
 static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
@@ -100,7 +101,8 @@ static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
   static const CUtensorMapL2promotion kPromo[4] = {CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_64B,
                                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(v.ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, kPromo[promo], CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, v.box[0] == 16 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                  kPromo[promo], CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled failed (%d): dims {%lld,%lld,%lld,%lld} strides {%lld,%lld,%lld} box {%d,%d,%d,%d}",
                    static_cast<int>(r), v.dims[0], v.dims[1], v.dims[2], v.dims[3], v.strides[0], v.strides[1],
@@ -110,9 +112,10 @@ static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
   return 0;
 }
 
-// [B, T, cols] bf16 row-major activations: box = 64 columns x box_rows rows (used by the attention kernels)
-int make_qkv_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int box_rows) {
-  ViewSpec v{ptr, {cols, T, B, 1}, {cols, static_cast<long long>(T) * cols, 0}, {64, box_rows, 1, 1}};
+// [B, T, cols] bf16 row-major activations: box = box_cols (64, SWIZZLE_128B, or 16, SWIZZLE_32B) columns x box_rows rows
+// (used by the attention kernels)
+int make_qkv_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int box_cols, int box_rows) {
+  ViewSpec v{ptr, {cols, T, B, 1}, {cols, static_cast<long long>(T) * cols, 0}, {box_cols, box_rows, 1, 1}};
   return make_tmap(out, v);
 }
 
@@ -124,8 +127,9 @@ int make_rows_tmap(CUtensorMap* out, const void* ptr, long long cols, long long 
 }
 
 // [B, T, cols] fp32 row-major (the attention backward's dQ accumulator): rank 3 (cols, T, B), so a box clips at T inside each
-// utterance; box = 32 columns (one 128-byte swizzle row) x box_rows rows.  Used as the destination of TMA reductions.
-int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_rows) {
+// utterance; box = 32 columns (one 128-byte swizzle row) or 16 columns (64-byte rows, not swizzled) x box_rows rows.  Used as
+// the destination of TMA reductions.
+int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_cols, int box_rows) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
     set_last_error("cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
@@ -133,11 +137,11 @@ int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int col
   }
   const cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(T), static_cast<cuuint64_t>(B)};
   const cuuint64_t strides[2] = {static_cast<cuuint64_t>(cols) * 4, static_cast<cuuint64_t>(T) * cols * 4};
-  const cuuint32_t box[3] = {32, static_cast<cuuint32_t>(box_rows), 1};
+  const cuuint32_t box[3] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows), 1};
   const cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled failed (%d) for the fp32 [%d, %d, %d] map", static_cast<int>(r), B, T, cols);
     return -3;
@@ -383,13 +387,15 @@ int b200s_posconv_gemm(const void* xpad, long long xpad_bs, int T, int B, int D,
   B200_CHECK_ARG(xpad && wp && out, "posconv_gemm: null pointer");
   B200_CHECK_ARG(D % G == 0, "posconv_gemm: D %% G != 0");
   const int Cg = D / G;
-  B200_CHECK_ARG(Cg <= 64 && Cg % 8 == 0, "posconv_gemm: channels per group %d must be <=64 and a multiple of 8", Cg);
+  B200_CHECK_ARG(Cg <= 128 && Cg % 8 == 0, "posconv_gemm: channels per group %d must be <=128 and a multiple of 8", Cg);
   B200_CHECK_ARG(D % 8 == 0, "posconv_gemm: D must be a multiple of 8");
   B200_CHECK_ARG(taps >= 1, "posconv_gemm: taps=%d must be positive", taps);
+  const int KB = Cg <= 64 ? 1 : 2;  // 64-channel blocks of the padded group width Cgp
+  B200_CHECK_ARG(KB == 1 || taps <= 129, "posconv_gemm: %d channels per group needs taps <= 129 (got %d)", Cg, taps);
   if (check_epilogue(epi)) return -1;
 
   CUtensorMap ta, tb;
-  ViewSpec vb{wp, {taps * 64LL, G * 64LL, 1, 1}, {taps * 64LL, 0, 0}, {64, 64, 1, 1}};
+  ViewSpec vb{wp, {taps * 64LL * KB, G * 64LL * KB, 1, 1}, {taps * 64LL * KB, 0, 0}, {64, 64, 1, 1}};
   if (make_tmap(&tb, vb)) return -3;
 
   GemmParams p;
@@ -407,7 +413,7 @@ int b200s_posconv_gemm(const void* xpad, long long xpad_bs, int T, int B, int D,
   p.flags = 0;
   fill_epilogue(p, epi);
   p.out = {out, out_bs, out_ld};
-  dim3 grid(G, p.m_tiles_per_batch * B, 1);
+  dim3 grid(G * KB, p.m_tiles_per_batch * B, 1);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
   if (taps <= 129) {
@@ -418,12 +424,19 @@ int b200s_posconv_gemm(const void* xpad, long long xpad_bs, int T, int B, int D,
     static std::once_flag once;
     static cudaError_t attr_err = cudaSuccess;
     std::call_once(once, [] {
-      attr_err = cudaFuncSetAttribute(posconv_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      PosconvCfg::kSmemBytes);
+      attr_err = cudaFuncSetAttribute(posconv_window_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      PosconvCfg<1>::kSmemBytes);
+      if (attr_err == cudaSuccess)
+        attr_err = cudaFuncSetAttribute(posconv_window_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        PosconvCfg<2>::kSmemBytes);
     });
     B200_CHECK_CUDA(attr_err);
-    B200_CHECK_CUDA(launch_pdl(posconv_window_kernel, grid, dim3(PosconvCfg::kThreads), PosconvCfg::kSmemBytes, st, ta, tb, p,
-                               taps, Cg));
+    if (KB == 1)
+      B200_CHECK_CUDA(launch_pdl(posconv_window_kernel<1>, grid, dim3(PosconvCfg<1>::kThreads), PosconvCfg<1>::kSmemBytes, st, ta,
+                                 tb, p, taps, Cg));
+    else
+      B200_CHECK_CUDA(launch_pdl(posconv_window_kernel<2>, grid, dim3(PosconvCfg<2>::kThreads), PosconvCfg<2>::kSmemBytes, st, ta,
+                                 tb, p, taps, Cg));
     B200_CHECK_LAUNCH();
     return 0;
   }
@@ -441,34 +454,41 @@ int b200s_posconv_wgrad(const void* dy, long long dy_bs, long long dy_rs, const 
   B200_CHECK_ARG(dy && xpad && dwp, "posconv_wgrad: null pointer");
   B200_CHECK_ARG(D % G == 0, "posconv_wgrad: D %% G != 0");
   const int Cg = D / G;
-  B200_CHECK_ARG(Cg <= 64 && Cg % 8 == 0, "posconv_wgrad: channels per group %d must be <=64 and a multiple of 8", Cg);
+  B200_CHECK_ARG(Cg <= 128 && Cg % 8 == 0, "posconv_wgrad: channels per group %d must be <=128 and a multiple of 8", Cg);
+  const int Cgp = Cg <= 64 ? 64 : 128;
 
-  CUtensorMap ta, tb;
+  CUtensorMap ta;
   ViewSpec va{dy, {D, T, B, 1}, {dy_rs, B > 1 ? dy_bs : 0, 0}, {64, 64, 1, 1}};
   if (make_tmap(&ta, va)) return -3;
-  ViewSpec vb{xpad, {D, taps, T, B}, {D, D, xpad_bs}, {64, 1, 64, 1}};
-  if (make_tmap(&tb, vb)) return -3;
+  // one launch per 64 input channels of the group: launch h reads xpad from channel 64 h of each group on (a view whose
+  // channels past D are zero-filled) and writes columns 64 h .. of each tap's Cgp-wide block of dwp
+  for (int h = 0; h * 64 < Cg; ++h) {
+    CUtensorMap tb;
+    ViewSpec vb{static_cast<const __nv_bfloat16*>(xpad) + 64 * h, {D - 64 * h, taps, T, B}, {D, D, xpad_bs}, {64, 1, 64, 1}};
+    if (make_tmap(&tb, vb)) return -3;
 
-  GemmParams p;
-  memset(&p, 0, sizeof(p));
-  p.m_rows = D;
-  p.m_tile_stride = Cg;
-  p.m_tile_valid = Cg;
-  p.m_tiles_per_batch = G;
-  p.n_total = taps * 64;
-  p.n_out_stride = 64;
-  p.n_tile_valid = 64;
-  p.k_blocks_per_batch = ceil_div(T, 64);
-  p.k_blocks = p.k_blocks_per_batch * B;
-  p.k_blocks_per_split = p.k_blocks;
-  // A coords: (m0 + sub, k0, kbatch, 0)   B coords: (m0, tap = n_tile, k0, kbatch)
-  p.ca[0][1] = 1; p.ca[0][7] = 1; p.ca[1][4] = 1; p.ca[2][5] = 1;
-  p.cb[0][1] = 1; p.cb[1][3] = 1; p.cb[2][4] = 1; p.cb[3][5] = 1;
-  p.flags = EPI_OUT_F32 | EPI_ATOMIC;
-  fill_epilogue(p, nullptr);
-  p.out = {dwp, 0, taps * 64LL};
-  dim3 grid(taps, G, 1);
-  return launch_gemm<64, true, true>(ta, tb, p, grid, static_cast<cudaStream_t>(stream));
+    GemmParams p;
+    memset(&p, 0, sizeof(p));
+    p.m_rows = D;
+    p.m_tile_stride = Cg;
+    p.m_tile_valid = Cg;
+    p.m_tiles_per_batch = G;
+    p.n_total = taps * Cgp;
+    p.n_out_stride = Cgp;
+    p.n_tile_valid = h == 0 ? 64 : Cg - 64 * h;  // (columns past Cg are never read)
+    p.k_blocks_per_batch = ceil_div(T, 64);
+    p.k_blocks = p.k_blocks_per_batch * B;
+    p.k_blocks_per_split = p.k_blocks;
+    // A coords: (m0 + sub, k0, kbatch, 0)   B coords: (m0, tap = n_tile, k0, kbatch)
+    p.ca[0][1] = 1; p.ca[0][7] = 1; p.ca[1][4] = 1; p.ca[2][5] = 1;
+    p.cb[0][1] = 1; p.cb[1][3] = 1; p.cb[2][4] = 1; p.cb[3][5] = 1;
+    p.flags = EPI_OUT_F32 | EPI_ATOMIC;
+    fill_epilogue(p, nullptr);
+    p.out = {dwp + 64 * h, 0, taps * static_cast<long long>(Cgp)};
+    dim3 grid(taps, G, 1);
+    if (const int rc = launch_gemm<64, true, true>(ta, tb, p, grid, static_cast<cudaStream_t>(stream))) return rc;
+  }
+  return 0;
 }
 
 }  // extern "C"

@@ -757,24 +757,29 @@ __global__ void __launch_bounds__(384, 1) gemm_ws_wgrad_kernel(const __grid_cons
 // shared-memory tile, shifted by j rows.  One 256-row TMA box brings the window in; every tap is four wgmma per consumer
 // warpgroup whose A descriptor starts j rows (j * 128 bytes) into the tile.  Only the per-tap weight tile (8 KB) streams through
 // the TMA ring, so the kernel reads ~1/3 of the bytes of the box-per-tap formulation.
-// grid (groups, m_tiles * batches); block 288 (two consumer warpgroups, TMA warp); fused tail = epilogue_chunk32.
+// grid (groups * KB, m_tiles * batches); block 288 (two consumer warpgroups, TMA warp); fused tail = epilogue_chunk32.
+// KB = 64-channel blocks of a group's padded width (Cgp = 64 KB): with KB = 2 (65..128 channels per group) the window and every
+// tap's weight tile are two 64-channel K blocks, and CTA (g, h) computes the group's output channels 64 h .. 64 h + 63 (the
+// epilogue keeps the valid ones; input channels past the group multiply zero weights).
+template <int KB>
 struct PosconvCfg {
-  static constexpr int kStages = 6;
-  static constexpr int kABytes = 256 * 128;  // 256 rows x 64 bf16
-  static constexpr int kBBytes = 64 * 128;   // 64 output channels x 64 input channels of one tap
+  static constexpr int kStages = KB == 1 ? 6 : 4;
+  static constexpr int kABytes = KB * 256 * 128;  // KB blocks of 256 rows x 64 bf16
+  static constexpr int kBBytes = KB * 64 * 128;   // 64 output channels x 64 KB input channels of one tap
   static constexpr int kSmemBytes = kABytes + kStages * kBBytes + 1024;
   static constexpr int kThreads = 288;
 };
 
+template <int KB>
 __global__ void __launch_bounds__(288, 2) posconv_window_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                 const __grid_constant__ CUtensorMap tmB,
                                                                 const __grid_constant__ GemmParams p, int taps, int cg) {
   pdl_launch_dependents();
-  using Cfg = PosconvCfg;
+  using Cfg = PosconvCfg<KB>;
   constexpr int kStages = Cfg::kStages;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int g = blockIdx.x;
+  const int g = blockIdx.x / KB, h = blockIdx.x % KB;
   const int mb = blockIdx.y / p.m_tiles_per_batch;
   const int m0 = (blockIdx.y % p.m_tiles_per_batch) * 128;
 
@@ -801,12 +806,16 @@ __global__ void __launch_bounds__(288, 2) posconv_window_kernel(const __grid_con
   if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(&a_full, Cfg::kABytes);
-      tma_load_4d(sA, &tmA, &a_full, g * cg, m0, mb, 0);  // rows m0 .. m0+255 of this group's channels (zero-filled past the end)
+#pragma unroll
+      for (int kb = 0; kb < KB; ++kb)  // rows m0 .. m0+255 of this group's channels (zero-filled past the end)
+        tma_load_4d(sA + kb * 32768, &tmA, &a_full, g * cg + 64 * kb, m0, mb, 0);
       for (int j = 0; j < taps; ++j) {
         const int s = j % kStages;
         mbar_wait(&empty_bar[s], ((j / kStages) & 1) ^ 1);
         mbar_expect_tx(&full_bar[s], Cfg::kBBytes);
-        tma_load_4d(sB + s * Cfg::kBBytes, &tmB, &full_bar[s], j * 64, g * 64, 0, 0);
+#pragma unroll
+        for (int kb = 0; kb < KB; ++kb)
+          tma_load_4d(sB + s * Cfg::kBBytes + kb * 8192, &tmB, &full_bar[s], (j * KB + kb) * 64, (g * KB + h) * 64, 0, 0);
       }
     }
   } else {
@@ -820,15 +829,17 @@ __global__ void __launch_bounds__(288, 2) posconv_window_kernel(const __grid_con
       const uint32_t sb = smem_u32(sB + s * Cfg::kBBytes);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_tile<64, false, false>(acc, make_smem_desc_sw128(sa + k * 32, 16, 1024), make_smem_desc_sw128(sb + k * 32, 16, 1024),
+      for (int k = 0; k < 4 * KB; ++k)
+        wgmma_tile<64, false, false>(acc, make_smem_desc_sw128(sa + (k >> 2) * 32768 + (k & 3) * 32, 16, 1024),
+                                     make_smem_desc_sw128(sb + (k >> 2) * 8192 + (k & 3) * 32, 16, 1024),
                                      (j > 0 || k > 0) ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<1>();
       if (j > 0 && lane == 0) mbar_arrive(&empty_bar[(j - 1) % kStages]);
     }
     wgmma_wait<0>();
-    gemm_consumer_tail<64>(p, acc, reinterpret_cast<float*>(smem), mb, m0, g * cg, cg, min(128, p.m_rows - m0));
+    gemm_consumer_tail<64>(p, acc, reinterpret_cast<float*>(smem), mb, m0, g * cg + 64 * h, min(64, cg - 64 * h),
+                           min(128, p.m_rows - m0));
   }
 }
 

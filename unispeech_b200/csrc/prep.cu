@@ -159,7 +159,9 @@ __global__ void unprep_conv_wgrad_kernel(const float* __restrict__ dwk, int Co, 
 }
 
 // ---- pos_conv weight norm -----------------------------------------------------------------------------------------
-// norm2[j] = sum_{co,ci} v[co,ci,j]^2  (and optionally dot[j] = sum dw*v for the backward).  The block partials are combined with
+// Channels per group Cg <= 128; the GEMM operands are padded to Cgp = 64 (Cg <= 64) or 128 channels per group (posconv_cgp).
+__host__ __device__ __forceinline__ int posconv_cgp(int Cg) { return Cg <= 64 ? 64 : 128; }
+// norm2[j] = sum_{co,ci} v[co,ci,j]^2  (and optionally dot[j] = sum dw*v for the backward; dwp is [G, Cg, taps, Cgp]).  The block partials are combined with
 // fp64 atomics: their order varies from launch to launch, but an fp64 sum of a few hundred fp32 partials rounds to the same fp32
 // value whatever the order (fp32 atomics did not: the weight norm, hence a few bf16 pos_conv weights, hence the whole forward pass
 // differed in the last bit between two runs on the same input -- found by tests/test_graph_gpu.py).
@@ -177,25 +179,26 @@ __global__ void posconv_tap_reduce_kernel(const float* __restrict__ v, const flo
     if (dwp) {
       const int co = r / Cg, ci = r % Cg;  // co global channel
       const int g = co / Cg, cog = co % Cg;
-      d += dwp[((static_cast<long long>(g) * Cg + cog) * taps + j) * 64 + ci] * x;
+      d += dwp[((static_cast<long long>(g) * Cg + cog) * taps + j) * posconv_cgp(Cg) + ci] * x;
     }
   }
   atomicAdd(norm2 + j, static_cast<double>(a));
   if (dwp) atomicAdd(dot + j, static_cast<double>(d));
 }
-// wp_fwd[(g*64+co), j*64+ci] = w[g*Cg+co, ci, j];   wp_dg[(g*64+ci), j'*64+co] = w[g*Cg+co, ci, taps-1-j']
+// wp_fwd[(g*Cgp+co), j*Cgp+ci] = w[g*Cg+co, ci, j];   wp_dg[(g*Cgp+ci), j'*Cgp+co] = w[g*Cg+co, ci, taps-1-j']
 // with w = gvec[j] * v / sqrt(norm2[j]); zero padding elsewhere.
 __global__ void posconv_prep_kernel(const float* __restrict__ v, const float* __restrict__ gvec,
                                     const double* __restrict__ norm2, int G, int Cg, int taps,
                                     __nv_bfloat16* __restrict__ wp_fwd, __nv_bfloat16* __restrict__ wp_dg) {
   pdl_grid_sync();
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const long long n = static_cast<long long>(G) * 64 * taps * 64;
+  const int P = posconv_cgp(Cg);
+  const long long n = static_cast<long long>(G) * P * taps * P;
   if (i >= n) return;
-  const int c = i % 64;            // inner (ci for fwd)
-  const int j = (i / 64) % taps;
-  const int r = (i / (64LL * taps)) % 64;  // row within group (co for fwd)
-  const int g = i / (64LL * taps * 64);
+  const int c = i % P;             // inner (ci for fwd)
+  const int j = (i / P) % taps;
+  const int r = (i / (static_cast<long long>(P) * taps)) % P;  // row within group (co for fwd)
+  const int g = i / (static_cast<long long>(P) * taps * P);
   float wf = 0.f, wd = 0.f;
   if (r < Cg && c < Cg) {
     // forward: row co=r, col ci=c, tap j
@@ -222,7 +225,7 @@ __global__ void posconv_unprep_kernel(const float* __restrict__ v, const float* 
   const int co = i / (static_cast<long long>(taps) * Cg);
   const int g = co / Cg, cog = co % Cg;
   const float inv = rsqrtf(static_cast<float>(norm2[j]));
-  const float dw = dwp[((static_cast<long long>(g) * Cg + cog) * taps + j) * 64 + ci];
+  const float dw = dwp[((static_cast<long long>(g) * Cg + cog) * taps + j) * posconv_cgp(Cg) + ci];
   dv[i] += gvec[j] * inv * dw - gvec[j] * static_cast<float>(dot[j]) * inv * inv * inv * v[i];
 }
 
@@ -295,7 +298,7 @@ int b200s_unprep_conv_wgrad(const float* dwk, int Co, int Ci, int k, float* dw, 
 int b200s_posconv_prep(const float* weight_v, const float* weight_g, int D, int G, int taps, float* norm2, void* wp_fwd,
                        void* wp_dgrad, b200s_stream stream) {
   B200_CHECK_ARG(weight_v && weight_g && norm2 && wp_fwd && wp_dgrad, "posconv_prep: null pointer");
-  B200_CHECK_ARG(taps <= 1024 && D % G == 0 && D / G <= 64, "posconv_prep: bad sizes");
+  B200_CHECK_ARG(taps <= 1024 && D % G == 0 && D / G <= 128, "posconv_prep: bad sizes (at most 128 channels per group)");
   const int Cg = D / G;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(norm2) & 7u) == 0, "posconv_prep: workspace must be 8-byte aligned");
@@ -304,7 +307,7 @@ int b200s_posconv_prep(const float* weight_v, const float* weight_g, int D, int 
   B200_CHECK_CUDA(launch_pdl(posconv_tap_reduce_kernel, dim3(4 * sm_count()), dim3(((taps + 31) / 32) * 32), 0, st, weight_v,
                              static_cast<const float*>(nullptr), D, Cg, taps, n2, static_cast<double*>(nullptr)));
   B200_CHECK_LAUNCH();
-  const long long n = static_cast<long long>(G) * 64 * taps * 64;
+  const long long n = static_cast<long long>(G) * posconv_cgp(Cg) * taps * posconv_cgp(Cg);
   B200_CHECK_CUDA(launch_pdl(posconv_prep_kernel, dim3(static_cast<unsigned>(ceil_div_ll(n, 256))), dim3(256), 0, st, 
       weight_v, weight_g, static_cast<const double*>(n2), G, Cg, taps, static_cast<__nv_bfloat16*>(wp_fwd),
       static_cast<__nv_bfloat16*>(wp_dgrad)));
@@ -312,10 +315,11 @@ int b200s_posconv_prep(const float* weight_v, const float* weight_g, int D, int 
   return 0;
 }
 
-// dwp: fp32 [G, Cg, taps, 64] from b200s_posconv_wgrad.  work: workspace of 4 * taps floats, 8-byte aligned (fp64[2 * taps]; zeroed here).
+// dwp: fp32 [G, Cg, taps, Cgp] from b200s_posconv_wgrad.  work: workspace of 4 * taps floats, 8-byte aligned (fp64[2 * taps]; zeroed here).
 int b200s_posconv_unprep(const float* weight_v, const float* weight_g, const float* dwp, int D, int G, int taps,
                          float* work, float* dweight_v, float* dweight_g, b200s_stream stream) {
   B200_CHECK_ARG(weight_v && weight_g && dwp && work && dweight_v && dweight_g, "posconv_unprep: null pointer");
+  B200_CHECK_ARG(D % G == 0 && D / G <= 128, "posconv_unprep: bad sizes (at most 128 channels per group)");
   const int Cg = D / G;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(work) & 7u) == 0, "posconv_unprep: workspace must be 8-byte aligned");

@@ -758,8 +758,9 @@ static int dispatch_width(int D, F&& f) {
     case 512: return f(std::integral_constant<int, 8>{}, std::integral_constant<int, 2>{});
     case 768: return f(std::integral_constant<int, 8>{}, std::integral_constant<int, 3>{});
     case 1024: return f(std::integral_constant<int, 8>{}, std::integral_constant<int, 4>{});
+    case 1280: return f(std::integral_constant<int, 8>{}, std::integral_constant<int, 5>{});
     default:
-      set_last_error("row kernels support widths 64/128/256/512/768/1024, got %d", D);
+      set_last_error("row kernels support widths 64/128/256/512/768/1024/1280, got %d", D);
       return -1;
   }
 }

@@ -173,6 +173,7 @@ class Engine:
     def __init__(self, model):
         self.m = model
         self.cfg = model.cfg
+        self.head_dim = self.cfg.encoder_embed_dim // self.cfg.encoder_attention_heads   # 64 or 80 (wavlm._check_supported)
         self.dev = None
         self.prepared_version = None
         self.lut_cache: Dict[int, torch.Tensor] = {}
@@ -198,7 +199,7 @@ class Engine:
         convs = m.conv_cfg
         C = convs[-1][0]
         assert all(c[0] == C for c in convs), "conv stack must have a constant channel count"
-        assert D == H * 64, "head_dim must be 64"
+        assert D == H * self.head_dim, "encoder_embed_dim must be a multiple of encoder_attention_heads"
         assert m.post_extract_proj is not None, "encoder_embed_dim must differ from the conv dim (projection layer)"
         e = lambda *s: torch.empty(*s, dtype=BF, device=device)
         self.wf, self.wd = {}, {}
@@ -209,7 +210,8 @@ class Engine:
             self.wd[i] = [e(C, ((k - rho + s - 1) // s) * C) for rho in range(min(s, k))]
         self.wp, self.wpT = e(D, C), e(C, D)
         G, taps = cfg.conv_pos_groups, cfg.conv_pos
-        self.pc_fwd, self.pc_dg = e(G, 64, taps, 64), e(G, 64, taps, 64)
+        Cgp = 64 if D // G <= 64 else 128   # padded group width of the pos_conv operands (b200s_posconv_prep)
+        self.pc_fwd, self.pc_dg = e(G, Cgp, taps, Cgp), e(G, Cgp, taps, Cgp)
         self.pc_norm2 = torch.zeros(2 * taps, dtype=torch.float32, device=device)   # holds fp64[taps] (deterministic tap norms)
         self.lw = []
         for lyr in m.encoder.layers:
@@ -599,7 +601,7 @@ class Engine:
         dpre = torch.zeros(B, Tpad, D, dtype=BF, device=dev)
         ops.dgelu_mul(dxs, T * D, D, st["pre"], T * D, D, dpre[:, half:], Tpad * D, D, T, B, D, self.g(pc.bias),
                       pre_is_grad=True)
-        dwp = torch.zeros(G, Cg, taps, 64, dtype=torch.float32, device=dev)
+        dwp = torch.zeros(G, Cg, taps, self.pc_fwd.shape[1], dtype=torch.float32, device=dev)
         ops.posconv_wgrad(dpre[:, half:], Tpad * D, D, xpad, Tpad * D, T, B, D, G, taps, dwp)
         work = torch.empty(4 * taps, dtype=torch.float32, device=dev)   # fp64[2 * taps]
         ops.posconv_unprep(pc.weight_v, pc.weight_g, dwp, D, G, taps, work, self.g(pc.weight_v), self.g(pc.weight_g))
@@ -652,10 +654,10 @@ class Engine:
         dmask = None
         if p_a > 0:  # dropout on the probabilities (WavLM/modules.py:551); the kernel leaves the keep bits for the backward
             dmask = torch.empty(ops.attn_dropout_mask_words(B, T, H), dtype=torch.int32, device=dev)
-            ops.attn_fwd_dropout(qkv, gate, tab, pad_u8, ao, lse, B, T, H, 64 ** -0.5, p_a,
-                                 d.key(DR.layer_site(idx, DR.L_ATTENTION)), dmask)
+            ops.attn_fwd_dropout(qkv, gate, tab, pad_u8, ao, lse, B, T, H, self.head_dim ** -0.5, p_a,
+                                 d.key(DR.layer_site(idx, DR.L_ATTENTION)), dmask, head_dim=self.head_dim)
         else:
-            ops.attn_fwd(qkv, gate, tab, pad_u8, ao, lse, B, T, H, 64 ** -0.5)
+            ops.attn_fwd(qkv, gate, tab, pad_u8, ao, lse, B, T, H, self.head_dim ** -0.5, head_dim=self.head_dim)
         y1 = e(B, T, D)
         if p_h > 0:  # x + dropout1(out_proj(attn)), WavLM/WavLM.py:702-703,726-727
             self._mm(ao, D, w["o"], D, y1, rag, T, B, bias=a.out_proj.bias)
@@ -782,10 +784,11 @@ class Engine:
             self._dq_acc_key = key
         if p_a > 0:
             ops.attn_bwd_fused_dropout(st["qkv"], st["ao"], dao, gate, tab, pad, st["lse"], delta, self._dq_acc, dqkv, dgate,
-                                       dtab if tab is not None else None, B, T, H, 64 ** -0.5, p_a, st["dmask"])
+                                       dtab if tab is not None else None, B, T, H, self.head_dim ** -0.5, p_a, st["dmask"],
+                                       head_dim=self.head_dim)
         else:
             ops.attn_bwd_fused(st["qkv"], st["ao"], dao, gate, tab, pad, st["lse"], delta, self._dq_acc, dqkv, dgate,
-                               dtab if tab is not None else None, B, T, H, 64 ** -0.5)
+                               dtab if tab is not None else None, B, T, H, self.head_dim ** -0.5, head_dim=self.head_dim)
         ops.colsum(dqkv, T * 3 * D, 3 * D, T, B, 3 * D, g(a.q_proj.bias).view(-1), valid=rag)  # q,k,v bias grads are adjacent in the flat buffer
         attn_in = st["xn"] if pre_ln else x
         dxg = None

@@ -242,21 +242,22 @@ def posconv_unprep(weight_v, weight_g, dwp, D, G, taps, work, dweight_v, dweight
 
 
 # ------------------------------------------------------------------------------------------------- attention
-def attn_fwd(qkv, gate, tab, key_pad, out, lse, B, T, H, scale):
+# head_dim: 64, or 80 without the relative-position bias (gate / tab None); D = H * head_dim.  Other values are an error.
+def attn_fwd(qkv, gate, tab, key_pad, out, lse, B, T, H, scale, head_dim=64):
     _call("b200s_attn_fwd", L.ptr(qkv), L.ptr(gate), L.ptr(tab), L.ptr(key_pad), L.ptr(out), L.ptr(lse), i32(B), i32(T),
-           i32(H), f32(scale), _s(), flops=4.0 * B * H * T * T * 64)
+           i32(H), f32(scale), i32(head_dim), _s(), flops=4.0 * B * H * T * T * head_dim)
 
 
-def attn_bwd(qkv, out, dout, gate, tab, key_pad, lse, delta, dqkv, dgate, dtab, B, T, H, scale):
+def attn_bwd(qkv, out, dout, gate, tab, key_pad, lse, delta, dqkv, dgate, dtab, B, T, H, scale, head_dim=64):
     _call("b200s_attn_bwd", L.ptr(qkv), L.ptr(out), L.ptr(dout), L.ptr(gate), L.ptr(tab), L.ptr(key_pad), L.ptr(lse),
-           L.ptr(delta), L.ptr(dqkv), L.ptr(dgate), L.ptr(dtab), i32(B), i32(T), i32(H), f32(scale), _s(),
-          flops=10.0 * B * H * T * T * 64)
+           L.ptr(delta), L.ptr(dqkv), L.ptr(dgate), L.ptr(dtab), i32(B), i32(T), i32(H), f32(scale), i32(head_dim), _s(),
+          flops=10.0 * B * H * T * T * head_dim)
 
 
-def attn_bwd_fused(qkv, out, dout, gate, tab, key_pad, lse, delta, dq_acc, dqkv, dgate, dtab, B, T, H, scale):
+def attn_bwd_fused(qkv, out, dout, gate, tab, key_pad, lse, delta, dq_acc, dqkv, dgate, dtab, B, T, H, scale, head_dim=64):
     _call("b200s_attn_bwd_fused", L.ptr(qkv), L.ptr(out), L.ptr(dout), L.ptr(gate), L.ptr(tab), L.ptr(key_pad), L.ptr(lse),
-           L.ptr(delta), L.ptr(dq_acc), L.ptr(dqkv), L.ptr(dgate), L.ptr(dtab), i32(B), i32(T), i32(H), f32(scale), _s(),
-          flops=10.0 * B * H * T * T * 64)
+           L.ptr(delta), L.ptr(dq_acc), L.ptr(dqkv), L.ptr(dgate), L.ptr(dtab), i32(B), i32(T), i32(H), f32(scale),
+           i32(head_dim), _s(), flops=10.0 * B * H * T * T * head_dim)
 
 
 # ------------------------------------------------------------------------------------------------- dropout
@@ -291,16 +292,17 @@ def attn_dropout_mask_words(B, T, H) -> int:
     return B * H * (4 * n) * (128 * n)
 
 
-def attn_fwd_dropout(qkv, gate, tab, key_pad, out, lse, B, T, H, scale, p, key, drop_mask):
+def attn_fwd_dropout(qkv, gate, tab, key_pad, out, lse, B, T, H, scale, p, key, drop_mask, head_dim=64):
     _call("b200s_attn_fwd_dropout", L.ptr(qkv), L.ptr(gate), L.ptr(tab), L.ptr(key_pad), L.ptr(out), L.ptr(lse), i32(B), i32(T),
-           i32(H), f32(scale), f32(p), u32(key[0]), u32(key[1]), L.ptr(drop_mask), _s(), flops=4.0 * B * H * T * T * 64)
+           i32(H), f32(scale), f32(p), u32(key[0]), u32(key[1]), L.ptr(drop_mask), i32(head_dim), _s(),
+           flops=4.0 * B * H * T * T * head_dim)
 
 
 def attn_bwd_fused_dropout(qkv, out, dout, gate, tab, key_pad, lse, delta, dq_acc, dqkv, dgate, dtab, B, T, H, scale, p,
-                           drop_mask):
+                           drop_mask, head_dim=64):
     _call("b200s_attn_bwd_fused_dropout", L.ptr(qkv), L.ptr(out), L.ptr(dout), L.ptr(gate), L.ptr(tab), L.ptr(key_pad),
            L.ptr(lse), L.ptr(delta), L.ptr(dq_acc), L.ptr(dqkv), L.ptr(dgate), L.ptr(dtab), i32(B), i32(T), i32(H), f32(scale),
-           f32(p), L.ptr(drop_mask), _s(), flops=10.0 * B * H * T * T * 64)
+           f32(p), L.ptr(drop_mask), i32(head_dim), _s(), flops=10.0 * B * H * T * T * head_dim)
 
 
 # ------------------------------------------------------------------------------------------------- optimizer

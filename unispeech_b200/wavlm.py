@@ -77,6 +77,14 @@ def _check_supported(cfg):
         bad.append("activation_fn != gelu")
     if eval(cfg.conv_feature_layers)[-1][0] == cfg.encoder_embed_dim:
         bad.append("conv feature width == encoder_embed_dim (the reference then has no post_extract_proj; the projection kernels assume one)")
+    D, H = cfg.encoder_embed_dim, cfg.encoder_attention_heads
+    head_dim = D // H if D % H == 0 else None
+    if head_dim not in (64, 80):
+        bad.append(f"attention head width {D}/{H} (the attention kernels take head widths 64 and 80)")
+    elif cfg.relative_position_embedding and head_dim != 64:
+        bad.append(f"relative_position_embedding at head width {head_dim} (the gated relative-position bias needs head width 64)")
+    if D % cfg.conv_pos_groups != 0 or D // cfg.conv_pos_groups > 128:
+        bad.append(f"pos_conv groups of {D}/{cfg.conv_pos_groups} channels (the pos_conv kernels take at most 128 channels per group)")
     return bad
 
 

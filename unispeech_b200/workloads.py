@@ -26,6 +26,11 @@ _MODELS: Dict[str, Tuple[dict, int, int]] = {
     "base": (dict(), 16, 15),
     "large": (dict(extractor_mode="layer_norm", encoder_layers=24, encoder_embed_dim=1024, encoder_ffn_embed_dim=4096,
                    encoder_attention_heads=16, layer_norm_first=True, normalize=True), 8, 20),
+    # XLS-R 1B / MMS-1B (HuBERT X-Large has the same encoder shape): head width 80, pos_conv groups of 80 channels, no
+    # relative-position bias, conv biases in the extractor
+    "xlsr1b": (dict(extractor_mode="layer_norm", encoder_layers=48, encoder_embed_dim=1280, encoder_ffn_embed_dim=5120,
+                    encoder_attention_heads=16, layer_norm_first=True, normalize=True, conv_bias=True,
+                    relative_position_embedding=False, gru_rel_pos=False), 8, 20),
     "tiny": (dict(encoder_layers=2, encoder_embed_dim=128, encoder_ffn_embed_dim=256, encoder_attention_heads=2,
                   conv_feature_layers="[(64,10,5)] + [(64,3,2)] * 4 + [(64,2,2)] * 2"), 4, 2),
 }
@@ -45,7 +50,7 @@ def num_frames(L: int, cfg: dict) -> int:
 
 def forward_flops(L: int, cfg: dict) -> float:
     """Algorithmic GEMM flops of one forward pass of one utterance of L samples (SURVEY.md section 8d):
-    sum_l 2 T_l 512 Cin_l k_l + 2 T 512 D + 2 T D (D/16) 128 + N (8 T D^2 + 4 T^2 D + 4 T D F + 2 T H 64 8); a step is 3x this."""
+    sum_l 2 T_l 512 Cin_l k_l + 2 T 512 D + 2 T D (D/16) 128 + N (8 T D^2 + 4 T^2 D + 4 T D F + 2 T H (D/H) 8); a step is 3x this."""
     D, Fd, H = cfg["encoder_embed_dim"], cfg["encoder_ffn_embed_dim"], cfg["encoder_attention_heads"]
     fl, cin, t = 0.0, 1, L
     for (dim, k, s) in eval(cfg["conv_feature_layers"]):
@@ -55,5 +60,5 @@ def forward_flops(L: int, cfg: dict) -> float:
     T = t
     fl += 2.0 * T * cin * D
     fl += 2.0 * T * D * (D // cfg["conv_pos_groups"]) * cfg["conv_pos"]
-    fl += cfg["encoder_layers"] * (8.0 * T * D * D + 4.0 * T * T * D + 4.0 * T * D * Fd + 2.0 * T * H * 64 * 8)
+    fl += cfg["encoder_layers"] * (8.0 * T * D * D + 4.0 * T * T * D + 4.0 * T * D * Fd + 2.0 * T * H * (D // H) * 8)
     return fl
