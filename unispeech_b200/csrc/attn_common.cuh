@@ -63,14 +63,4 @@ static inline long long attn_drop_mask_words(int B, int H, int T) {
   return static_cast<long long>(B) * H * (4 * n) * (kAttnTile * n);
 }
 
-// write 8 consecutive bf16 of row r, 16-byte chunk index `chunk` (0..15 over 128 columns) into a K-major SWIZZLE_128B tile
-// made of two [128 rows][64 cols] blocks (the layout of a K-major wgmma operand, and -- read as
-// MN-major -- for the transposed use).
-__device__ __forceinline__ void store_sw128_chunk(uint8_t* tile, int r, int chunk, uint4 v) {
-  const int kb = chunk >> 3;       // which 64-column block
-  const int c = chunk & 7;         // 16-byte chunk inside the 128-byte row
-  uint8_t* p = tile + kb * 16384 + r * 128 + ((c ^ (r & 7)) << 4);
-  *reinterpret_cast<uint4*>(p) = v;
-}
-
 }  // namespace b200

@@ -38,9 +38,8 @@ extern long long g_launch_count;
     B200_CHECK_CUDA(cudaGetLastError()); \
   } while (0)
 
-// Launch with programmatic dependent launch enabled (B200S_PDL=0 disables): the kernel's CTAs can be scheduled while the
-// previous kernel of the stream is still draining; every kernel calls pdl_wait() (ptx.cuh) before its first global access.
-bool pdl_enabled();
+// Launch with programmatic dependent launch enabled: the kernel's CTAs can be scheduled while the previous kernel of the
+// stream is still draining; every kernel calls pdl_wait() (ptx.cuh) before its first global access.
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
                                      Args&&... args) {
@@ -54,7 +53,7 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

@@ -1,11 +1,11 @@
 // First layer of ConvFeatureExtractionModel: Conv1d(1, C, k=10, stride=5, bias=conv_bias) on the raw waveform, fused with its
 // normalisation and GELU (WavLM/WavLM.py:400-426,485-504).  Cin = 1 makes this HBM-bound (20 flop per output element),
 // so it is a CUDA-core kernel: one warp per output frame, each lane owns C/32 channels, weights in shared memory,
-// channels-last bf16 output [B, Tpad, C].  The conv output is never stored: statistics passes and the backward
-// recompute it from the waveform (10 samples per frame).
-//   mode GN ("default" extractor, WavLM-Base): Fp32GroupNorm(C, C) = per-(b, channel) statistics over ALL frames
-//            -> pass 1 accumulates sum / sum-of-squares (fp64 atomics), pass 2 normalises + GELU.
-//   mode LN ("layer_norm" extractor, WavLM-Large): Fp32LayerNorm over channels per frame, single pass.
+// channels-last bf16 output [B, Tpad, C].  The conv output is never stored: the backward recomputes it from the waveform
+// (10 samples per frame).
+//   mode GN ("default" extractor, WavLM-Base): Fp32GroupNorm(C, C) = per-(b, channel) statistics over ALL frames; its kernels
+//            are in conv0_gn.cu, which derives the statistics from the waveform autocorrelation.
+//   mode LN ("layer_norm" extractor, WavLM-Large): Fp32LayerNorm over channels per frame, single pass (the kernels below).
 #include <algorithm>
 
 #include "../../include/unispeech_b200.h"
@@ -120,58 +120,11 @@ __device__ __forceinline__ void block_channel_atomic(const float* acc, T* dst, i
 }
 
 // ---------------------------------------------------------------------------------------------- forward kernels
-// GN pass 1: stats[b][c] = {sum, sumsq} over t (fp64 atomics)
+// LN over channels + GELU (writes per-frame mean / rstd)
 template <int C>
-__global__ void __launch_bounds__(256) conv0_gn_stats_kernel(const float* __restrict__ wav, long long L, int T, int k,
-                                                             int s, const float* __restrict__ w,
-                                                             double* __restrict__ stats) {
-  pdl_grid_sync();
-  using M = LaneMap<C>;
-  extern __shared__ float smem[];
-  float* w_s = smem;            // [k][C]
-  float* red = smem + kMaxTaps * C;  // [8][C]
-  load_weights<C>(w, k, w_s);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int b = blockIdx.y;
-  const float* wav_b = wav + static_cast<long long>(b) * L;
-  float s1[M::CPL], s2[M::CPL];
-#pragma unroll
-  for (int i = 0; i < M::CPL; ++i) s1[i] = s2[i] = 0.f;
-  for (int t = blockIdx.x * 8 + warp; t < T; t += gridDim.x * 8) {
-    float acc[M::CPL];
-    conv_frame<C>(wav_b, L, t, k, s, w_s, lane, acc, nullptr);
-#pragma unroll
-    for (int i = 0; i < M::CPL; ++i) {
-      s1[i] += acc[i];
-      s2[i] += acc[i] * acc[i];
-    }
-  }
-  block_channel_atomic<C, double>(s1, stats + static_cast<long long>(b) * C * 2, 2, red);
-  block_channel_atomic<C, double>(s2, stats + static_cast<long long>(b) * C * 2 + 1, 2, red);
-}
-
-template <int C>
-__device__ __forceinline__ void gn_mean_rstd(const double* __restrict__ stats_b, int T, int lane, float* mean,
-                                             float* rstd) {
-  using M = LaneMap<C>;
-#pragma unroll
-  for (int g = 0; g < M::NG; ++g)
-#pragma unroll
-    for (int v = 0; v < M::V; ++v) {
-      const int c = M::chan(lane, g, v);
-      const double m = stats_b[c * 2] / T;
-      const double var = stats_b[c * 2 + 1] / T - m * m;
-      mean[g * M::V + v] = static_cast<float>(m);
-      rstd[g * M::V + v] = static_cast<float>(1.0 / sqrt((var > 0 ? var : 0) + 1e-5));
-    }
-}
-
-// MODE 0: GN apply (needs stats);  MODE 1: LN over channels (writes per-frame mean / rstd)
-template <int C, int MODE>
 __global__ void __launch_bounds__(256) conv0_fwd_kernel(const float* __restrict__ wav, long long L, int T, int k, int s,
                                                         const float* __restrict__ w, const float* __restrict__ gamma,
-                                                        const float* __restrict__ beta,
-                                                        const double* __restrict__ stats, float* __restrict__ fmean,
+                                                        const float* __restrict__ beta, float* __restrict__ fmean,
                                                         float* __restrict__ frstd, __nv_bfloat16* __restrict__ out,
                                                         long long out_bs, const float* __restrict__ bias) {
   pdl_grid_sync();
@@ -182,7 +135,7 @@ __global__ void __launch_bounds__(256) conv0_fwd_kernel(const float* __restrict_
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int b = blockIdx.y;
   const float* wav_b = wav + static_cast<long long>(b) * L;
-  float g[M::CPL], be[M::CPL], mean[M::CPL], rstd[M::CPL];
+  float g[M::CPL], be[M::CPL];
 #pragma unroll
   for (int gi = 0; gi < M::NG; ++gi)
 #pragma unroll
@@ -190,99 +143,38 @@ __global__ void __launch_bounds__(256) conv0_fwd_kernel(const float* __restrict_
       g[gi * M::V + v] = gamma[M::chan(lane, gi, v)];
       be[gi * M::V + v] = beta[M::chan(lane, gi, v)];
     }
-  if (MODE == 0) gn_mean_rstd<C>(stats + static_cast<long long>(b) * C * 2, T, lane, mean, rstd);
   for (int t = blockIdx.x * 8 + warp; t < T; t += gridDim.x * 8) {
     float acc[M::CPL];
     conv_frame<C>(wav_b, L, t, k, s, w_s, lane, acc, nullptr);
-    if (MODE == 0) {
+    if (bias != nullptr) add_bias<C>(bias, lane, acc);
+    float su = 0.f;
 #pragma unroll
-      for (int i = 0; i < M::CPL; ++i) acc[i] = gelu_f((acc[i] - mean[i]) * rstd[i] * g[i] + be[i]);
-    } else {
-      if (bias != nullptr) add_bias<C>(bias, lane, acc);
-      float su = 0.f;
+    for (int i = 0; i < M::CPL; ++i) su += acc[i];
+    const float m = warp_sum(su) * (1.0f / C);
+    float q = 0.f;
 #pragma unroll
-      for (int i = 0; i < M::CPL; ++i) su += acc[i];
-      const float m = warp_sum(su) * (1.0f / C);
-      float q = 0.f;
+    for (int i = 0; i < M::CPL; ++i) {
+      const float d = acc[i] - m;
+      q += d * d;
+    }
+    const float r = rsqrtf(warp_sum(q) * (1.0f / C) + 1e-5f);
 #pragma unroll
-      for (int i = 0; i < M::CPL; ++i) {
-        const float d = acc[i] - m;
-        q += d * d;
-      }
-      const float r = rsqrtf(warp_sum(q) * (1.0f / C) + 1e-5f);
-#pragma unroll
-      for (int i = 0; i < M::CPL; ++i) acc[i] = gelu_f((acc[i] - m) * r * g[i] + be[i]);
-      if (lane == 0) {
-        fmean[static_cast<long long>(b) * T + t] = m;
-        frstd[static_cast<long long>(b) * T + t] = r;
-      }
+    for (int i = 0; i < M::CPL; ++i) acc[i] = gelu_f((acc[i] - m) * r * g[i] + be[i]);
+    if (lane == 0) {
+      fmean[static_cast<long long>(b) * T + t] = m;
+      frstd[static_cast<long long>(b) * T + t] = r;
     }
     store_frame<C>(out + b * out_bs + static_cast<long long>(t) * C, acc, lane);
   }
 }
 
 // ---------------------------------------------------------------------------------------------- backward kernels
-// GN backward pass A: per (b,c) S1 = sum_t dxhat, S2 = sum_t dxhat*xhat (float atomics into bstats[b][c][2]),
-// and dgamma[c] += sum dz*xhat, dbeta[c] += sum dz, where dz = da * gelu'(gamma*xhat+beta), dxhat = dz*gamma.
-template <int C>
-__global__ void __launch_bounds__(256) conv0_gn_bwd_stats_kernel(const float* __restrict__ wav, long long L, int T, int k,
-                                                                 int s, const float* __restrict__ w,
-                                                                 const float* __restrict__ gamma,
-                                                                 const float* __restrict__ beta,
-                                                                 const double* __restrict__ stats,
-                                                                 const __nv_bfloat16* __restrict__ da, long long da_bs,
-                                                                 float* __restrict__ bstats, float* __restrict__ dgamma,
-                                                                 float* __restrict__ dbeta) {
-  pdl_grid_sync();
-  using M = LaneMap<C>;
-  extern __shared__ float smem[];
-  float* w_s = smem;
-  float* red = smem + kMaxTaps * C;
-  load_weights<C>(w, k, w_s);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int b = blockIdx.y;
-  const float* wav_b = wav + static_cast<long long>(b) * L;
-  float g[M::CPL], be[M::CPL], mean[M::CPL], rstd[M::CPL], s1[M::CPL], s2[M::CPL], ag[M::CPL], ab[M::CPL];
-#pragma unroll
-  for (int gi = 0; gi < M::NG; ++gi)
-#pragma unroll
-    for (int v = 0; v < M::V; ++v) {
-      g[gi * M::V + v] = gamma[M::chan(lane, gi, v)];
-      be[gi * M::V + v] = beta[M::chan(lane, gi, v)];
-    }
-  gn_mean_rstd<C>(stats + static_cast<long long>(b) * C * 2, T, lane, mean, rstd);
-#pragma unroll
-  for (int i = 0; i < M::CPL; ++i) s1[i] = s2[i] = ag[i] = ab[i] = 0.f;
-  for (int t = blockIdx.x * 8 + warp; t < T; t += gridDim.x * 8) {
-    float acc[M::CPL], d[M::CPL];
-    conv_frame<C>(wav_b, L, t, k, s, w_s, lane, acc, nullptr);
-    load_frame<C>(da + b * da_bs + static_cast<long long>(t) * C, d, lane);
-#pragma unroll
-    for (int i = 0; i < M::CPL; ++i) {
-      const float xh = (acc[i] - mean[i]) * rstd[i];
-      const float dz = d[i] * gelu_grad_f(g[i] * xh + be[i]);
-      ag[i] += dz * xh;
-      ab[i] += dz;
-      const float dxh = dz * g[i];
-      s1[i] += dxh;
-      s2[i] += dxh * xh;
-    }
-  }
-  block_channel_atomic<C, float>(s1, bstats + static_cast<long long>(b) * C * 2, 2, red);
-  block_channel_atomic<C, float>(s2, bstats + static_cast<long long>(b) * C * 2 + 1, 2, red);
-  block_channel_atomic<C, float>(ag, dgamma, 1, red);
-  block_channel_atomic<C, float>(ab, dbeta, 1, red);
-}
-
-// weight gradient for taps [j0, j0+JT):  dW[c, j] += sum_{b,t} dconv[b,t,c] * wav[b, s*t + j]
-// MODE 0 (GN): dconv = rstd_bc * (dxhat - S1/T - xhat*S2/T);   MODE 1 (LN): per-frame statistics, also accumulates
-// dgamma/dbeta when j0 == 0.
-template <int C, int MODE, int JT>
+// LN-mode weight gradient for taps [j0, j0+JT):  dW[c, j] += sum_{b,t} dconv[b,t,c] * wav[b, s*t + j], with dconv from the
+// per-frame statistics; also accumulates dgamma / dbeta (and dbias) when j0 == 0.
+template <int C, int JT>
 __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restrict__ wav, long long L, int T, int k, int s,
                                                            const float* __restrict__ w, const float* __restrict__ gamma,
                                                            const float* __restrict__ beta,
-                                                           const double* __restrict__ stats,
-                                                           const float* __restrict__ bstats,
                                                            const float* __restrict__ fmean, const float* __restrict__ frstd,
                                                            const __nv_bfloat16* __restrict__ da, long long da_bs, int j0,
                                                            float* __restrict__ dw, float* __restrict__ dgamma,
@@ -297,7 +189,7 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int b = blockIdx.y;
   const float* wav_b = wav + static_cast<long long>(b) * L;
-  float g[M::CPL], be[M::CPL], mean[M::CPL], rstd[M::CPL], m1[M::CPL], m2[M::CPL];
+  float g[M::CPL], be[M::CPL];
   float ag[M::CPL], ab[M::CPL], adb[M::CPL];
   float acc_dw[JT][M::CPL];
 #pragma unroll
@@ -307,12 +199,7 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
       const int c = M::chan(lane, gi, v);
       g[gi * M::V + v] = gamma[c];
       be[gi * M::V + v] = beta[c];
-      if (MODE == 0) {
-        m1[gi * M::V + v] = bstats[(static_cast<long long>(b) * C + c) * 2] / T;
-        m2[gi * M::V + v] = bstats[(static_cast<long long>(b) * C + c) * 2 + 1] / T;
-      }
     }
-  if (MODE == 0) gn_mean_rstd<C>(stats + static_cast<long long>(b) * C * 2, T, lane, mean, rstd);
 #pragma unroll
   for (int i = 0; i < M::CPL; ++i) {
     ag[i] = ab[i] = adb[i] = 0.f;
@@ -323,36 +210,27 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
     float acc[M::CPL], d[M::CPL], win[kMaxTaps];
     conv_frame<C>(wav_b, L, t, k, s, w_s, lane, acc, win);
     load_frame<C>(da + b * da_bs + static_cast<long long>(t) * C, d, lane);
-    if (MODE == 0) {
+    if (bias != nullptr) add_bias<C>(bias, lane, acc);
+    const float m = fmean[static_cast<long long>(b) * T + t], r = frstd[static_cast<long long>(b) * T + t];
+    float q1 = 0.f, q2 = 0.f;
 #pragma unroll
-      for (int i = 0; i < M::CPL; ++i) {
-        const float xh = (acc[i] - mean[i]) * rstd[i];
-        const float dxh = d[i] * gelu_grad_f(g[i] * xh + be[i]) * g[i];
-        d[i] = rstd[i] * (dxh - m1[i] - xh * m2[i]);
-      }
-    } else {
-      if (bias != nullptr) add_bias<C>(bias, lane, acc);
-      const float m = fmean[static_cast<long long>(b) * T + t], r = frstd[static_cast<long long>(b) * T + t];
-      float q1 = 0.f, q2 = 0.f;
+    for (int i = 0; i < M::CPL; ++i) {
+      const float xh = (acc[i] - m) * r;
+      const float dz = d[i] * gelu_grad_f(g[i] * xh + be[i]);
+      ag[i] += dz * xh;
+      ab[i] += dz;
+      const float dxh = dz * g[i];
+      acc[i] = xh;
+      d[i] = dxh;
+      q1 += dxh;
+      q2 += dxh * xh;
+    }
+    q1 = warp_sum(q1) * (1.0f / C);
+    q2 = warp_sum(q2) * (1.0f / C);
 #pragma unroll
-      for (int i = 0; i < M::CPL; ++i) {
-        const float xh = (acc[i] - m) * r;
-        const float dz = d[i] * gelu_grad_f(g[i] * xh + be[i]);
-        ag[i] += dz * xh;
-        ab[i] += dz;
-        const float dxh = dz * g[i];
-        acc[i] = xh;
-        d[i] = dxh;
-        q1 += dxh;
-        q2 += dxh * xh;
-      }
-      q1 = warp_sum(q1) * (1.0f / C);
-      q2 = warp_sum(q2) * (1.0f / C);
-#pragma unroll
-      for (int i = 0; i < M::CPL; ++i) {
-        d[i] = r * (d[i] - q1 - acc[i] * q2);
-        adb[i] += d[i];  // d bias: the tap whose input is 1
-      }
+    for (int i = 0; i < M::CPL; ++i) {
+      d[i] = r * (d[i] - q1 - acc[i] * q2);
+      adb[i] += d[i];  // d bias: the tap whose input is 1
     }
 #pragma unroll
     for (int j = 0; j < JT; ++j) {
@@ -364,7 +242,7 @@ __global__ void __launch_bounds__(256) conv0_bwd_dw_kernel(const float* __restri
 #pragma unroll
   for (int j = 0; j < JT; ++j)
     if (j0 + j < k) block_channel_atomic<C, float>(acc_dw[j], dw + (j0 + j), k, red);  // dw layout [C, 1, k]
-  if (MODE == 1 && j0 == 0) {
+  if (j0 == 0) {
     block_channel_atomic<C, float>(ag, dgamma, 1, red);
     block_channel_atomic<C, float>(ab, dbeta, 1, red);
     if (dbias != nullptr) block_channel_atomic<C, float>(adb, dbias, 1, red);
@@ -517,17 +395,15 @@ int b200s_conv0_fwd(const float* wav, long long L, int B, int T, int C, int k, i
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   dim3 grid(conv0_grid_x(T), B);
   DISPATCH_C(C, {
-    const size_t sm_w = sizeof(float) * kMaxTaps * kC, sm_red = sizeof(float) * 8 * kC;
+    const size_t sm_w = sizeof(float) * kMaxTaps * kC;
     if (mode == 0) {
       // GroupNorm(C, C) normalises every (utterance, channel) over all its frames: a per-channel constant shifts that mean by
       // bias[c] and leaves the variance unchanged, so the bias cancels exactly -- it is not applied (and gets no gradient)
-      (void)sm_red;
-      (void)bias;
       if (int rc = conv0_gn_stats_launch(wav, L, B, T, kC, k, s, w, stats, st)) return rc;  // analytic, from the autocorrelation
       return conv0_gn_fwd_apply_launch(wav, L, B, T, kC, k, s, w, gamma, beta, stats, out, out_bs, st);
     } else {
-      B200_CHECK_CUDA(launch_pdl(conv0_fwd_kernel<kC, 1>, dim3(grid), dim3(256), sm_w, st, wav, L, T, k, s, w, gamma, beta, nullptr, fmean, frstd,
-                                                      static_cast<__nv_bfloat16*>(out), out_bs, bias));
+      B200_CHECK_CUDA(launch_pdl(conv0_fwd_kernel<kC>, dim3(grid), dim3(256), sm_w, st, wav, L, T, k, s, w, gamma, beta, fmean, frstd,
+                                 static_cast<__nv_bfloat16*>(out), out_bs, bias));
     }
     B200_CHECK_LAUNCH();
   })
@@ -554,7 +430,6 @@ int b200s_conv0_bwd_ws(const float* wav, long long L, int B, int T, int C, int k
     constexpr int JT = 5;
     if (mode == 0) {
       // (GroupNorm mode: the bias cancels in the forward pass, its gradient is exactly zero -- dbias is left untouched)
-      (void)grid;
       if (int rc = conv0_gn_bwd_launch(wav, L, B, T, kC, k, s, w, gamma, beta, stats, bstats, da, da_bs, dw, dgamma, dbeta, st))
         return rc;
     } else if (dconv_ws != nullptr && k <= 10) {
@@ -568,11 +443,11 @@ int b200s_conv0_bwd_ws(const float* wav, long long L, int B, int T, int C, int k
                                  static_cast<const __nv_bfloat16*>(dconv_ws), ws_bs, dw, dbias));
       B200_CHECK_LAUNCH();
     } else {
-      B200_CHECK_CUDA(cudaFuncSetAttribute(conv0_bwd_dw_kernel<kC, 1, JT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      B200_CHECK_CUDA(cudaFuncSetAttribute(conv0_bwd_dw_kernel<kC, JT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            static_cast<int>(sm)));
       for (int j0 = 0; j0 < k; j0 += JT) {
-        B200_CHECK_CUDA(launch_pdl(conv0_bwd_dw_kernel<kC, 1, JT>, dim3(grid), dim3(256), sm, st, wav, L, T, k, s, w, gamma, beta, nullptr, nullptr, fmean,
-                                                             frstd, dap, da_bs, j0, dw, dgamma, dbeta, bias, dbias));
+        B200_CHECK_CUDA(launch_pdl(conv0_bwd_dw_kernel<kC, JT>, dim3(grid), dim3(256), sm, st, wav, L, T, k, s, w, gamma, beta, fmean,
+                                   frstd, dap, da_bs, j0, dw, dgamma, dbeta, bias, dbias));
         B200_CHECK_LAUNCH();
       }
     }

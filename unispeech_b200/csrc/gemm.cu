@@ -1,6 +1,5 @@
 // Host side of the wgmma GEMM family: TMA tensor-map construction, tile mapping and launch.
 #include <stdarg.h>
-#include <stdlib.h>
 
 #include <algorithm>
 #include <mutex>
@@ -20,14 +19,6 @@ void set_last_error(const char* fmt, ...) {
   va_start(ap, fmt);
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
-}
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200S_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
 }
 int sm_count() {
   static int n = 0;
@@ -64,8 +55,8 @@ struct ViewSpec {
   int box[4];
 };
 
-// bf16, zero OOB fill; 128B swizzle, or 32B for a box of 16 columns (the last 16 columns of an 80-wide attention head).
-// Returns 0 on success.
+// bf16, zero OOB fill, 256-byte L2 promotion; 128B swizzle, or 32B for a box of 16 columns (the last 16 columns of an 80-wide
+// attention head).  Returns 0 on success.
 static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
@@ -93,16 +84,9 @@ static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
     set_last_error("tensor map base pointer %p is not 16-byte aligned", v.ptr);
     return -1;
   }
-  static int promo = -1;  // L2 promotion of the TMA loads: 256 B by default, B200S_TMAP_L2PROMO=0..3 (none/64/128/256) for A/B runs
-  if (promo < 0) {
-    const char* e = getenv("B200S_TMAP_L2PROMO");
-    promo = (e && e[0] >= '0' && e[0] <= '3') ? (e[0] - '0') : 3;
-  }
-  static const CUtensorMapL2promotion kPromo[4] = {CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_64B,
-                                                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(v.ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, v.box[0] == 16 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-                  kPromo[promo], CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled failed (%d): dims {%lld,%lld,%lld,%lld} strides {%lld,%lld,%lld} box {%d,%d,%d,%d}",
                    static_cast<int>(r), v.dims[0], v.dims[1], v.dims[2], v.dims[3], v.strides[0], v.strides[1],

@@ -85,20 +85,6 @@ __device__ __forceinline__ bool named_bar_any(int id, int count, bool pred) {
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
 }
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-          smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
                                             int c3) {
   asm volatile(
@@ -108,14 +94,6 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// TMA store of one shared-memory box (bulk async-group completion); coordinates beyond the tensor bounds are clipped
-// (the library's tensor maps are all rank 4: the coordinate count must match the map)
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
 // TMA element-wise fp32 add of one shared-memory box into global memory (bulk async-group completion; the data type comes
 // from the rank-3 tensor map); coordinates beyond the tensor bounds are clipped
 __device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2) {
@@ -269,7 +247,7 @@ __device__ __forceinline__ void setmaxnreg_inc() {
 
 // Accumulator fragment of a 64 x N wgmma (thread t of the warpgroup, warp w = t / 32, lane l):
 //   d[i] is row 16 w + l / 4 + 8 ((i / 2) & 1), column 8 (i / 4) + 2 (l & 3) + (i & 1).
-// Rows [row0, row0 + 64) of a row-major fp32 shared-memory tile (pitch in floats, even) <-> the fragment.
+// The fragment -> rows [row0, row0 + 64) of a row-major fp32 shared-memory tile (pitch in floats, even).
 template <int N>
 __device__ __forceinline__ void acc_to_smem(const float* d, float* tile, int pitch, int row0) {
   const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
@@ -277,17 +255,6 @@ __device__ __forceinline__ void acc_to_smem(const float* d, float* tile, int pit
 #pragma unroll
   for (int i = 0; i < N / 2; i += 2)
     *reinterpret_cast<float2*>(base + 8 * ((i >> 1) & 1) * pitch + 8 * (i >> 2)) = make_float2(d[i], d[i + 1]);
-}
-template <int N>
-__device__ __forceinline__ void smem_to_acc(float* d, const float* tile, int pitch, int row0) {
-  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
-  const float* base = tile + (row0 + 16 * w + (l >> 2)) * pitch + 2 * (l & 3);
-#pragma unroll
-  for (int i = 0; i < N / 2; i += 2) {
-    const float2 v = *reinterpret_cast<const float2*>(base + 8 * ((i >> 1) & 1) * pitch + 8 * (i >> 2));
-    d[i] = v.x;
-    d[i + 1] = v.y;
-  }
 }
 
 // ---------------------------------------------------------------- misc math / packing
@@ -400,43 +367,6 @@ __device__ __forceinline__ float warp_colsum32(const float (&v)[32], int lane) {
   const float send = up ? d[0] : d[1];
   const float keep = up ? d[1] : d[0];
   return keep + __shfl_xor_sync(0xffffffffu, send, 1);
-}
-
-// Same for a 16-column register tile: 16 shuffles; on return lanes 2c and 2c+1 both hold the sum of column c.
-__device__ __forceinline__ float warp_colsum16(const float (&v)[16], int lane) {
-  float a[8], b[4], c[2];
-  {
-    const bool up = (lane & 16) != 0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float send = up ? v[i] : v[i + 8];
-      const float keep = up ? v[i + 8] : v[i];
-      a[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-    }
-  }
-  {
-    const bool up = (lane & 8) != 0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float send = up ? a[i] : a[i + 4];
-      const float keep = up ? a[i + 4] : a[i];
-      b[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-    }
-  }
-  {
-    const bool up = (lane & 4) != 0;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const float send = up ? b[i] : b[i + 2];
-      const float keep = up ? b[i + 2] : b[i];
-      c[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-    }
-  }
-  const bool up = (lane & 2) != 0;
-  const float send = up ? c[0] : c[1];
-  const float keep = up ? c[1] : c[0];
-  const float d = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-  return d + __shfl_xor_sync(0xffffffffu, d, 1);
 }
 
 }  // namespace b200

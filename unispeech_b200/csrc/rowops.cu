@@ -220,11 +220,11 @@ __global__ void __launch_bounds__(256, 4) ln_fwd_kernel(const __nv_bfloat16* __r
   }
 }
 
-// Wide rows (D = 256 * NW: 512 / 768 / 1024): the row is spread over the NW warps of the block, one 16-byte vector per thread, R rows
-// per iteration with all their loads issued up front; mean and variance (two-pass, as above) cross the warps through shared
-// memory with one block barrier each.  The gate of a head is an 8-lane affair exactly as in the warp-per-row kernel, but all
-// heads of a row are evaluated in parallel (thread t owns columns 8t..8t+7 = head t / 8).
-template <int NW, int R, bool GATE, bool GELU>
+// Gate-fused forward at wide rows (D = 256 * NW: 512 / 768 / 1024): the row is spread over the NW warps of the block, one
+// 16-byte vector per thread, R rows per iteration with all their loads issued up front; mean and variance (two-pass, as above)
+// cross the warps through shared memory with one block barrier each.  The gate of a head is an 8-lane affair exactly as in the
+// warp-per-row kernel, but all heads of a row are evaluated in parallel (thread t owns columns 8t..8t+7 = head t / 8).
+template <int NW, int R>
 __global__ void __launch_bounds__(32 * NW) ln_fwd_wide_kernel(const __nv_bfloat16* __restrict__ x, RowView xv,
                                                              const float* __restrict__ gamma, const float* __restrict__ beta,
                                                              __nv_bfloat16* __restrict__ y, RowView yv,
@@ -242,18 +242,16 @@ __global__ void __launch_bounds__(32 * NW) ln_fwd_wide_kernel(const __nv_bfloat1
     g[j] = gamma[c0 + j];
     b[j] = beta[c0 + j];
   }
-  float wa[GATE ? 8 : 1], wb[GATE ? 8 : 1], gba = 0.f, gbb = 0.f, a_h = 0.f;
-  if constexpr (GATE) {
+  float wa[8], wb[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int c = (lane & 7) * 8 + j;
-      wa[j] = ga.grep_w[c] + ga.grep_w[64 + c] + ga.grep_w[128 + c] + ga.grep_w[192 + c];
-      wb[j] = ga.grep_w[256 + c] + ga.grep_w[320 + c] + ga.grep_w[384 + c] + ga.grep_w[448 + c];
-    }
-    gba = ga.grep_b[0] + ga.grep_b[1] + ga.grep_b[2] + ga.grep_b[3];
-    gbb = ga.grep_b[4] + ga.grep_b[5] + ga.grep_b[6] + ga.grep_b[7];
-    a_h = ga.grep_a[threadIdx.x >> 3];
+  for (int j = 0; j < 8; ++j) {
+    const int c = (lane & 7) * 8 + j;
+    wa[j] = ga.grep_w[c] + ga.grep_w[64 + c] + ga.grep_w[128 + c] + ga.grep_w[192 + c];
+    wb[j] = ga.grep_w[256 + c] + ga.grep_w[320 + c] + ga.grep_w[384 + c] + ga.grep_w[448 + c];
   }
+  const float gba = ga.grep_b[0] + ga.grep_b[1] + ga.grep_b[2] + ga.grep_b[3];
+  const float gbb = ga.grep_b[4] + ga.grep_b[5] + ga.grep_b[6] + ga.grep_b[7];
+  const float a_h = ga.grep_a[threadIdx.x >> 3];
   __shared__ float red[2][NW][R];
   for (long long r0 = static_cast<long long>(blockIdx.x) * R; r0 < rows; r0 += static_cast<long long>(gridDim.x) * R) {
     uint4 raw[R];
@@ -319,12 +317,8 @@ __global__ void __launch_bounds__(32 * NW) ln_fwd_wide_kernel(const __nv_bfloat1
       uint32_t ou[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        float o0 = (v[i][2 * k] - mean[i]) * rstd[i] * g[2 * k] + b[2 * k];
-        float o1 = (v[i][2 * k + 1] - mean[i]) * rstd[i] * g[2 * k + 1] + b[2 * k + 1];
-        if (GELU) {
-          o0 = gelu_f(o0);
-          o1 = gelu_f(o1);
-        }
+        const float o0 = (v[i][2 * k] - mean[i]) * rstd[i] * g[2 * k] + b[2 * k];
+        const float o1 = (v[i][2 * k + 1] - mean[i]) * rstd[i] * g[2 * k + 1] + b[2 * k + 1];
         ou[k] = dead[i] ? 0u : pack_bf16x2(o0, o1);
       }
       if (r < rows) {
@@ -334,38 +328,36 @@ __global__ void __launch_bounds__(32 * NW) ln_fwd_wide_kernel(const __nv_bfloat1
           if (rstd_out) rstd_out[r] = dead[i] ? 0.f : rstd[i];
         }
       }
-      if constexpr (GATE) {
-        float sa = 0.f, sb = 0.f;
+      float sa = 0.f, sb = 0.f;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float2 yb = unpack_bf16x2(ou[k]);  // what the attention kernel will read
-          sa = fmaf(yb.x, wa[2 * k], sa);
-          sa = fmaf(yb.y, wa[2 * k + 1], sa);
-          sb = fmaf(yb.x, wb[2 * k], sb);
-          sb = fmaf(yb.y, wb[2 * k + 1], sb);
-        }
+      for (int k = 0; k < 4; ++k) {
+        const float2 yb = unpack_bf16x2(ou[k]);  // what the attention kernel will read
+        sa = fmaf(yb.x, wa[2 * k], sa);
+        sa = fmaf(yb.y, wa[2 * k + 1], sa);
+        sb = fmaf(yb.x, wb[2 * k], sb);
+        sb = fmaf(yb.y, wb[2 * k + 1], sb);
+      }
 #pragma unroll
-        for (int o = 1; o < 8; o <<= 1) {
-          sa += __shfl_xor_sync(0xffffffffu, sa, o);
-          sb += __shfl_xor_sync(0xffffffffu, sb, o);
-        }
-        if ((lane & 7) == 0 && r < rows) {
-          const long long bidx = rb[i], t = rt[i];  // (the gate variant's views have T rows per batch)
-          const float g1 = 1.0f / (1.0f + __expf(-(sa + gba)));
-          const float g2 = 1.0f / (1.0f + __expf(-(sb + gbb)));
-          ga.gate[(bidx * ga.H + (threadIdx.x >> 3)) * ga.T + t] = dead[i] ? 1.0f : g1 * (g2 * a_h - 1.0f) + 2.0f;
-        }
+      for (int o = 1; o < 8; o <<= 1) {
+        sa += __shfl_xor_sync(0xffffffffu, sa, o);
+        sb += __shfl_xor_sync(0xffffffffu, sb, o);
+      }
+      if ((lane & 7) == 0 && r < rows) {
+        const long long bidx = rb[i], t = rt[i];  // (the views have T rows per batch)
+        const float g1 = 1.0f / (1.0f + __expf(-(sa + gba)));
+        const float g2 = 1.0f / (1.0f + __expf(-(sb + gbb)));
+        ga.gate[(bidx * ga.H + (threadIdx.x >> 3)) * ga.T + t] = dead[i] ? 1.0f : g1 * (g2 * a_h - 1.0f) + 2.0f;
       }
     }
   }
 }
 
-template <bool GATE, bool GELU, typename... Args>
+template <typename... Args>
 static int launch_ln_fwd_wide(int D, long long rows, cudaStream_t st, Args... args) {
   constexpr int R = 4;
   auto go = [&](auto nw) {
     constexpr int NW = decltype(nw)::value;
-    auto kern = ln_fwd_wide_kernel<NW, R, GATE, GELU>;
+    auto kern = ln_fwd_wide_kernel<NW, R>;
     static const int cap = resident_grid(kern, 32 * NW);
     const int grid = static_cast<int>(std::min<long long>(ceil_div_ll(rows, R), cap));
     B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(32 * NW), 0, st, args...));
@@ -588,159 +580,6 @@ __global__ void __launch_bounds__(256, 2) ln_bwd_kernel(const __nv_bfloat16* __r
   }
 }
 
-// Wide rows (D = 256 * NW, NW = 2..4: the encoder widths 512 / 768 / 1024): a row is spread over the NW warps of the block, one
-// 16-byte vector per thread, and the block walks R rows per iteration.  A thread owns 8 COLUMNS for the whole kernel, so the
-// parameter-gradient partials (d gamma, d beta, column sums of dx) are 24 registers instead of a shared-memory read-modify-write
-// per row and element (the warp-per-row kernel above moved 16 KB through shared memory per 6 KB row and ran at 20 % of the HBM
-// peak); the two row sums cross the warps through one double-buffered shared exchange and ONE block barrier per R rows.  All
-// loads of the R rows (dy, x, dres, statistics) are issued before the first use.  Across the barrier a row is kept as the RAW
-// packed vectors (12 registers) and x-hat / d x-hat are re-derived afterwards (two FMAs) -- except in the GELU variant, whose
-// derivative is too expensive to evaluate twice.
-template <int NW, int R, bool GELU>
-__global__ void __launch_bounds__(32 * NW, 16 / NW) ln_bwd_wide_kernel(const __nv_bfloat16* __restrict__ dy, RowView dyv,
-                                                             const __nv_bfloat16* __restrict__ x, RowView xv,
-                                                             const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
-                                                             const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                             const __nv_bfloat16* __restrict__ dres, RowView dresv,
-                                                             __nv_bfloat16* __restrict__ dx, RowView dxv,
-                                                             float* __restrict__ dgamma, float* __restrict__ dbeta,
-                                                             float* __restrict__ colsum, long long rows, int vec_atomics) {
-  pdl_grid_sync();
-  constexpr int D = 256 * NW;
-  const int lane = threadIdx.x & 31;
-  const int warp = threadIdx.x >> 5;
-  const int c0 = threadIdx.x * 8;
-  float g[8], bt[GELU ? 8 : 1];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    g[j] = gamma[c0 + j];
-    if (GELU) bt[j] = beta[c0 + j];
-  }
-  float ag[8], ab[8], ac[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) ag[j] = ab[j] = ac[j] = 0.f;
-  __shared__ float red[2][NW][2 * R];
-  const bool want_c = colsum != nullptr;
-  int it = 0;
-  for (long long r0 = static_cast<long long>(blockIdx.x) * R; r0 < rows; r0 += static_cast<long long>(gridDim.x) * R, ++it) {
-    uint4 xr[R], dr[R], rr[R];
-    float mean[R], rstd[R];
-    long long dxo[R];
-#pragma unroll
-    for (int i = 0; i < R; ++i) {
-      const long long r = r0 + i;
-      rr[i] = make_uint4(0u, 0u, 0u, 0u);
-      if (r < rows) {
-        unsigned rb, rt;  // every view of one call has the same rows-per-batch: one division per row
-        xv.split(r, rb, rt);
-        xr[i] = *reinterpret_cast<const uint4*>(x + xv.at(rb, rt) + c0);
-        dr[i] = *reinterpret_cast<const uint4*>(dy + dyv.at(rb, rt) + c0);
-        if (dres != nullptr) rr[i] = *reinterpret_cast<const uint4*>(dres + dresv.at(rb, rt) + c0);
-        dxo[i] = dxv.at(rb, rt);
-        mean[i] = mean_in[r];
-        rstd[i] = rstd_in[r];
-      } else {  // past the end: contributes zeros everywhere, never stored
-        xr[i] = dr[i] = make_uint4(0u, 0u, 0u, 0u);
-        mean[i] = rstd[i] = 0.f;
-        dxo[i] = 0;
-      }
-    }
-    float dz[GELU ? R : 1][8], s1[R], s2[R];
-#pragma unroll
-    for (int i = 0; i < R; ++i) {
-      const uint32_t xu[4] = {xr[i].x, xr[i].y, xr[i].z, xr[i].w};
-      const uint32_t du[4] = {dr[i].x, dr[i].y, dr[i].z, dr[i].w};
-      s1[i] = s2[i] = 0.f;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float2 xf = unpack_bf16x2(xu[k]), df = unpack_bf16x2(du[k]);
-        const float xv2[2] = {xf.x, xf.y}, dv2[2] = {df.x, df.y};
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int j = 2 * k + h;
-          const float xn = (xv2[h] - mean[i]) * rstd[i];
-          float d = dv2[h];
-          if (GELU) d *= gelu_grad_f(g[j] * xn + bt[j]);
-          ag[j] = fmaf(d, xn, ag[j]);
-          ab[j] += d;
-          const float dxh = d * g[j];
-          if (GELU) dz[i][j] = dxh;
-          s1[i] += dxh;
-          s2[i] = fmaf(dxh, xn, s2[i]);
-        }
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < R; ++i) {
-      s1[i] = warp_sum(s1[i]);
-      s2[i] = warp_sum(s2[i]);
-    }
-    float* mine = red[it & 1][warp];
-    if (lane == 0) {
-#pragma unroll
-      for (int i = 0; i < R; ++i) {
-        mine[2 * i] = s1[i];
-        mine[2 * i + 1] = s2[i];
-      }
-    }
-    __syncthreads();  // (the buffer of iteration it - 1 is re-written only after every warp has passed this barrier once more)
-    if (!GELU) {
-      // make the packed vectors opaque so that x-hat and d x-hat are RE-DERIVED below instead of being carried across the
-      // barrier in 16 registers per row (common-subexpression elimination would otherwise keep them)
-#pragma unroll
-      for (int i = 0; i < R; ++i) {
-        asm volatile("" : "+r"(xr[i].x), "+r"(xr[i].y), "+r"(xr[i].z), "+r"(xr[i].w));
-        asm volatile("" : "+r"(dr[i].x), "+r"(dr[i].y), "+r"(dr[i].z), "+r"(dr[i].w));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < R; ++i) {
-      float t1 = 0.f, t2 = 0.f;
-#pragma unroll
-      for (int w = 0; w < NW; ++w) {
-        t1 += red[it & 1][w][2 * i];
-        t2 += red[it & 1][w][2 * i + 1];
-      }
-      t1 *= (1.0f / D);
-      t2 *= (1.0f / D);
-      const long long r = r0 + i;
-      const uint32_t xu[4] = {xr[i].x, xr[i].y, xr[i].z, xr[i].w};
-      const uint32_t du[4] = {dr[i].x, dr[i].y, dr[i].z, dr[i].w};
-      const uint32_t ru[4] = {rr[i].x, rr[i].y, rr[i].z, rr[i].w};
-      uint32_t ou[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float2 xf = unpack_bf16x2(xu[k]), df = unpack_bf16x2(du[k]), rf = unpack_bf16x2(ru[k]);
-        const float xn0 = (xf.x - mean[i]) * rstd[i], xn1 = (xf.y - mean[i]) * rstd[i];
-        const float z0 = GELU ? dz[GELU ? i : 0][2 * k] : df.x * g[2 * k];
-        const float z1 = GELU ? dz[GELU ? i : 0][2 * k + 1] : df.y * g[2 * k + 1];
-        const float o0 = rf.x + rstd[i] * (z0 - t1 - xn0 * t2);
-        const float o1 = rf.y + rstd[i] * (z1 - t1 - xn1 * t2);
-        ou[k] = pack_bf16x2(o0, o1);
-        if (want_c) {  // the column sum is taken over dx AS STORED (what the producer's weight-gradient GEMM reads)
-          const float2 of = unpack_bf16x2(ou[k]);
-          ac[2 * k] += of.x;
-          ac[2 * k + 1] += of.y;
-        }
-      }
-      if (r < rows) *reinterpret_cast<uint4*>(dx + dxo[i] + c0) = make_uint4(ou[0], ou[1], ou[2], ou[3]);
-    }
-  }
-  auto flush = [&](float* dst, const float* v) {
-    if (dst == nullptr) return;
-    if (vec_atomics) {
-      atomicAdd(reinterpret_cast<float4*>(dst + c0), make_float4(v[0], v[1], v[2], v[3]));
-      atomicAdd(reinterpret_cast<float4*>(dst + c0 + 4), make_float4(v[4], v[5], v[6], v[7]));
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) atomicAdd(dst + c0 + j, v[j]);
-    }
-  };
-  flush(dgamma, ag);
-  flush(dbeta, ab);
-  flush(colsum, ac);
-}
-
 // blocks of `threads` threads of kernel `k` that fit the chip at once (a grid-stride kernel gains nothing from more)
 template <typename K>
 static int resident_grid(K k, int threads) {
@@ -763,29 +602,6 @@ static int dispatch_width(int D, F&& f) {
       set_last_error("row kernels support widths 64/128/256/512/768/1024/1280, got %d", D);
       return -1;
   }
-}
-
-// Which LayerNorm kernels run at the wide widths (512 / 768 / 1024): the block-per-row-group kernels for the gate-fused forward only;
-// elsewhere the warp-per-row kernels -- one block barrier per row group stalls all of a block's warps on the same loads, while
-// independent warp-per-row chains overlap better (tools/bench_rowops.py --norms compares the two).
-// B200S_LN_WIDE=0 / 1 forces the warp-per-row / wide kernels everywhere (A/B runs).
-static int ln_wide_mode() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200S_LN_WIDE");
-    v = (e && e[0] == '0') ? 0 : (e && e[0] == '1') ? 1 : 2;
-  }
-  return v;
-}
-static bool ln_wide_enabled(bool gate_fwd) { return ln_wide_mode() == 1 || (ln_wide_mode() == 2 && gate_fwd); }
-
-static int ln_wide_rows() {  // rows per iteration of the wide backward kernel (B200S_LN_R=2|4, micro-benchmark knob)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200S_LN_R");
-    v = (e && e[0] == '2') ? 2 : 4;
-  }
-  return v;
 }
 
 // one row per warp and iteration, 8 warps per block, four resident blocks per SM
@@ -1307,12 +1123,6 @@ static int layer_norm_fwd_impl(const void* x, long long x_bs, long long x_rs, co
   RowView xv{x_bs, x_rs, rows_per_batch}, yv{y_bs, y_rs, rows_per_batch};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const GateArgs no_gate{nullptr, nullptr, nullptr, nullptr, 0, 1};
-  if (ln_wide_enabled(false) && (D == 512 || D == 768 || D == 1024)) {
-    const __nv_bfloat16* xp = static_cast<const __nv_bfloat16*>(x);
-    __nv_bfloat16* yp = static_cast<__nv_bfloat16*>(y);
-    return gelu ? launch_ln_fwd_wide<false, true>(D, rows, st, xp, xv, gamma, beta, yp, yv, mean, rstd, rows, 1e-5f, no_gate, valid)
-                : launch_ln_fwd_wide<false, false>(D, rows, st, xp, xv, gamma, beta, yp, yv, mean, rstd, rows, 1e-5f, no_gate, valid);
-  }
   int rc = dispatch_width(D, [&](auto vec, auto nch) {
     if (gelu) {
       B200_CHECK_CUDA(launch_pdl(ln_fwd_kernel<decltype(vec)::value, decltype(nch)::value, false, true>, dim3(ln_fwd_grid(rows)),
@@ -1331,7 +1141,10 @@ static int layer_norm_fwd_impl(const void* x, long long x_bs, long long x_rs, co
 }
 
 // LayerNorm forward that also writes the gru_rel_pos gate of the attention consuming y (replaces b200s_gate_fwd + one pass
-// over y).  D = H * 64 in {768, 1024}; x/y contiguous-row views as in b200s_layer_norm_fwd; gate: fp32 [B, H, T].
+// over y).  D = H * 64 in {256, 512, 768, 1024}; x/y contiguous-row views as in b200s_layer_norm_fwd; gate: fp32 [B, H, T].
+// At 512 / 768 / 1024 this is the one LayerNorm that runs the block-per-row-group kernel; every other LayerNorm call uses the
+// warp-per-row kernels at all widths -- one block barrier per row group stalls all of a block's warps on the same loads, while
+// independent warp-per-row chains overlap better.
 static int layer_norm_gate_fwd_impl(const void* x, long long x_bs, long long x_rs, const float* gamma, const float* beta, void* y,
                                     long long y_bs, long long y_rs, float* mean, float* rstd, int T, int B, int D,
                                     const float* grep_w, const float* grep_b, const float* grep_a, int H, float* gate,
@@ -1344,19 +1157,13 @@ static int layer_norm_gate_fwd_impl(const void* x, long long x_bs, long long x_r
   RowView xv{x_bs, x_rs, T}, yv{y_bs, y_rs, T};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const GateArgs ga{grep_w, grep_b, grep_a, gate, H, T};
-  if (ln_wide_enabled(true) && (D == 512 || D == 768 || D == 1024)) {
-    return launch_ln_fwd_wide<true, false>(D, rows, st, static_cast<const __nv_bfloat16*>(x), xv, gamma, beta,
-                                           static_cast<__nv_bfloat16*>(y), yv, mean, rstd, rows, 1e-5f, ga, valid);
+  if (D != 256) {
+    return launch_ln_fwd_wide(D, rows, st, static_cast<const __nv_bfloat16*>(x), xv, gamma, beta, static_cast<__nv_bfloat16*>(y),
+                              yv, mean, rstd, rows, 1e-5f, ga, valid);
   }
-  int rc = dispatch_width(D, [&](auto vec, auto nch) {
-    if constexpr (decltype(vec)::value == 8) {
-      B200_CHECK_CUDA(launch_pdl(ln_fwd_kernel<8, decltype(nch)::value, true, false>, dim3(ln_fwd_grid(rows)), dim3(256), 0, st,
-                                 static_cast<const __nv_bfloat16*>(x), xv, gamma, beta, static_cast<__nv_bfloat16*>(y), yv, mean,
-                                 rstd, rows, 1e-5f, ga, valid));
-    }
-    return 0;
-  });
-  if (rc) return rc;
+  B200_CHECK_CUDA(launch_pdl(ln_fwd_kernel<8, 1, true, false>, dim3(ln_fwd_grid(rows)), dim3(256), 0, st,
+                             static_cast<const __nv_bfloat16*>(x), xv, gamma, beta, static_cast<__nv_bfloat16*>(y), yv, mean, rstd,
+                             rows, 1e-5f, ga, valid));
   B200_CHECK_LAUNCH();
   return 0;
 }
@@ -1373,36 +1180,6 @@ static int layer_norm_bwd_impl(const void* dy, long long dy_bs, long long dy_rs,
   RowView dyv{dy_bs, dy_rs, rows_per_batch}, xv{x_bs, x_rs, rows_per_batch}, rv{dres_bs, dres_rs, rows_per_batch},
       dxv{dx_bs, dx_rs, rows_per_batch};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (valid == nullptr && ln_wide_enabled(false) && (D == 512 || D == 768 || D == 1024)) {  // (the wide kernel has no ragged form)
-    const auto aligned16 = [](const float* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-    const int vec_atomics = aligned16(dgamma) && aligned16(dbeta) && aligned16(colsum);
-    auto go = [&](auto nw, auto rr, auto ge) {
-      constexpr int NW = decltype(nw)::value, R = decltype(rr)::value;
-      auto kern = ln_bwd_wide_kernel<NW, R, decltype(ge)::value>;
-      static const int cap = resident_grid(kern, 32 * NW);
-      const int grid = static_cast<int>(std::min<long long>(ceil_div_ll(rows, R), cap));
-      B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(32 * NW), 0, st, static_cast<const __nv_bfloat16*>(dy), dyv,
-                                 static_cast<const __nv_bfloat16*>(x), xv, mean, rstd, gamma, beta,
-                                 static_cast<const __nv_bfloat16*>(dres), rv, static_cast<__nv_bfloat16*>(dx), dxv, dgamma, dbeta,
-                                 colsum, rows, vec_atomics));
-      return 0;
-    };
-    using I2 = std::integral_constant<int, 2>;
-    using I3 = std::integral_constant<int, 3>;
-    using I4 = std::integral_constant<int, 4>;
-    const int r_sel = ln_wide_rows();
-    int rcw;
-    if (gelu) {
-      rcw = D == 512 ? go(I2{}, I2{}, std::true_type{}) : D == 768 ? go(I3{}, I2{}, std::true_type{}) : go(I4{}, I2{}, std::true_type{});
-    } else if (r_sel == 2) {
-      rcw = D == 512 ? go(I2{}, I2{}, std::false_type{}) : D == 768 ? go(I3{}, I2{}, std::false_type{}) : go(I4{}, I2{}, std::false_type{});
-    } else {
-      rcw = D == 512 ? go(I2{}, I4{}, std::false_type{}) : D == 768 ? go(I3{}, I4{}, std::false_type{}) : go(I4{}, I4{}, std::false_type{});
-    }
-    if (rcw) return rcw;
-    B200_CHECK_LAUNCH();
-    return 0;
-  }
   long long blocks = ceil_div_ll(rows, 8 * 4);  // >=4 rows per warp so the column partial sums amortise
   const long long cap = static_cast<long long>(sm_count()) * 2;
   if (blocks > cap) blocks = cap;
