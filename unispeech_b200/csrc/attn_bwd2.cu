@@ -245,23 +245,24 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
 
     // diagonal sums of the staged gate*dS tile of query tile qi.  Task (e, s): elements (key (ii + e) & 127, query ii) for
     // ii = 16 s .. 16 s + 15: diagonal key - query = e (not wrapped, ii + e < 128) or e - 128 (wrapped).  The wrap point is a
-    // per-task constant, so every load is base + immediate.
+    // per-task constant, so every load is base + immediate.  The two diagonals are summed separately: the wrapped sum taken as
+    // (all - not wrapped) would carry an error of EPS32 times the other diagonal's sum, which can be larger than its own.
     auto diag_task = [&](int qi, int e, int s) {
       const int w0 = kAttnTile - e - 16 * s;  // queries ii = 16 s + c with c >= w0 are on the wrapped diagonal
       const uint32_t base_nw = smem_u32(wtile) + static_cast<uint32_t>(((16 * s + e) * kWStride + 16 * s) * 2);
       const uint32_t base_w = base_nw - static_cast<uint32_t>(kAttnTile * kWStride * 2);
-      float acc_all = 0.f, acc_nw = 0.f;
+      float acc_w = 0.f, acc_nw = 0.f;
 #pragma unroll
       for (int c = 0; c < 16; ++c) {
         const bool wrapped = c >= w0;
         uint32_t v16;
         asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v16) : "r"((wrapped ? base_w : base_nw) + c * (kWStride + 1) * 2));
         const float v = __uint_as_float(v16 << 16);
-        acc_all += v;
-        if (!wrapped) acc_nw += v;
+        if (wrapped) acc_w += v;
+        else acc_nw += v;
       }
       if (w0 > 0) atomicAdd(&dtab_acc[kAttnTile + e], acc_nw);   // upper block (m = e + 128)
-      if (w0 < 16) atomicAdd(&dtab_acc[e], acc_all - acc_nw);    // lower block (m = e)
+      if (w0 < 16) atomicAdd(&dtab_acc[e], acc_w);               // lower block (m = e)
     };
 
     mbar_wait(&kv_full, 0);
