@@ -107,7 +107,7 @@ int b200s_posconv_wgrad(const void* dy, long long dy_bs, long long dy_rs, const 
  * Replaces compute_bias + gate multiply + F.multi_head_attention_forward (WavLM/modules.py:417-455,504-563); the
  * [B*H,T,T] bias is never materialised (it is Toeplitz).  qkv: bf16 [B,T,3D] fused projection output; gate: fp32
  * [B,H,T] or NULL (=1); tab: fp32 [H,2T-1] or NULL (no bias); key_pad: uint8 [B,T] or NULL; out: bf16 [B,T,D];
- * lse: fp32 [B,H,T] log2-domain log-sum-exp (saved for backward).  head_dim HD = 64, or 80 with tab = NULL (D = H * HD;
+ * lse: fp32 [B,H,T] log2-domain log-sum-exp (saved for backward).  head_dim HD = 64, or 80 / 120 with tab = NULL (D = H * HD;
  * any other value is an error); any T >= 1 with B*H*T < 2^32 (the kernel stages the bias window and key mask per key tile:
  * its shared memory does not depend on T).  The same head_dim argument ends every attention entry point below. */
 int b200s_attn_fwd(const void* qkv, const float* gate, const float* tab, const uint8_t* key_pad, void* out,

@@ -1,7 +1,8 @@
 """Micro-benchmark of the attention kernels at the WavLM-Base (16 x 749, 12 heads) and -Large (8 x 999, 16 heads) shapes.
     python tools/bench_attn.py [--reps 10] [--only base|large|long|wide] [--dropout 0.1]
 `--only wide` times the forward, the forward with dropout (--dropout, else 0.1) and the fused backward without the bias at
-8 x 999 with 16 heads at head width 80 (the 1280-wide encoders) next to head width 64 at the same shape; it runs only when asked.
+8 x 999 with 16 heads at head widths 80 (the 1280-wide encoders) and 120 (XLS-R 2B) next to head width 64 at the same shape;
+it runs only when asked.
 `--only long` times one utterance with 16 heads at T = 8192 (164 s: the forward and both backward entry points) and
 T = 16384 (the forward), and checks every call once against the fp32 reference one head at a time (one [T, T] fp32
 matrix is 1 GB at T = 16384).
@@ -209,12 +210,12 @@ for name, B, T, H in (("base", 16, 749, 12), ("large", 8, 999, 16)):
             all_ok &= check_bwd(k, fn, qkv, gate if bias else None, tab if bias else None, dout, dqkv, dgate, dtab if bias else None,
                                 B, T, H, keep, args.dropout)
             del keep
-# 1280-wide encoders (XLS-R 1B, MMS-1B, HuBERT X-Large): head width 80, no relative-position bias, beside head width 64 at the same
-# B, T, H.  Algorithmic FLOPs scale with the head width.
+# 1280-wide encoders (XLS-R 1B, MMS-1B, HuBERT X-Large) and XLS-R 2B: head widths 80 and 120, no relative-position bias, beside
+# head width 64 at the same B, T, H.  Algorithmic FLOPs scale with the head width.
 if args.only == "wide":
     B, T, H = 8, 999, 16
     p_w = args.dropout if args.dropout > 0 else 0.1
-    for hd in (64, 80):
+    for hd in (64, 80, 120):
         D = H * hd
         torch.manual_seed(0)
         qkv = torch.randn(B, T, 3 * D, device=dev).to(torch.bfloat16)

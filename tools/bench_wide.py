@@ -1,4 +1,5 @@
-"""The 1280-wide encoders (`xlsr1b` workload: XLS-R 1B / MMS-1B shape, 48 layers, head width 80) on one GPU:
+"""The wide encoders on one GPU: `xlsr1b` (XLS-R 1B / MMS-1B shape, 48 x 1280, head width 80, the default) or `xlsr2b`
+(XLS-R 2B, 48 x 1920, head width 120), chosen with --workload:
 
 * one `Wav2VecCtc` fine-tuning step (forward, CTC loss, backward, `FusedAdam`) on 8 x 20 s: ms per step, median and range over
   rounds;
@@ -8,7 +9,7 @@
 
 Weights are the modules' default initialisation (timing does not depend on them).  Prints one JSON line.
 
-    python tools/bench_wide.py [--rounds 5] [--steps 5] [--warmup 2]
+    python tools/bench_wide.py [--workload xlsr1b|xlsr2b] [--rounds 5] [--steps 5] [--warmup 2]
 """
 import argparse
 import json
@@ -29,6 +30,7 @@ from unispeech_b200.optim import FusedAdam  # noqa: E402
 from unispeech_b200.wav2vec2 import Wav2Vec2Config, Wav2Vec2Model  # noqa: E402
 
 ap = argparse.ArgumentParser()
+ap.add_argument("--workload", choices=("xlsr1b", "xlsr2b"), default="xlsr1b")
 ap.add_argument("--rounds", type=int, default=5)
 ap.add_argument("--steps", type=int, default=5, help="timed steps per round")
 ap.add_argument("--warmup", type=int, default=2)
@@ -45,7 +47,7 @@ except (OSError, subprocess.SubprocessError):
     card = ""
 card = card or f"{torch.cuda.get_device_name(0)}, power limit unknown"
 
-cfg, B, secs = W.model_config("xlsr1b")
+cfg, B, secs = W.model_config(args.workload)
 cfg = dict(cfg, dropout=0.0, attention_dropout=0.0, mask_prob=0.65)
 L = secs * W.SR
 torch.manual_seed(0)
@@ -101,8 +103,9 @@ with torch.no_grad():
         fwd_rate.append(B * secs * args.steps / (time.perf_counter() - t0))
 
 res = {
-    "workload": f"xlsr1b (48 x 1280 / 5120, 16 heads of width 80, pre-LN, no relative-position bias), batch {B} x {secs} s, "
-                f"Wav2VecCtc vocab {args.vocab}, mask_prob 0.65, dropout 0",
+    "workload": f"{args.workload} ({cfg['encoder_layers']} x {cfg['encoder_embed_dim']} / {cfg['encoder_ffn_embed_dim']}, "
+                f"{cfg['encoder_attention_heads']} heads of width {cfg['encoder_embed_dim'] // cfg['encoder_attention_heads']}, "
+                f"pre-LN, no relative-position bias), batch {B} x {secs} s, Wav2VecCtc vocab {args.vocab}, mask_prob 0.65, dropout 0",
     "card": card,
     "finetune_ms_per_step": {"median": float(np.median(step_ms)), "min": min(step_ms), "max": max(step_ms),
                              "rounds": args.rounds, "steps_per_round": args.steps},

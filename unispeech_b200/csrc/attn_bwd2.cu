@@ -50,6 +50,11 @@
 // tile is one [128 keys][64 queries] block, and dQ = dS K is split over the keys instead of the queries: each warpgroup
 // reduces its 64 keys' share of the tile's 64 x 80 dQ (TMA reductions of 32 + 32 + 16 columns).  The dropout mask words are
 // the same (a tile covers two 32-query blocks instead of four).
+// Head width 120 (no bias) keeps those 64-query tiles.  K / V are [2 blocks][128 keys][128 B] and Q / dO [2][64][128 B] with a
+// zero tail (attn_common.cuh); S^T / dP^T take eight k16 steps, dV and dK are one n128 wgmma each (64 + 64 accumulator
+// registers, columns 120..127 dead), and dQ = dS K is split over the columns instead: warpgroup w computes columns
+// 64 w .. 64 w + 63 of the tile's 64 x 120 dQ over all 128 keys and reduces them with two 32-column boxes of the head-shaped
+// fp32 map, whose last box clips at column 120.  Each dQ element is reduced once per key tile, as at width 64.
 #include "../../include/unispeech_b200.h"
 #include "attn_common.cuh"
 #include "common.h"
@@ -76,21 +81,23 @@ constexpr int kFThreads = 256;     // two warpgroups
 //   WG's own staged rows); per stage lse, Delta*scale, gate*log2e, gate/scale [4][128] fp32 at 164864; d gate partial column
 //   sums [8 warps][128] fp32 at 168960; 174080 bytes with the alignment slack (+ 2 KB static: bias window and d tab blocks).
 // At HD = 80: 20 KB K / V tiles, 10 KB Q / dO stages (64 queries), one 16 KB dS^T block, and 20 KB of dQ staging per WG
-// (two [64][32] SWIZZLE_128B boxes and one [64][16] fp32 box): 148480 bytes.  Both are the same for every T.
+// (two [64][32] SWIZZLE_128B boxes and one [64][16] fp32 box): 148480 bytes.  At HD = 120: 32 KB K / V tiles, 16 KB Q / dO
+// stages, one 16 KB dS^T block and 16 KB of dQ staging per WG: 189440 bytes.  All are the same for every T.
 template <int HD>
 struct BwdMap {
   static constexpr int kQT = HD == 64 ? kAttnTile : 64;  // queries per tile
-  static constexpr int kKV = kAttnTile * HD * 2;           // one K or V tile
-  static constexpr int kQS = kQT * HD * 2;                 // one Q or dO stage
+  static constexpr int kKV = kAttnTile * attn_tile_cols<HD>() * 2;  // one K or V tile
+  static constexpr int kQS = kQT * attn_tile_cols<HD>() * 2;        // one Q or dO stage
   static constexpr int kFK = 0, kFV = kKV, kFQ = 2 * kKV, kFDO = kFQ + 2 * kQS, kFDS = kFDO + 2 * kQS;
   static constexpr int kFW = kFDS + kAttnTile * kQT * 2;
-  static constexpr int kFDQ1 = HD == 64 ? 17408 : 64 * HD * 4;
-  static constexpr int kFWBytes = kFDQ1 + (HD == 64 ? 16384 : 64 * HD * 4);
+  static constexpr int kFDQ1 = HD == 64 ? 17408 : HD == 80 ? 64 * HD * 4 : 16384;
+  static constexpr int kFWBytes = kFDQ1 + (HD == 80 ? 64 * HD * 4 : 16384);
   static constexpr int kFScal = kFW + kFWBytes;
   static constexpr int kFDg = kFScal + 2 * 4 * 512;
   static constexpr int kFSmem = kFDg + 8 * 512 + 1024;
 };
 static_assert(BwdMap<64>::kFDS == 98304 && BwdMap<64>::kFScal == 164864 && BwdMap<64>::kFSmem == 174080, "HD 64 map");
+static_assert(BwdMap<80>::kFSmem == 148480 && BwdMap<120>::kFSmem == 189440, "HD 80 / 120 maps");
 
 }  // namespace
 
@@ -102,9 +109,10 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
                                                                       const __grid_constant__ CUtensorMap tm_do16,
                                                                       const __grid_constant__ CUtensorMap tm_dq16,
                                                                       const __grid_constant__ AttnParams p) {
-  static_assert(HD == 64 || (HD == 80 && !HAS_BIAS), "head width 64, or 80 without the relative-position bias");
+  static_assert(HD == 64 || ((HD == 80 || HD == 120) && !HAS_BIAS), "head width 64, or 80 / 120 without the relative-position bias");
   using M = BwdMap<HD>;
   constexpr int QT = M::kQT, kFDS = M::kFDS, kFW = M::kFW, kFDQ1 = M::kFDQ1;
+  constexpr int kA = HD == 120 ? 64 : 32;  // dK / dV accumulator registers of the first (or only) wgmma
   pdl_grid_sync();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int k0 = blockIdx.x * kAttnTile, h = blockIdx.y, b = blockIdx.z;
@@ -240,7 +248,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     const uint32_t ak = smem_u32(sK) + w * 8192, av = smem_u32(sV) + w * 8192;
     uint32_t* wtile = reinterpret_cast<uint32_t*>(smem + kFW);
 
-    float dv_acc[32], dk_acc[32];  // written by the first tile's MMAs (scale_d = 0)
+    float dv_acc[kA], dk_acc[kA];  // written by the first tile's MMAs (scale_d = 0)
     float dv16[8], dk16[8];        // their columns 64..79 (HD = 80 only)
 
     // diagonal sums of the staged gate*dS tile of query tile qi.  Task (e, s): elements (key (ii + e) & 127, query ii) for
@@ -271,11 +279,13 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       mbar_wait(&qdo_full[st], (qi >> 1) & 1);
       const uint32_t bq = smem_u32(sQ + st * M::kQS), bdo = smem_u32(sDO + st * M::kQS);
       float s_acc[QT / 2], d_acc[QT / 2];
-      // S^T = K_w Q^T and dP^T = V_w dO^T over the head width (at HD = 80 the fifth k16 step reads the 32-byte blocks)
+      // S^T = K_w Q^T and dP^T = V_w dO^T over the head width (at HD = 80 the fifth k16 step reads the 32-byte blocks; at
+      // HD = 120 steps 4..7 read the second 64-column blocks)
       auto scores = [&](float* acc, uint32_t a, uint32_t bt) {
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t da = make_smem_desc_sw128(a + k * 32, 16, 1024), db = make_smem_desc_sw128(bt + k * 32, 16, 1024);
+        for (int k = 0; k < (HD == 120 ? 8 : 4); ++k) {
+          const uint64_t da = make_smem_desc_sw128(a + (k >> 2) * (kAttnTile * 128) + (k & 3) * 32, 16, 1024),
+                         db = make_smem_desc_sw128(bt + (k >> 2) * (QT * 128) + (k & 3) * 32, 16, 1024);
           if (QT == 128) wgmma_m64n128k16<0, 0>(acc, da, db, k > 0 ? 1u : 0u);
           else wgmma_m64n64k16<0, 0>(acc, da, db, k > 0 ? 1u : 0u);
         }
@@ -390,7 +400,10 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < QT / 16; ++k) {  // K = the tile's queries, 16 per step
-        wgmma_m64n64k16_rs<1>(dv_acc, p16 + 4 * k, make_smem_desc_sw128(bdo + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+        if (HD == 120)
+          wgmma_m64n128k16_rs<1>(dv_acc, p16 + 4 * k, make_smem_desc_sw128(bdo + k * 2048, QT * 128, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+        else
+          wgmma_m64n64k16_rs<1>(dv_acc, p16 + 4 * k, make_smem_desc_sw128(bdo + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
         if (HD == 80)
           wgmma_m64n16k16_rs<1>(dv16, p16 + 4 * k, make_smem_desc_sw32(bdo + QT * 128 + k * 512), (qi > 0 || k > 0) ? 1u : 0u);
       }
@@ -403,15 +416,17 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
 #pragma unroll
       for (int k = 0; k < QT / 16; ++k) {
         const uint64_t da = make_smem_desc_sw128(smem_u32(sDS) + (k >> 2) * 16384 + w * 8192 + (k & 3) * 32, 16, 1024);
-        wgmma_m64n64k16<0, 1>(dk_acc, da, make_smem_desc_sw128(bq + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+        if (HD == 120) wgmma_m64n128k16<0, 1>(dk_acc, da, make_smem_desc_sw128(bq + k * 2048, QT * 128, 1024), (qi > 0 || k > 0) ? 1u : 0u);
+        else wgmma_m64n64k16<0, 1>(dk_acc, da, make_smem_desc_sw128(bq + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
         if (HD == 80) wgmma_m64n16k16<0, 1>(dk16, da, make_smem_desc_sw32(bq + QT * 128 + k * 512), (qi > 0 || k > 0) ? 1u : 0u);
       }
       // ---- dQ = dS K.  HD 64: this WG's 64 queries, K = 128 keys.  HD 80: the tile's 64 queries, K = this WG's 64 keys (the two
-      // WGs' shares are added by the reductions).  A = the dS^T tile read MN-major, 16 keys per step.
+      // WGs' shares are added by the reductions).  HD 120: the tile's 64 queries x this WG's 64 columns, K = 128 keys.  A = the
+      // dS^T tile read MN-major, 16 keys per step.
       float dq[32], dq16[8];
-      constexpr int kDqSteps = QT == kAttnTile ? 8 : 4;
-      const uint32_t dq_a = smem_u32(sDS) + (QT == kAttnTile ? w * 16384 : w * 8192);
-      const uint32_t dq_b = smem_u32(sK) + (QT == kAttnTile ? 0 : w * 8192);
+      constexpr int kDqSteps = QT == kAttnTile || HD == 120 ? 8 : 4;
+      const uint32_t dq_a = smem_u32(sDS) + (QT == kAttnTile ? w * 16384 : HD == 120 ? 0 : w * 8192);
+      const uint32_t dq_b = smem_u32(sK) + (QT == kAttnTile ? 0 : HD == 120 ? w * 16384 : w * 8192);
 #pragma unroll
       for (int k = 0; k < kDqSteps; ++k) {
         const uint64_t da = make_smem_desc_sw128(dq_a + k * 2048, 16384, 1024);
@@ -482,7 +497,11 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       fence_proxy_async_smem();
       named_bar_sync(2 + w, 128);
       const int dq_row = QT == kAttnTile ? qi * kAttnTile + 64 * w : qi * QT;
-      if (flusher && dq_row < T) {
+      if (HD == 120 && flusher && dq_row < T) {  // head-shaped map: (column in the head, head, row, batch); the box at 96 clips
+        tma_reduce_add_4d(&tm_dq, smem_u32(dq_stage), 64 * w, h, dq_row, b);
+        tma_reduce_add_4d(&tm_dq, smem_u32(dq_stage) + 8192, 64 * w + 32, h, dq_row, b);
+        bulk_commit();
+      } else if (flusher && dq_row < T) {
         tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage), h * HD, dq_row, b);
         tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage) + 8192, h * HD + 32, dq_row, b);
         if (HD == 80) tma_reduce_add_3d(&tm_dq16, smem_u32(dq_stage) + 16384, h * HD + 64, dq_row, b);
@@ -508,7 +527,8 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
         __nv_bfloat16* dst = p.dqkv + (static_cast<long long>(b) * T + key) * (3 * D) + h * HD + fc;
         const float rp = DROP ? p.drop_rp : 1.0f;   // dV = (P o M)^T dO / (1-p)
 #pragma unroll
-        for (int g = 0; g < 8; ++g) {
+        for (int g = 0; g < kA / 4; ++g) {
+          if (8 * g >= HD) continue;  // HD 120: columns 120..127 belong to the next head (or the next section)
           *reinterpret_cast<uint32_t*>(dst + 2 * D + 8 * g) = pack_bf16x2(dv_acc[4 * g + 2 * rr] * rp, dv_acc[4 * g + 2 * rr + 1] * rp);
           *reinterpret_cast<uint32_t*>(dst + D + 8 * g) = pack_bf16x2(dk_acc[4 * g + 2 * rr], dk_acc[4 * g + 2 * rr + 1]);
         }
@@ -582,6 +602,8 @@ __global__ void __launch_bounds__(256) attn_dq_convert_kernel(float* __restrict_
 
 int make_qkv_tmap(CUtensorMap* out, const void* qkv, int T, int B, int D3, int box_cols, int box_rows);
 int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_cols, int box_rows);
+int make_head_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int hd, int box_rows);
+int make_f32_head_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int hd, int box_rows);
 
 
 // Delta pre-kernel, the fused kernel and the dQ conversion on one stream (see the entry points below for the contract).
@@ -591,16 +613,22 @@ static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, c
                            int head_dim, cudaStream_t st) {
   const int D = H * head_dim;
   const long long rows = static_cast<long long>(B) * T;
-  B200_CHECK_CUDA(launch_pdl(head_dim == 80 ? attn_delta2_kernel<80> : attn_delta2_kernel<64>, dim3(static_cast<unsigned>(ceil_div_ll(rows * 32, 256))), dim3(256), 0, st,
+  B200_CHECK_CUDA(launch_pdl(head_dim == 120 ? attn_delta2_kernel<120> : head_dim == 80 ? attn_delta2_kernel<80> : attn_delta2_kernel<64>, dim3(static_cast<unsigned>(ceil_div_ll(rows * 32, 256))), dim3(256), 0, st,
       static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), B, T, H, delta,
       tab != nullptr ? dgate : nullptr));
   B200_CHECK_LAUNCH();
 
   CUtensorMap tm_qkv, tm_do, tm_dq, tm_qkv16, tm_do16, tm_dq16;
   const int box_rows = head_dim == 64 ? kAttnTile : BwdMap<80>::kQT;
-  if (make_qkv_tmap(&tm_qkv, qkv, T, B, 3 * D, 64, box_rows)) return -3;
-  if (make_qkv_tmap(&tm_do, dout, T, B, D, 64, box_rows)) return -3;
-  if (make_f32_rows_tmap(&tm_dq, dq_acc, T, B, D, 32, 64)) return -3;
+  if (head_dim == 120) {
+    if (make_head_tmap(&tm_qkv, qkv, T, B, 3 * D, 120, box_rows)) return -3;
+    if (make_head_tmap(&tm_do, dout, T, B, D, 120, box_rows)) return -3;
+    if (make_f32_head_tmap(&tm_dq, dq_acc, T, B, D, 120, 64)) return -3;
+  } else {
+    if (make_qkv_tmap(&tm_qkv, qkv, T, B, 3 * D, 64, box_rows)) return -3;
+    if (make_qkv_tmap(&tm_do, dout, T, B, D, 64, box_rows)) return -3;
+    if (make_f32_rows_tmap(&tm_dq, dq_acc, T, B, D, 32, 64)) return -3;
+  }
   if (head_dim == 80) {
     if (make_qkv_tmap(&tm_qkv16, qkv, T, B, 3 * D, 16, box_rows)) return -3;
     if (make_qkv_tmap(&tm_do16, dout, T, B, D, 16, box_rows)) return -3;
@@ -626,11 +654,12 @@ static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, c
   p.drop_mask = const_cast<uint32_t*>(drop_mask);
   p.drop_rp = 1.0f / (1.0f - drop_p);
   const int N = p.n_tiles;
-  const int smem = head_dim == 64 ? BwdMap<64>::kFSmem : BwdMap<80>::kFSmem;
+  const int smem = head_dim == 64 ? BwdMap<64>::kFSmem : head_dim == 80 ? BwdMap<80>::kFSmem : BwdMap<120>::kFSmem;
   dim3 grid(N, H, B);
   void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                const AttnParams) =
-      head_dim == 80 ? (drop ? attn_bwd_fused_kernel<80, false, true> : attn_bwd_fused_kernel<80, false, false>)
+      head_dim == 120 ? (drop ? attn_bwd_fused_kernel<120, false, true> : attn_bwd_fused_kernel<120, false, false>)
+      : head_dim == 80 ? (drop ? attn_bwd_fused_kernel<80, false, true> : attn_bwd_fused_kernel<80, false, false>)
       : tab != nullptr ? (drop ? attn_bwd_fused_kernel<64, true, true> : attn_bwd_fused_kernel<64, true, false>)
                        : (drop ? attn_bwd_fused_kernel<64, false, true> : attn_bwd_fused_kernel<64, false, false>);
   B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -657,7 +686,8 @@ int b200s_attn_bwd(const void* qkv, const void* out, const void* dout, const flo
                    const uint8_t* key_pad, const float* lse, float* delta, void* dqkv, float* dgate, float* dtab, int B,
                    int T, int H, float scale, int head_dim, b200s_stream stream) {
   B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv, "attn_bwd: null pointer");
-  B200_CHECK_ARG(head_dim == 64 || head_dim == 80, "attn_bwd: head_dim=%d is not supported (64 or 80)", head_dim);
+  B200_CHECK_ARG(head_dim == 64 || head_dim == 80 || head_dim == 120, "attn_bwd: head_dim=%d is not supported (64, 80 or 120)",
+                 head_dim);
   B200_CHECK_ARG(head_dim == 64 || tab == nullptr, "attn_bwd: the relative-position bias needs head_dim 64 (got %d)", head_dim);
   B200_CHECK_ARG(T >= 1, "attn_bwd: T=%d out of range", T);
   B200_CHECK_ARG(!tab || (dgate && dtab), "attn_bwd: bias given but dgate/dtab missing");
@@ -679,7 +709,8 @@ int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* d
                                  float* dgate, float* dtab, int B, int T, int H, float scale, float drop_p,
                                  const uint32_t* drop_mask, int head_dim, b200s_stream stream) {
   B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv && dq_acc, "attn_bwd_fused: null pointer");
-  B200_CHECK_ARG(head_dim == 64 || head_dim == 80, "attn_bwd_fused: head_dim=%d is not supported (64 or 80)", head_dim);
+  B200_CHECK_ARG(head_dim == 64 || head_dim == 80 || head_dim == 120, "attn_bwd_fused: head_dim=%d is not supported (64, 80 or 120)",
+                 head_dim);
   B200_CHECK_ARG(head_dim == 64 || tab == nullptr, "attn_bwd_fused: the relative-position bias needs head_dim 64 (got %d)",
                  head_dim);
   B200_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f, "attn_bwd_fused: dropout p=%f out of range [0,1)", static_cast<double>(drop_p));

@@ -103,6 +103,14 @@ int make_qkv_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int
   return make_tmap(out, v);
 }
 
+// [B, T, cols] bf16 seen as [B, T, cols / hd heads, hd] (innermost dimension = one attention head): box = 64 columns of one
+// head x box_rows rows.  A box that starts at column 64 of a 120-wide head gets zeros for columns 120..127 instead of the
+// next head's columns (used by the attention kernels at head width 120)
+int make_head_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int hd, int box_rows) {
+  ViewSpec v{ptr, {hd, cols / hd, T, B}, {hd, cols, static_cast<long long>(T) * cols}, {64, 1, box_rows, 1}};
+  return make_tmap(out, v);
+}
+
 // [batches, rows, cols] bf16 with arbitrary row / batch strides (elements): box = 64 columns x box_rows rows (k-means operands)
 int make_rows_tmap(CUtensorMap* out, const void* ptr, long long cols, long long rows, long long batches, long long row_stride,
                    long long batch_stride, int box_rows) {
@@ -128,6 +136,32 @@ int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int col
                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled failed (%d) for the fp32 [%d, %d, %d] map", static_cast<int>(r), B, T, cols);
+    return -3;
+  }
+  return 0;
+}
+
+// [B, T, cols] fp32 seen as [B, T, cols / hd heads, hd] (the attention backward's dQ accumulator at head width 120): box = 32
+// columns of one head (SWIZZLE_128B) x box_rows rows.  As a TMA reduction destination the box clips at the head's last column
+// and at T, so the columns of the next head are never written.
+int make_f32_head_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int hd, int box_rows) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) {
+    set_last_error("cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
+    return -3;
+  }
+  const cuuint64_t dims[4] = {static_cast<cuuint64_t>(hd), static_cast<cuuint64_t>(cols / hd), static_cast<cuuint64_t>(T),
+                              static_cast<cuuint64_t>(B)};
+  const cuuint64_t strides[3] = {static_cast<cuuint64_t>(hd) * 4, static_cast<cuuint64_t>(cols) * 4,
+                                 static_cast<cuuint64_t>(T) * cols * 4};
+  const cuuint32_t box[4] = {32, 1, static_cast<cuuint32_t>(box_rows), 1};
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(ptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled failed (%d) for the fp32 head map [%d, %d, %d / %d, %d]", static_cast<int>(r), B, T,
+                   cols, hd, hd);
     return -3;
   }
   return 0;

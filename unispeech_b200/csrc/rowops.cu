@@ -109,8 +109,9 @@ struct GateArgs {
   int H, T;
 };
 
+// (D = 1920: 60 values per lane do not fit the 64 registers of four resident blocks; two blocks give 128)
 template <int VEC, int NCH, bool GATE, bool GELU>
-__global__ void __launch_bounds__(256, 4) ln_fwd_kernel(const __nv_bfloat16* __restrict__ x, RowView xv,
+__global__ void __launch_bounds__(256, 32 * VEC * NCH > 1280 ? 2 : 4) ln_fwd_kernel(const __nv_bfloat16* __restrict__ x, RowView xv,
                                                      const float* __restrict__ gamma, const float* __restrict__ beta,
                                                      __nv_bfloat16* __restrict__ y, RowView yv,
                                                      float* __restrict__ mean_out, float* __restrict__ rstd_out,
@@ -431,8 +432,9 @@ __device__ __forceinline__ void smem_add_perm(float* base, int ch, int lane, con
   }
 }
 
+// (D = 1920: one resident block, which its 195 KB of column partials allow anyway, so 60 values per lane fit in registers)
 template <int VEC, int NCH>
-__global__ void __launch_bounds__(256, 2) ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, RowView dyv,
+__global__ void __launch_bounds__(256, 32 * VEC * NCH > 1280 ? 1 : 2) ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, RowView dyv,
                                                         const __nv_bfloat16* __restrict__ x, RowView xv,
                                                         const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
                                                         const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -598,8 +600,9 @@ static int dispatch_width(int D, F&& f) {
     case 768: return f(std::integral_constant<int, 8>{}, std::integral_constant<int, 3>{});
     case 1024: return f(std::integral_constant<int, 8>{}, std::integral_constant<int, 4>{});
     case 1280: return f(std::integral_constant<int, 8>{}, std::integral_constant<int, 5>{});
+    case 1920: return f(std::integral_constant<int, 4>{}, std::integral_constant<int, 15>{});  // not 32 x 8 x n
     default:
-      set_last_error("row kernels support widths 64/128/256/512/768/1024/1280, got %d", D);
+      set_last_error("row kernels support widths 64/128/256/512/768/1024/1280/1920, got %d", D);
       return -1;
   }
 }

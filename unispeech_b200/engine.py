@@ -173,7 +173,7 @@ class Engine:
     def __init__(self, model):
         self.m = model
         self.cfg = model.cfg
-        self.head_dim = self.cfg.encoder_embed_dim // self.cfg.encoder_attention_heads   # 64 or 80 (wavlm._check_supported)
+        self.head_dim = self.cfg.encoder_embed_dim // self.cfg.encoder_attention_heads   # 64, 80 or 120 (wavlm._check_supported)
         self.dev = None
         self.prepared_version = None
         self.lut_cache: Dict[int, torch.Tensor] = {}

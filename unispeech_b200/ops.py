@@ -242,7 +242,7 @@ def posconv_unprep(weight_v, weight_g, dwp, D, G, taps, work, dweight_v, dweight
 
 
 # ------------------------------------------------------------------------------------------------- attention
-# head_dim: 64, or 80 without the relative-position bias (gate / tab None); D = H * head_dim.  Other values are an error.
+# head_dim: 64, or 80 / 120 without the relative-position bias (gate / tab None); D = H * head_dim.  Other values are an error.
 def attn_fwd(qkv, gate, tab, key_pad, out, lse, B, T, H, scale, head_dim=64):
     _call("b200s_attn_fwd", L.ptr(qkv), L.ptr(gate), L.ptr(tab), L.ptr(key_pad), L.ptr(out), L.ptr(lse), i32(B), i32(T),
            i32(H), f32(scale), i32(head_dim), _s(), flops=4.0 * B * H * T * T * head_dim)

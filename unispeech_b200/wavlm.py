@@ -79,8 +79,8 @@ def _check_supported(cfg):
         bad.append("conv feature width == encoder_embed_dim (the reference then has no post_extract_proj; the projection kernels assume one)")
     D, H = cfg.encoder_embed_dim, cfg.encoder_attention_heads
     head_dim = D // H if D % H == 0 else None
-    if head_dim not in (64, 80):
-        bad.append(f"attention head width {D}/{H} (the attention kernels take head widths 64 and 80)")
+    if head_dim not in (64, 80, 120):
+        bad.append(f"attention head width {D}/{H} (the attention kernels take head widths 64, 80 and 120)")
     elif cfg.relative_position_embedding and head_dim != 64:
         bad.append(f"relative_position_embedding at head width {head_dim} (the gated relative-position bias needs head width 64)")
     if D % cfg.conv_pos_groups != 0 or D // cfg.conv_pos_groups > 128:

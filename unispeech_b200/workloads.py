@@ -31,6 +31,11 @@ _MODELS: Dict[str, Tuple[dict, int, int]] = {
     "xlsr1b": (dict(extractor_mode="layer_norm", encoder_layers=48, encoder_embed_dim=1280, encoder_ffn_embed_dim=5120,
                     encoder_attention_heads=16, layer_norm_first=True, normalize=True, conv_bias=True,
                     relative_position_embedding=False, gru_rel_pos=False), 8, 20),
+    # XLS-R 2B: head width 120, pos_conv groups of 120 channels, otherwise as xlsr1b.  8 x 20 s per GPU fits one 80 GB card:
+    # the fine-tuning step peaks at 64.6 GiB allocated (tools/bench_wide.py --workload xlsr2b, H100 80GB HBM3)
+    "xlsr2b": (dict(extractor_mode="layer_norm", encoder_layers=48, encoder_embed_dim=1920, encoder_ffn_embed_dim=7680,
+                    encoder_attention_heads=16, layer_norm_first=True, normalize=True, conv_bias=True,
+                    relative_position_embedding=False, gru_rel_pos=False), 8, 20),
     "tiny": (dict(encoder_layers=2, encoder_embed_dim=128, encoder_ffn_embed_dim=256, encoder_attention_heads=2,
                   conv_feature_layers="[(64,10,5)] + [(64,3,2)] * 4 + [(64,2,2)] * 2"), 4, 2),
 }
