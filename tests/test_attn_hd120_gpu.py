@@ -1,8 +1,9 @@
 """Attention at head width 120 (XLS-R 2B: D = 1920, 16 heads), without the relative-position bias: forward output and
 log-sum-exp against fp64, dQ / dK / dV through b200s_attn_bwd and b200s_attn_bwd_fused against fp64 autograd with a sentinel in
 dqkv (unwritten columns show), attention dropout (keep bits equal to the hash, forward / backward equal to the reference run
-with those bits), neighbour isolation (a 120-wide head is read and written as exactly 120 columns: the zero-filled tail of its
-second 64-column block never holds the next head's columns), and LayerNorm (+GELU) at D = 1920."""
+with those bits), neighbour isolation at head widths 64, 80 and 120 (a head is read and written as exactly its own columns through
+the head-shaped tensor maps; at 120 the zero-filled tail of its second 64-column block never holds the next head's columns), and
+LayerNorm (+GELU) at D = 1920."""
 import pytest
 import torch
 
@@ -23,27 +24,27 @@ CASES = [  # B, T, H, valid frames per utterance (None: no padding)
 ]
 
 
-def run_fwd(qkv, pad, B, T, H):
+def run_fwd(qkv, pad, B, T, H, hd=HD):
     from unispeech_b200 import ops
-    out = torch.full((B, T, H * HD), SENTINEL, device=qkv.device, dtype=torch.bfloat16)
+    out = torch.full((B, T, H * hd), SENTINEL, device=qkv.device, dtype=torch.bfloat16)
     lse = torch.empty(B, H, T, device=qkv.device)
-    ops.attn_fwd(qkv, None, None, pad, out, lse, B, T, H, HD ** -0.5, head_dim=HD)
+    ops.attn_fwd(qkv, None, None, pad, out, lse, B, T, H, hd ** -0.5, head_dim=hd)
     return out, lse
 
 
-def run_bwd(qkv, out, dout, lse, pad, B, T, H, fused=True):
+def run_bwd(qkv, out, dout, lse, pad, B, T, H, fused=True, hd=HD):
     from unispeech_b200 import ops
-    D = H * HD
+    D = H * hd
     delta = torch.empty(B, H, T, device=qkv.device)
     dqkv = torch.full((B, T, 3 * D), SENTINEL, device=qkv.device, dtype=torch.bfloat16)
     if fused:
         dq_acc = torch.zeros(B, T, D, device=qkv.device)
-        ops.attn_bwd_fused(qkv, out, dout, None, None, pad, lse, delta, dq_acc, dqkv, None, None, B, T, H, HD ** -0.5,
-                           head_dim=HD)
+        ops.attn_bwd_fused(qkv, out, dout, None, None, pad, lse, delta, dq_acc, dqkv, None, None, B, T, H, hd ** -0.5,
+                           head_dim=hd)
         torch.cuda.synchronize()
         assert dq_acc.abs().max().item() == 0.0
     else:
-        ops.attn_bwd(qkv, out, dout, None, None, pad, lse, delta, dqkv, None, None, B, T, H, HD ** -0.5, head_dim=HD)
+        ops.attn_bwd(qkv, out, dout, None, None, pad, lse, delta, dqkv, None, None, B, T, H, hd ** -0.5, head_dim=hd)
         torch.cuda.synchronize()
     return dqkv
 
@@ -77,19 +78,20 @@ def test_attn_hd120_long(cuda_device):
 
 
 @pytest.mark.parametrize("head", [0, 2, 3])
-def test_attn_hd120_neighbours_isolated(cuda_device, head):
+@pytest.mark.parametrize("hd", [64, 80, 120])
+def test_attn_hd120_neighbours_isolated(cuda_device, hd, head):
     """Every column outside head `head` of q, k and v (the other heads, and the same head of the other two sections) holds
     +-1e3.  The head's output and log-sum-exp must equal those of a run with zeros there bit for bit, its gradients up to the
-    rounding of the dQ reductions, and both must match fp64.  head = 3 is the
-    last head of each section (its second block's tail is the next section's first head, or the end of the row)."""
+    rounding of the dQ reductions, and both must match fp64.  head = 3 is the last head of each section (at width 120 its
+    second block's tail is the next section's first head, or the end of the row)."""
     B, T, H = 2, 300, 4
-    D = H * HD
-    qkv, pad, dout = make_inputs(cuda_device, B, T, H, HD, (300, 170), seed=head + 31)
+    D = H * hd
+    qkv, pad, dout = make_inputs(cuda_device, B, T, H, hd, (300, 170), seed=head + 31)
     cols = torch.zeros(3 * D, dtype=torch.bool, device=cuda_device)
     for sec in range(3):
-        cols[sec * D + head * HD: sec * D + (head + 1) * HD] = True
+        cols[sec * D + head * hd: sec * D + (head + 1) * hd] = True
     own = torch.zeros(D, dtype=torch.bool, device=cuda_device)
-    own[head * HD:(head + 1) * HD] = True
+    own[head * hd:(head + 1) * hd] = True
     g = torch.Generator(device=cuda_device).manual_seed(head)
     loud = torch.where(torch.rand(B, T, 3 * D, device=cuda_device, generator=g) < 0.5, -1e3, 1e3).to(torch.bfloat16)
     quiet = qkv.clone()
@@ -99,8 +101,8 @@ def test_attn_hd120_neighbours_isolated(cuda_device, head):
     dout_h[..., ~own] = 0
     res = []
     for x in (quiet, noisy):
-        out, lse = run_fwd(x, pad, B, T, H)
-        dqkv = run_bwd(x, out, dout_h, lse, pad, B, T, H)
+        out, lse = run_fwd(x, pad, B, T, H, hd=hd)
+        dqkv = run_bwd(x, out, dout_h, lse, pad, B, T, H, hd=hd)
         res.append((out, lse, dqkv))
     (o0, l0, g0), (o1, l1, g1) = res
     rows = pad == 0
@@ -111,8 +113,8 @@ def test_attn_hd120_neighbours_isolated(cuda_device, head):
     ga, gb = g0[..., cols][rows].double(), g1[..., cols][rows].double()
     assert (ga - gb).abs().max().item() <= 2.0 ** -7 * ga.abs().max().item()
     # and the head's results are right
-    check_fwd(o1[..., own].contiguous(), l1[:, head:head + 1].contiguous(), quiet[..., cols].contiguous(), pad, B, T, 1, HD)
-    check_bwd(g1[..., cols].contiguous(), quiet[..., cols].contiguous(), pad, dout[..., own].contiguous(), B, T, 1, HD)
+    check_fwd(o1[..., own].contiguous(), l1[:, head:head + 1].contiguous(), quiet[..., cols].contiguous(), pad, B, T, 1, hd)
+    check_bwd(g1[..., cols].contiguous(), quiet[..., cols].contiguous(), pad, dout[..., own].contiguous(), B, T, 1, hd)
 
 
 @pytest.mark.parametrize("B,T,H,valid", [(2, 300, 3, (300, 200)), (1, 520, 2, None)])

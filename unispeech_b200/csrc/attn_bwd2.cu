@@ -45,16 +45,15 @@
 // Dropout: the keep bit of (query i, key j) is bit i & 31 of word drop_mask[block(i), j], written by the forward kernel.
 // Padding: a CTA whose 128 keys are all padded writes zero dK / dV rows and exits; query tiles that are fully padded at the end
 // of the utterance are not visited (their probabilities are zero: the forward leaves lse = +inf there).
-// Head width 80 (no bias; tiles and MMAs as in attn_common.cuh): dK / dV take 80 accumulator registers instead of 64, which
-// the 128-query tiling above cannot afford, so the query tile is 64 rows: S^T / dP^T are m64n64 (32 registers each), the dS^T
-// tile is one [128 keys][64 queries] block, and dQ = dS K is split over the keys instead of the queries: each warpgroup
-// reduces its 64 keys' share of the tile's 64 x 80 dQ (TMA reductions of 32 + 32 + 16 columns).  The dropout mask words are
-// the same (a tile covers two 32-query blocks instead of four).
-// Head width 120 (no bias) keeps those 64-query tiles.  K / V are [2 blocks][128 keys][128 B] and Q / dO [2][64][128 B] with a
-// zero tail (attn_common.cuh); S^T / dP^T take eight k16 steps, dV and dK are one n128 wgmma each (64 + 64 accumulator
-// registers, columns 120..127 dead), and dQ = dS K is split over the columns instead: warpgroup w computes columns
-// 64 w .. 64 w + 63 of the tile's 64 x 120 dQ over all 128 keys and reduces them with two 32-column boxes of the head-shaped
-// fp32 map, whose last box clips at column 120.  Each dQ element is reduced once per key tile, as at width 64.
+// Head widths 80 and 120 (no bias; tiles, maps and MMA shapes per width in attn_common.cuh): dK / dV take 80 or 128
+// accumulator registers instead of 64, which the 128-query tiling above cannot afford, so the query tile is 64 rows: S^T / dP^T
+// are m64n64 (32 registers each) and the dS^T tile is one [128 keys][64 queries] block.  The dropout mask words are the same
+// (a tile covers two 32-query blocks instead of four).  dQ = dS K is decomposed per width, each dQ element reduced through
+// the head-shaped fp32 map ([64 queries][32 columns] SWIZZLE_128B boxes, and at 80 a [64][16] unswizzled one):
+// - 64: warpgroup w computes queries 64 w .. 64 w + 63 of the tile over all 128 keys, once per key tile;
+// - 80: each warpgroup computes its 64 keys' share of the tile's 64 x 80 dQ (the reductions add the two shares);
+// - 120: warpgroup w computes columns 64 w .. 64 w + 63 of the tile's 64 x 120 dQ over all 128 keys, once per key tile; the
+//   box at column 96 clips at 120.
 #include "../../include/unispeech_b200.h"
 #include "attn_common.cuh"
 #include "common.h"
@@ -86,8 +85,8 @@ constexpr int kFThreads = 256;     // two warpgroups
 template <int HD>
 struct BwdMap {
   static constexpr int kQT = HD == 64 ? kAttnTile : 64;  // queries per tile
-  static constexpr int kKV = kAttnTile * attn_tile_cols<HD>() * 2;  // one K or V tile
-  static constexpr int kQS = kQT * attn_tile_cols<HD>() * 2;        // one Q or dO stage
+  static constexpr int kKV = kAttnTile * HeadTile<HD>::kCols * 2;  // one K or V tile
+  static constexpr int kQS = kQT * HeadTile<HD>::kCols * 2;        // one Q or dO stage
   static constexpr int kFK = 0, kFV = kKV, kFQ = 2 * kKV, kFDO = kFQ + 2 * kQS, kFDS = kFDO + 2 * kQS;
   static constexpr int kFW = kFDS + kAttnTile * kQT * 2;
   static constexpr int kFDQ1 = HD == 64 ? 17408 : HD == 80 ? 64 * HD * 4 : 16384;
@@ -109,10 +108,10 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
                                                                       const __grid_constant__ CUtensorMap tm_do16,
                                                                       const __grid_constant__ CUtensorMap tm_dq16,
                                                                       const __grid_constant__ AttnParams p) {
-  static_assert(HD == 64 || ((HD == 80 || HD == 120) && !HAS_BIAS), "head width 64, or 80 / 120 without the relative-position bias");
+  using HT = HeadTile<HD>;
+  static_assert(HT::kBias || !HAS_BIAS, "the relative-position bias at this head width");
   using M = BwdMap<HD>;
   constexpr int QT = M::kQT, kFDS = M::kFDS, kFW = M::kFW, kFDQ1 = M::kFDQ1;
-  constexpr int kA = HD == 120 ? 64 : 32;  // dK / dV accumulator registers of the first (or only) wgmma
   pdl_grid_sync();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int k0 = blockIdx.x * kAttnTile, h = blockIdx.y, b = blockIdx.z;
@@ -179,7 +178,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     tma_prefetch_desc(&tm_qkv);
     tma_prefetch_desc(&tm_do);
     tma_prefetch_desc(&tm_dq);
-    if (HD == 80) {
+    if (HT::kTail) {
       tma_prefetch_desc(&tm_qkv16);
       tma_prefetch_desc(&tm_do16);
       tma_prefetch_desc(&tm_dq16);
@@ -188,12 +187,12 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     for (int i = 0; i < 2; ++i) mbar_init(&qdo_full[i], 1);
     fence_mbar_init();
     mbar_expect_tx(&kv_full, 2 * M::kKV);
-    tma_load_head<HD, kAttnTile, QT>(sK, &tm_qkv, &tm_qkv16, &kv_full, D + h * HD, k0, b);
-    tma_load_head<HD, kAttnTile, QT>(sV, &tm_qkv, &tm_qkv16, &kv_full, 2 * D + h * HD, k0, b);
+    tma_load_head<HD, kAttnTile, QT>(sK, &tm_qkv, &tm_qkv16, &kv_full, p.H + h, k0, b);
+    tma_load_head<HD, kAttnTile, QT>(sV, &tm_qkv, &tm_qkv16, &kv_full, 2 * p.H + h, k0, b);
     for (int qi = 0; qi < 2 && qi < NQ; ++qi) {
       mbar_expect_tx(&qdo_full[qi], 2 * M::kQS);
-      tma_load_head<HD, QT, QT>(sQ + qi * M::kQS, &tm_qkv, &tm_qkv16, &qdo_full[qi], h * HD, qi * QT, b);
-      tma_load_head<HD, QT, QT>(sDO + qi * M::kQS, &tm_do, &tm_do16, &qdo_full[qi], h * HD, qi * QT, b);
+      tma_load_head<HD, QT, QT>(sQ + qi * M::kQS, &tm_qkv, &tm_qkv16, &qdo_full[qi], h, qi * QT, b);
+      tma_load_head<HD, QT, QT>(sDO + qi * M::kQS, &tm_do, &tm_do16, &qdo_full[qi], h, qi * QT, b);
     }
   }
 
@@ -245,11 +244,11 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
     for (int rr = 0; rr < 2; ++rr) row_masked[rr] = ((key_mask_s[(kr + 8 * rr) >> 5] >> ((kr + 8 * rr) & 31)) & 1u) != 0u;
     const bool flusher = (tid & 127) == 0;   // issues this WG's dQ reductions
     uint8_t* dq_stage = smem + kFW + w * kFDQ1;
-    const uint32_t ak = smem_u32(sK) + w * 8192, av = smem_u32(sV) + w * 8192;
+    const uint32_t ak = smem_u32(sK) + w * 8192, av = smem_u32(sV) + w * 8192;  // this WG's 64 rows of K, V
     uint32_t* wtile = reinterpret_cast<uint32_t*>(smem + kFW);
+    const uint32_t* kw_row = p.drop_mask + bh * (4 * N) * (N * kAttnTile) + k0 + kr;  // dropout words of key row kr, block 0
 
-    float dv_acc[kA], dk_acc[kA];  // written by the first tile's MMAs (scale_d = 0)
-    float dv16[8], dk16[8];        // their columns 64..79 (HD = 80 only)
+    HeadAcc<HD> dv_acc, dk_acc;  // written by the first tile's MMAs (scale_d = 0)
 
     // diagonal sums of the staged gate*dS tile of query tile qi.  Task (e, s): elements (key (ii + e) & 127, query ii) for
     // ii = 16 s .. 16 s + 15: diagonal key - query = e (not wrapped, ii + e < 128) or e - 128 (wrapped).  The wrap point is a
@@ -279,24 +278,12 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       mbar_wait(&qdo_full[st], (qi >> 1) & 1);
       const uint32_t bq = smem_u32(sQ + st * M::kQS), bdo = smem_u32(sDO + st * M::kQS);
       float s_acc[QT / 2], d_acc[QT / 2];
-      // S^T = K_w Q^T and dP^T = V_w dO^T over the head width (at HD = 80 the fifth k16 step reads the 32-byte blocks; at
-      // HD = 120 steps 4..7 read the second 64-column blocks)
-      auto scores = [&](float* acc, uint32_t a, uint32_t bt) {
-#pragma unroll
-        for (int k = 0; k < (HD == 120 ? 8 : 4); ++k) {
-          const uint64_t da = make_smem_desc_sw128(a + (k >> 2) * (kAttnTile * 128) + (k & 3) * 32, 16, 1024),
-                         db = make_smem_desc_sw128(bt + (k >> 2) * (QT * 128) + (k & 3) * 32, 16, 1024);
-          if (QT == 128) wgmma_m64n128k16<0, 0>(acc, da, db, k > 0 ? 1u : 0u);
-          else wgmma_m64n64k16<0, 0>(acc, da, db, k > 0 ? 1u : 0u);
-        }
-        if (HD == 80)
-          wgmma_m64n64k16<0, 0>(acc, make_smem_desc_sw32(a - w * 8192 + kAttnTile * 128 + w * 2048),
-                                make_smem_desc_sw32(bt + QT * 128), 1u);
-        wgmma_commit();
-      };
+      // S^T = K_w Q^T and dP^T = V_w dO^T over the head width
       wgmma_fence();
-      scores(s_acc, ak, bq);
-      scores(d_acc, av, bdo);
+      mma_k_head<HD, QT>(s_acc, ak, 64 * w, bq);
+      wgmma_commit();
+      mma_k_head<HD, QT>(d_acc, av, 64 * w, bdo);
+      wgmma_commit();
       // dropout keep words of this thread's two key rows for the tile's 32-query blocks
       uint32_t kw[2][QT / 32];
       if (DROP) {
@@ -304,7 +291,7 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
         for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
           for (int blk = 0; blk < QT / 32; ++blk)
-            kw[rr][blk] = p.drop_mask[(bh * (4 * N) + qi * (QT / 32) + blk) * (N * kAttnTile) + k0 + kr + 8 * rr];
+            kw[rr][blk] = kw_row[(qi * (QT / 32) + blk) * (N * kAttnTile) + 8 * rr];  // < 512 N^2: int below T = 262,016
       }
       // the previous tile's dQ reduction has read this WG's staging buffer before the buffer is written again
       if (qi > 0) {
@@ -398,28 +385,14 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
 
       // ---- dV += P^T dO (this WG's 64 keys; A = P^T from registers)
       wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < QT / 16; ++k) {  // K = the tile's queries, 16 per step
-        if (HD == 120)
-          wgmma_m64n128k16_rs<1>(dv_acc, p16 + 4 * k, make_smem_desc_sw128(bdo + k * 2048, QT * 128, 1024), (qi > 0 || k > 0) ? 1u : 0u);
-        else
-          wgmma_m64n64k16_rs<1>(dv_acc, p16 + 4 * k, make_smem_desc_sw128(bdo + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
-        if (HD == 80)
-          wgmma_m64n16k16_rs<1>(dv16, p16 + 4 * k, make_smem_desc_sw32(bdo + QT * 128 + k * 512), (qi > 0 || k > 0) ? 1u : 0u);
-      }
+      mma_n_head<HD, QT>(dv_acc, p16, bdo, qi > 0);  // K = the tile's queries
       wgmma_commit();
       fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
       named_bar_sync(1, kFThreads);
 
       // ---- dK += dS^T Q (this WG's 64 keys; A = its rows of the dS^T tile, K-major).  From shared memory rather than registers:
       // 32 more live registers through the dS^T pass would spill.
-#pragma unroll
-      for (int k = 0; k < QT / 16; ++k) {
-        const uint64_t da = make_smem_desc_sw128(smem_u32(sDS) + (k >> 2) * 16384 + w * 8192 + (k & 3) * 32, 16, 1024);
-        if (HD == 120) wgmma_m64n128k16<0, 1>(dk_acc, da, make_smem_desc_sw128(bq + k * 2048, QT * 128, 1024), (qi > 0 || k > 0) ? 1u : 0u);
-        else wgmma_m64n64k16<0, 1>(dk_acc, da, make_smem_desc_sw128(bq + k * 2048, 8192, 1024), (qi > 0 || k > 0) ? 1u : 0u);
-        if (HD == 80) wgmma_m64n16k16<0, 1>(dk16, da, make_smem_desc_sw32(bq + QT * 128 + k * 512), (qi > 0 || k > 0) ? 1u : 0u);
-      }
+      mma_n_head<HD, QT>(dk_acc, smem_u32(sDS), 64 * w, bq, qi > 0);
       // ---- dQ = dS K.  HD 64: this WG's 64 queries, K = 128 keys.  HD 80: the tile's 64 queries, K = this WG's 64 keys (the two
       // WGs' shares are added by the reductions).  HD 120: the tile's 64 queries x this WG's 64 columns, K = 128 keys.  A = the
       // dS^T tile read MN-major, 16 keys per step.
@@ -469,8 +442,8 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       named_bar_sync(1, kFThreads);  // the Q / dO stage, the staging, dS^T and d gate tiles of this query tile are consumed
       if (tid == 0 && qi + 2 < NQ) {
         mbar_expect_tx(&qdo_full[st], 2 * M::kQS);
-        tma_load_head<HD, QT, QT>(sQ + st * M::kQS, &tm_qkv, &tm_qkv16, &qdo_full[st], h * HD, (qi + 2) * QT, b);
-        tma_load_head<HD, QT, QT>(sDO + st * M::kQS, &tm_do, &tm_do16, &qdo_full[st], h * HD, (qi + 2) * QT, b);
+        tma_load_head<HD, QT, QT>(sQ + st * M::kQS, &tm_qkv, &tm_qkv16, &qdo_full[st], h, (qi + 2) * QT, b);
+        tma_load_head<HD, QT, QT>(sDO + st * M::kQS, &tm_do, &tm_do16, &qdo_full[st], h, (qi + 2) * QT, b);
       }
 
       // dQ rows of this WG -> the staging boxes ([64 queries][32 fp32], SWIZZLE_128B, and at HD = 80 [64][16] fp32 behind
@@ -497,14 +470,11 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       fence_proxy_async_smem();
       named_bar_sync(2 + w, 128);
       const int dq_row = QT == kAttnTile ? qi * kAttnTile + 64 * w : qi * QT;
-      if (HD == 120 && flusher && dq_row < T) {  // head-shaped map: (column in the head, head, row, batch); the box at 96 clips
-        tma_reduce_add_4d(&tm_dq, smem_u32(dq_stage), 64 * w, h, dq_row, b);
-        tma_reduce_add_4d(&tm_dq, smem_u32(dq_stage) + 8192, 64 * w + 32, h, dq_row, b);
-        bulk_commit();
-      } else if (flusher && dq_row < T) {
-        tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage), h * HD, dq_row, b);
-        tma_reduce_add_3d(&tm_dq, smem_u32(dq_stage) + 8192, h * HD + 32, dq_row, b);
-        if (HD == 80) tma_reduce_add_3d(&tm_dq16, smem_u32(dq_stage) + 16384, h * HD + 64, dq_row, b);
+      if (flusher && dq_row < T) {
+        const int dq_col = HD == 120 ? 64 * w : 0;
+        tma_reduce_add_4d(&tm_dq, smem_u32(dq_stage), dq_col, h, dq_row, b);
+        tma_reduce_add_4d(&tm_dq, smem_u32(dq_stage) + 8192, dq_col + 32, h, dq_row, b);
+        if (HD == 80) tma_reduce_add_4d(&tm_dq16, smem_u32(dq_stage) + 16384, 64, h, dq_row, b);
         bulk_commit();
       }
       if (HAS_BIAS && tid >= kAttnTile) {
@@ -525,20 +495,8 @@ __global__ void __launch_bounds__(kFThreads, 1) attn_bwd_fused_kernel(const __gr
       const int key = k0 + kr + 8 * rr;
       if (key < T) {
         __nv_bfloat16* dst = p.dqkv + (static_cast<long long>(b) * T + key) * (3 * D) + h * HD + fc;
-        const float rp = DROP ? p.drop_rp : 1.0f;   // dV = (P o M)^T dO / (1-p)
-#pragma unroll
-        for (int g = 0; g < kA / 4; ++g) {
-          if (8 * g >= HD) continue;  // HD 120: columns 120..127 belong to the next head (or the next section)
-          *reinterpret_cast<uint32_t*>(dst + 2 * D + 8 * g) = pack_bf16x2(dv_acc[4 * g + 2 * rr] * rp, dv_acc[4 * g + 2 * rr + 1] * rp);
-          *reinterpret_cast<uint32_t*>(dst + D + 8 * g) = pack_bf16x2(dk_acc[4 * g + 2 * rr], dk_acc[4 * g + 2 * rr + 1]);
-        }
-        if (HD == 80) {
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            *reinterpret_cast<uint32_t*>(dst + 2 * D + 64 + 8 * g) = pack_bf16x2(dv16[4 * g + 2 * rr] * rp, dv16[4 * g + 2 * rr + 1] * rp);
-            *reinterpret_cast<uint32_t*>(dst + D + 64 + 8 * g) = pack_bf16x2(dk16[4 * g + 2 * rr], dk16[4 * g + 2 * rr + 1]);
-          }
-        }
+        dv_acc.store_row(dst + 2 * D, rr, DROP ? p.drop_rp : 1.0f);  // dV = (P o M)^T dO / (1-p)
+        dk_acc.store_row(dst + D, rr, 1.0f);
       }
     }
   }
@@ -600,12 +558,6 @@ __global__ void __launch_bounds__(256) attn_dq_convert_kernel(float* __restrict_
   }
 }
 
-int make_qkv_tmap(CUtensorMap* out, const void* qkv, int T, int B, int D3, int box_cols, int box_rows);
-int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_cols, int box_rows);
-int make_head_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int hd, int box_rows);
-int make_f32_head_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int hd, int box_rows);
-
-
 // Delta pre-kernel, the fused kernel and the dQ conversion on one stream (see the entry points below for the contract).
 static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, const float* gate, const float* tab,
                            const uint8_t* key_pad, const float* lse, float* delta, float* dq_acc, void* dqkv, float* dgate,
@@ -613,31 +565,17 @@ static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, c
                            int head_dim, cudaStream_t st) {
   const int D = H * head_dim;
   const long long rows = static_cast<long long>(B) * T;
-  B200_CHECK_CUDA(launch_pdl(head_dim == 120 ? attn_delta2_kernel<120> : head_dim == 80 ? attn_delta2_kernel<80> : attn_delta2_kernel<64>, dim3(static_cast<unsigned>(ceil_div_ll(rows * 32, 256))), dim3(256), 0, st,
-      static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), B, T, H, delta,
-      tab != nullptr ? dgate : nullptr));
-  B200_CHECK_LAUNCH();
-
   CUtensorMap tm_qkv, tm_do, tm_dq, tm_qkv16, tm_do16, tm_dq16;
   const int box_rows = head_dim == 64 ? kAttnTile : BwdMap<80>::kQT;
-  if (head_dim == 120) {
-    if (make_head_tmap(&tm_qkv, qkv, T, B, 3 * D, 120, box_rows)) return -3;
-    if (make_head_tmap(&tm_do, dout, T, B, D, 120, box_rows)) return -3;
-    if (make_f32_head_tmap(&tm_dq, dq_acc, T, B, D, 120, 64)) return -3;
-  } else {
-    if (make_qkv_tmap(&tm_qkv, qkv, T, B, 3 * D, 64, box_rows)) return -3;
-    if (make_qkv_tmap(&tm_do, dout, T, B, D, 64, box_rows)) return -3;
-    if (make_f32_rows_tmap(&tm_dq, dq_acc, T, B, D, 32, 64)) return -3;
-  }
-  if (head_dim == 80) {
-    if (make_qkv_tmap(&tm_qkv16, qkv, T, B, 3 * D, 16, box_rows)) return -3;
-    if (make_qkv_tmap(&tm_do16, dout, T, B, D, 16, box_rows)) return -3;
-    if (make_f32_rows_tmap(&tm_dq16, dq_acc, T, B, D, 16, 64)) return -3;
-  } else {  // not read
-    tm_qkv16 = tm_qkv;
-    tm_do16 = tm_do;
-    tm_dq16 = tm_dq;
-  }
+  if (make_operand_tmaps(&tm_qkv, &tm_qkv16, qkv, T, B, 3 * D, head_dim, box_rows)) return -3;
+  if (make_operand_tmaps(&tm_do, &tm_do16, dout, T, B, D, head_dim, box_rows)) return -3;
+  // dQ reductions: [64 queries][32 columns] boxes (one 128-byte swizzle row), and at width 80 [64][16] unswizzled
+  if (make_head_tmap(&tm_dq, dq_acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, T, B, D, head_dim, 32, 64, CU_TENSOR_MAP_SWIZZLE_128B))
+    return -3;
+  tm_dq16 = tm_dq;
+  if (head_dim == 80 &&
+      make_head_tmap(&tm_dq16, dq_acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, T, B, D, head_dim, 16, 64, CU_TENSOR_MAP_SWIZZLE_NONE))
+    return -3;
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.T = T; p.H = H; p.B = B; p.D = D;
@@ -653,18 +591,20 @@ static int attn_bwd_launch(const void* qkv, const void* out, const void* dout, c
   const bool drop = drop_p > 0.f;
   p.drop_mask = const_cast<uint32_t*>(drop_mask);
   p.drop_rp = 1.0f / (1.0f - drop_p);
-  const int N = p.n_tiles;
-  const int smem = head_dim == 64 ? BwdMap<64>::kFSmem : head_dim == 80 ? BwdMap<80>::kFSmem : BwdMap<120>::kFSmem;
-  dim3 grid(N, H, B);
-  void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
-               const AttnParams) =
-      head_dim == 120 ? (drop ? attn_bwd_fused_kernel<120, false, true> : attn_bwd_fused_kernel<120, false, false>)
-      : head_dim == 80 ? (drop ? attn_bwd_fused_kernel<80, false, true> : attn_bwd_fused_kernel<80, false, false>)
-      : tab != nullptr ? (drop ? attn_bwd_fused_kernel<64, true, true> : attn_bwd_fused_kernel<64, true, false>)
-                       : (drop ? attn_bwd_fused_kernel<64, false, true> : attn_bwd_fused_kernel<64, false, false>);
-  B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFThreads), smem, st, tm_qkv, tm_do, tm_dq, tm_qkv16, tm_do16, tm_dq16, p));
-  B200_CHECK_LAUNCH();
+  const int rc = attn_dispatch(head_dim, tab != nullptr, drop, [&](auto hd, auto bias, auto dp) {
+    B200_CHECK_CUDA(launch_pdl(attn_delta2_kernel<hd>, dim3(static_cast<unsigned>(ceil_div_ll(rows * 32, 256))), dim3(256), 0,
+                               st, static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), B, T, H,
+                               delta, tab != nullptr ? dgate : nullptr));
+    B200_CHECK_LAUNCH();
+    const auto kern = attn_bwd_fused_kernel<hd, bias, dp>;
+    constexpr int smem = BwdMap<hd>::kFSmem;
+    B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    B200_CHECK_CUDA(launch_pdl(kern, dim3(p.n_tiles, H, B), dim3(kFThreads), smem, st, tm_qkv, tm_do, tm_dq, tm_qkv16, tm_do16,
+                               tm_dq16, p));
+    B200_CHECK_LAUNCH();
+    return 0;
+  });
+  if (rc) return rc;
   const long long nvec = rows * (D / 8);
   const int blocks = static_cast<int>(std::min<long long>(ceil_div_ll(nvec, 256), static_cast<long long>(sm_count()) * 16));
   B200_CHECK_CUDA(launch_pdl(attn_dq_convert_kernel, dim3(blocks), dim3(256), 0, st, dq_acc, static_cast<__nv_bfloat16*>(dqkv), rows, D));
@@ -686,9 +626,7 @@ int b200s_attn_bwd(const void* qkv, const void* out, const void* dout, const flo
                    const uint8_t* key_pad, const float* lse, float* delta, void* dqkv, float* dgate, float* dtab, int B,
                    int T, int H, float scale, int head_dim, b200s_stream stream) {
   B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv, "attn_bwd: null pointer");
-  B200_CHECK_ARG(head_dim == 64 || head_dim == 80 || head_dim == 120, "attn_bwd: head_dim=%d is not supported (64, 80 or 120)",
-                 head_dim);
-  B200_CHECK_ARG(head_dim == 64 || tab == nullptr, "attn_bwd: the relative-position bias needs head_dim 64 (got %d)", head_dim);
+  if (const int rc = attn_check_head("attn_bwd", head_dim, tab != nullptr)) return rc;
   B200_CHECK_ARG(T >= 1, "attn_bwd: T=%d out of range", T);
   B200_CHECK_ARG(!tab || (dgate && dtab), "attn_bwd: bias given but dgate/dtab missing");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -709,10 +647,7 @@ int b200s_attn_bwd_fused_dropout(const void* qkv, const void* out, const void* d
                                  float* dgate, float* dtab, int B, int T, int H, float scale, float drop_p,
                                  const uint32_t* drop_mask, int head_dim, b200s_stream stream) {
   B200_CHECK_ARG(qkv && out && dout && lse && delta && dqkv && dq_acc, "attn_bwd_fused: null pointer");
-  B200_CHECK_ARG(head_dim == 64 || head_dim == 80 || head_dim == 120, "attn_bwd_fused: head_dim=%d is not supported (64, 80 or 120)",
-                 head_dim);
-  B200_CHECK_ARG(head_dim == 64 || tab == nullptr, "attn_bwd_fused: the relative-position bias needs head_dim 64 (got %d)",
-                 head_dim);
+  if (const int rc = attn_check_head("attn_bwd_fused", head_dim, tab != nullptr)) return rc;
   B200_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f, "attn_bwd_fused: dropout p=%f out of range [0,1)", static_cast<double>(drop_p));
   B200_CHECK_ARG(drop_p == 0.f || drop_mask != nullptr, "attn_bwd_fused: dropout needs the mask written by b200s_attn_fwd_dropout");
   B200_CHECK_ARG(T >= 1, "attn_bwd_fused: T=%d out of range", T);

@@ -28,10 +28,8 @@
 // few MB and stays in L2.
 // Dropout: the keep bits of a column pair are one hash word; a warp holds 16 consecutive query rows, i.e. one 16-bit half of
 // each mask word, which it assembles from ballots and stores as u16 (no cross-warp merge).
-// Head width HD = 64 or 80 (attn_common.cuh): at 80 a tile is 20 KB instead of 16, S = Q K^T takes a fifth k16 step on the
-// SWIZZLE_32B blocks and O += P V an n16 wgmma next to the n64 one, so O is 40 fp32 registers per thread instead of 32.
-// At HD = 120 a tile is two 64-column blocks (32 KB, zero tail), S takes eight k16 steps and O += P V is one n128 wgmma, so O
-// is 64 fp32 registers per thread (columns 120..127 are zero and never stored).
+// Head width HD = 64, 80 or 120: tiles, maps and MMA shapes per width are in attn_common.cuh (HeadTile).  A tile is 16, 20 or
+// 32 KB and O is 32, 40 or 64 fp32 registers per thread (at 120 columns 120..127 are zero and never stored).
 // Shared memory: 5 tiles of Q / K / V rings (81920 B at HD 64, 102400 B at 80, 163840 B at 120) + 2 x 2704 B of stages
 // + 1024 B alignment = 88352 B (HD 64), 108832 B (HD 80) or 170272 B (HD 120) for every T.
 #include "../../include/unispeech_b200.h"
@@ -64,7 +62,7 @@ constexpr int kStageFloats = kMaskOff + kAttnTile + 4;
 // rings, then the two per-key-tile stages (bias copies, key mask, flag)
 template <int HD>
 struct FwdMap {
-  static constexpr int kTile = kAttnTile * attn_tile_cols<HD>() * 2;  // one [128][HD] bf16 tile
+  static constexpr int kTile = kAttnTile * HeadTile<HD>::kCols * 2;  // one [128][HD] bf16 tile
   static constexpr int kQ = 0, kK = kTile, kV = 3 * kTile, kStage = 5 * kTile;
   static constexpr int kSmem = kStage + 2 * kStageFloats * 4 + 1024;  // (+ 1024 for the alignment of the base)
 };
@@ -74,9 +72,9 @@ template <int HD, bool HAS_BIAS, bool DROP>
 __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_constant__ CUtensorMap tm,
                                                                  const __grid_constant__ CUtensorMap tm16,
                                                                  const __grid_constant__ AttnParams p) {
-  static_assert(HD == 64 || ((HD == 80 || HD == 120) && !HAS_BIAS), "head width 64, or 80 / 120 without the relative-position bias");
+  using HT = HeadTile<HD>;
+  static_assert(HT::kBias || !HAS_BIAS, "the relative-position bias at this head width");
   using M = FwdMap<HD>;
-  constexpr int kO = HD == 120 ? 64 : 32;  // O accumulator registers of the first (or only) wgmma
   pdl_grid_sync();
   const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
   const int q0 = blockIdx.x * kAttnTile, h = blockIdx.y, b = blockIdx.z;
@@ -123,18 +121,18 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
   auto load_k = [&](int n) {
     const int s = n & 1;
     mbar_expect_tx(&k_full[s], M::kTile);
-    tma_load_head<HD, kAttnTile, kAttnTile>(smem + M::kK + s * M::kTile, &tm, &tm16, &k_full[s], D + h * HD, n * kAttnTile, b);
+    tma_load_head<HD, kAttnTile, kAttnTile>(smem + M::kK + s * M::kTile, &tm, &tm16, &k_full[s], p.H + h, n * kAttnTile, b);
   };
   auto load_v = [&](int n) {
     const int s = n & 1;
     mbar_expect_tx(&v_full[s], M::kTile);
-    tma_load_head<HD, kAttnTile, kAttnTile>(smem + M::kV + s * M::kTile, &tm, &tm16, &v_full[s], 2 * D + h * HD, n * kAttnTile, b);
+    tma_load_head<HD, kAttnTile, kAttnTile>(smem + M::kV + s * M::kTile, &tm, &tm16, &v_full[s], 2 * p.H + h, n * kAttnTile, b);
   };
   if (tid == 0) {
     // the TMA thread initialises the barriers and puts Q and the first two K / V tiles in flight right away (the other warps
     // see the barriers after the __syncthreads below)
     tma_prefetch_desc(&tm);
-    if (HD == 80) tma_prefetch_desc(&tm16);
+    if (HT::kTail) tma_prefetch_desc(&tm16);
     mbar_init(&q_full, 1);
 #pragma unroll
     for (int s = 0; s < 2; ++s) {
@@ -146,7 +144,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
     }
     fence_mbar_init();
     mbar_expect_tx(&q_full, M::kTile);
-    tma_load_head<HD, kAttnTile, kAttnTile>(sQ, &tm, &tm16, &q_full, h * HD, q0, b);
+    tma_load_head<HD, kAttnTile, kAttnTile>(sQ, &tm, &tm16, &q_full, h, q0, b);
     for (int n = 0; n < 2 && n < n_eff; ++n) {
       load_k(n);
       load_v(n);
@@ -235,14 +233,10 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
                                                            (N * kAttnTile)) + ((row16 >> 4) & 1);
   }
 
-  float o[kO];   // O rows r0, r0 + 8 x columns 0..63 (0..127 at HD = 120), fragment layout
-  float o16[8];  // ... x columns 64..79 (HD = 80 only)
-#pragma unroll
-  for (int i = 0; i < kO; ++i) o[i] = 0.f;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) o16[i] = 0.f;
+  HeadAcc<HD> o;  // O rows r0, r0 + 8
+  o.zero();
   float m_ref[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-  const uint32_t aQ = smem_u32(sQ) + 8192 * c;
+  const uint32_t aQ = smem_u32(sQ) + 8192 * c;  // this consumer's 64 rows of Q
 
   // ping-pong: consumer c issues its S MMAs after syncing on barrier 1 + c, then arrives on the other's barrier 2 - c, so
   // that one warpgroup's softmax runs while the other's MMAs hold the tensor pipe
@@ -258,13 +252,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
     const uint32_t bK = smem_u32(smem + M::kK + s * M::kTile);
     auto qk = [&]() {  // S = Q K_n^T
       wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < (HD == 120 ? 8 : 4); ++k)  // HD 120: k = 4..7 on the second block (16384 B on), its tail zero
-        wgmma_m64n128k16<0, 0>(acc, make_smem_desc_sw128(aQ + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
-                               make_smem_desc_sw128(bK + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024), k > 0 ? 1u : 0u);
-      if (HD == 80)  // columns 64..79: the 32-byte blocks behind the 128-row tiles
-        wgmma_m64n128k16<0, 0>(acc, make_smem_desc_sw32(smem_u32(sQ) + kAttnTile * 128 + 2048 * c),
-                               make_smem_desc_sw32(bK + kAttnTile * 128), 1u);
+      mma_k_head<HD, kAttnTile>(acc, aQ, 64 * c, bK);
       wgmma_commit();
     };
     qk();
@@ -377,16 +365,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
         const float factor = (m_ref[rr] == -INFINITY) ? 0.f : fast_exp2(m_ref[rr] - m_new);
         l_run[rr] *= factor;
         m_ref[rr] = m_new;
-#pragma unroll
-        for (int g = 0; g < kO / 4; ++g) {
-          o[4 * g + 2 * rr] *= factor;
-          o[4 * g + 2 * rr + 1] *= factor;
-        }
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          o16[4 * g + 2 * rr] *= factor;
-          o16[4 * g + 2 * rr + 1] *= factor;
-        }
+        o.scale_row(rr, factor);
       }
     }
     if (lane == 0) mbar_arrive(&k_empty[s]);
@@ -397,12 +376,7 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
     mbar_wait(&v_full[s], (n >> 1) & 1);
     const uint32_t bV = smem_u32(smem + M::kV + s * M::kTile);
     wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      if (HD == 120) wgmma_m64n128k16_rs<1>(o, pk + 4 * k, make_smem_desc_sw128(bV + k * 2048, 16384, 1024), 1u);
-      else wgmma_m64n64k16_rs<1>(o, pk + 4 * k, make_smem_desc_sw128(bV + k * 2048, 8192, 1024), 1u);
-      if (HD == 80) wgmma_m64n16k16_rs<1>(o16, pk + 4 * k, make_smem_desc_sw32(bV + kAttnTile * 128 + k * 512), 1u);
-    }
+    mma_n_head<HD, kAttnTile>(o, pk, bV, true);
     wgmma_commit();
     wgmma_wait<0>();
     if (lane == 0) mbar_arrive(&v_empty[s]);
@@ -419,21 +393,10 @@ __global__ void __launch_bounds__(kFwdThreads, 1) attn_fwd_kernel(const __grid_c
       if (p.lse != nullptr && quad == 0)
         p.lse[(static_cast<long long>(b) * p.H + h) * T + row] = (l > 0.f) ? (m_ref[rr] + log2f(l)) : INFINITY;
       const float inv = l > 0.f ? (DROP ? p.drop_rp : 1.0f) / l : 0.f;
-      __nv_bfloat16* dst = p.out + (static_cast<long long>(b) * T + row) * D + h * HD + 2 * quad;
-#pragma unroll
-      for (int g = 0; g < kO / 4; ++g)  // (HD 120: group 15, columns 120..127, belongs to the next head)
-        if (8 * g < HD) *reinterpret_cast<uint32_t*>(dst + 8 * g) = pack_bf16x2(o[4 * g + 2 * rr] * inv, o[4 * g + 2 * rr + 1] * inv);
-      if (HD == 80) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g)
-          *reinterpret_cast<uint32_t*>(dst + 64 + 8 * g) = pack_bf16x2(o16[4 * g + 2 * rr] * inv, o16[4 * g + 2 * rr + 1] * inv);
-      }
+      o.store_row(p.out + (static_cast<long long>(b) * T + row) * D + h * HD + 2 * quad, rr, inv);
     }
   }
 }
-
-int make_qkv_tmap(CUtensorMap* out, const void* qkv, int T, int B, int D3, int box_cols, int box_rows);
-int make_head_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int hd, int box_rows);
 
 }  // namespace b200
 
@@ -450,9 +413,7 @@ int b200s_attn_fwd_dropout(const void* qkv, const float* gate, const float* tab,
                            int B, int T, int H, float scale, float drop_p, uint32_t key0, uint32_t key1, uint32_t* drop_mask,
                            int head_dim, b200s_stream stream) {
   B200_CHECK_ARG(qkv && out, "attn_fwd: null pointer");
-  B200_CHECK_ARG(head_dim == 64 || head_dim == 80 || head_dim == 120, "attn_fwd: head_dim=%d is not supported (64, 80 or 120)",
-                 head_dim);
-  B200_CHECK_ARG(head_dim == 64 || tab == nullptr, "attn_fwd: the relative-position bias needs head_dim 64 (got %d)", head_dim);
+  if (const int rc = attn_check_head("attn_fwd", head_dim, tab != nullptr)) return rc;
   B200_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f, "attn_fwd: dropout p=%f out of range [0,1)", static_cast<double>(drop_p));
   B200_CHECK_ARG(drop_p == 0.f || drop_mask != nullptr, "attn_fwd: dropout needs the mask buffer (b200s_attn_dropout_mask_words)");
   B200_CHECK_ARG(static_cast<long long>(B) * H * T < (1LL << 32), "attn_fwd: B*H*T exceeds the 32-bit dropout row counter");
@@ -463,17 +424,7 @@ int b200s_attn_fwd_dropout(const void* qkv, const float* gate, const float* tab,
   p.T = T; p.H = H; p.B = B; p.D = D;
   p.n_tiles = ceil_div(T, kAttnTile);
   B200_CHECK_ARG(T >= 1, "attn_fwd: T=%d out of range", T);
-  const int smem = head_dim == 64 ? FwdMap<64>::kSmem : head_dim == 80 ? FwdMap<80>::kSmem : FwdMap<120>::kSmem;
-  if (head_dim == 120) {
-    if (make_head_tmap(&tm, qkv, T, B, 3 * D, 120, kAttnTile)) return -3;
-  } else if (make_qkv_tmap(&tm, qkv, T, B, 3 * D, 64, kAttnTile)) {
-    return -3;
-  }
-  if (head_dim == 80) {
-    if (make_qkv_tmap(&tm16, qkv, T, B, 3 * D, 16, kAttnTile)) return -3;
-  } else {
-    tm16 = tm;  // not read
-  }
+  if (make_operand_tmaps(&tm, &tm16, qkv, T, B, 3 * D, head_dim, kAttnTile)) return -3;
   p.scale = scale;
   p.gate = gate; p.tab = tab; p.key_pad = key_pad;
   p.out = static_cast<__nv_bfloat16*>(out);
@@ -485,15 +436,14 @@ int b200s_attn_fwd_dropout(const void* qkv, const float* gate, const float* tab,
   p.drop_rp = 1.0f / (1.0f - drop_p);
   dim3 grid(ceil_div(T, kAttnTile), H, B);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  void (*kern)(const CUtensorMap, const CUtensorMap, const AttnParams) =
-      head_dim == 120 ? (drop ? attn_fwd_kernel<120, false, true> : attn_fwd_kernel<120, false, false>)
-      : head_dim == 80 ? (drop ? attn_fwd_kernel<80, false, true> : attn_fwd_kernel<80, false, false>)
-      : tab != nullptr ? (drop ? attn_fwd_kernel<64, true, true> : attn_fwd_kernel<64, true, false>)
-                       : (drop ? attn_fwd_kernel<64, false, true> : attn_fwd_kernel<64, false, false>);
-  B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFwdThreads), smem, st, tm, tm16, p));
-  B200_CHECK_LAUNCH();
-  return 0;
+  return attn_dispatch(head_dim, tab != nullptr, drop, [&](auto hd, auto bias, auto dp) {
+    const auto kern = attn_fwd_kernel<hd, bias, dp>;
+    constexpr int smem = FwdMap<hd>::kSmem;
+    B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    B200_CHECK_CUDA(launch_pdl(kern, grid, dim3(kFwdThreads), smem, st, tm, tm16, p));
+    B200_CHECK_LAUNCH();
+    return 0;
+  });
 }
 
 int b200s_attn_fwd(const void* qkv, const float* gate, const float* tab, const uint8_t* key_pad, void* out, float* lse,

@@ -53,16 +53,20 @@ struct ViewSpec {
   long long dims[4];     // elements; dims[0] contiguous
   long long strides[3];  // elements, for dims 1..3
   int box[4];
+  CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B;
 };
 
-// bf16, zero OOB fill, 256-byte L2 promotion; 128B swizzle, or 32B for a box of 16 columns (the last 16 columns of an 80-wide
-// attention head).  Returns 0 on success.
+// bf16 or fp32, zero OOB fill; bf16 maps (MMA operands) promote 256-byte L2 lines, fp32 maps (reduction destinations) none.
+// Returns 0 on success.
 static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
     set_last_error("cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
     return -3;
   }
+  const bool f32 = v.dtype == CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const long long esize = f32 ? 4 : 2;
   cuuint64_t dims[4];
   cuuint64_t strides[3];
   cuuint32_t box[4];
@@ -73,20 +77,19 @@ static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
   }
   for (int i = 0; i < 3; ++i) {
     long long s = v.strides[i];
-    if (s <= 0) s = (i == 0 ? v.dims[0] : static_cast<long long>(strides[i - 1] / 2) * v.dims[i]);
-    if (s % 8 != 0) {
-      set_last_error("tensor map stride %lld (dim %d) is not a multiple of 8 elements", s, i + 1);
+    if (s <= 0) s = (i == 0 ? v.dims[0] : static_cast<long long>(strides[i - 1] / esize) * v.dims[i]);
+    if (s * esize % 16 != 0) {
+      set_last_error("tensor map stride %lld (dim %d) is not a multiple of 16 bytes", s, i + 1);
       return -1;
     }
-    strides[i] = static_cast<cuuint64_t>(s) * 2;
+    strides[i] = static_cast<cuuint64_t>(s * esize);
   }
   if ((reinterpret_cast<uintptr_t>(v.ptr) & 15) != 0) {
     set_last_error("tensor map base pointer %p is not 16-byte aligned", v.ptr);
     return -1;
   }
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(v.ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, v.box[0] == 16 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = fn(out, v.dtype, 4, const_cast<void*>(v.ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, v.swizzle,
+                  f32 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled failed (%d): dims {%lld,%lld,%lld,%lld} strides {%lld,%lld,%lld} box {%d,%d,%d,%d}",
                    static_cast<int>(r), v.dims[0], v.dims[1], v.dims[2], v.dims[3], v.strides[0], v.strides[1],
@@ -96,18 +99,13 @@ static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
   return 0;
 }
 
-// [B, T, cols] bf16 row-major activations: box = box_cols (64, SWIZZLE_128B, or 16, SWIZZLE_32B) columns x box_rows rows
-// (used by the attention kernels)
-int make_qkv_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int box_cols, int box_rows) {
-  ViewSpec v{ptr, {cols, T, B, 1}, {cols, static_cast<long long>(T) * cols, 0}, {box_cols, box_rows, 1, 1}};
-  return make_tmap(out, v);
-}
-
-// [B, T, cols] bf16 seen as [B, T, cols / hd heads, hd] (innermost dimension = one attention head): box = 64 columns of one
-// head x box_rows rows.  A box that starts at column 64 of a 120-wide head gets zeros for columns 120..127 instead of the
-// next head's columns (used by the attention kernels at head width 120)
-int make_head_tmap(CUtensorMap* out, const void* ptr, int T, int B, int cols, int hd, int box_rows) {
-  ViewSpec v{ptr, {hd, cols / hd, T, B}, {hd, cols, static_cast<long long>(T) * cols}, {64, 1, box_rows, 1}};
+// [B, T, cols] bf16 or fp32 row-major seen as [B, T, cols / hd heads, hd] (innermost dimension = one attention head): box =
+// box_cols columns of one head x box_rows rows, addressed by (column in the head, head slot, row, batch).  A load box that
+// reaches past the head's last column gets zeros there, and a reduction box is clipped there (and at T), so no column of a
+// neighbouring head is read or written (the attention kernels' operands and dQ accumulator).
+int make_head_tmap(CUtensorMap* out, const void* ptr, CUtensorMapDataType dtype, int T, int B, int cols, int hd, int box_cols,
+                   int box_rows, CUtensorMapSwizzle swizzle) {
+  ViewSpec v{ptr, {hd, cols / hd, T, B}, {hd, cols, static_cast<long long>(T) * cols}, {box_cols, 1, box_rows, 1}, dtype, swizzle};
   return make_tmap(out, v);
 }
 
@@ -116,55 +114,6 @@ int make_rows_tmap(CUtensorMap* out, const void* ptr, long long cols, long long 
                    long long batch_stride, int box_rows) {
   ViewSpec v{ptr, {cols, rows, batches, 1}, {row_stride, batches > 1 ? batch_stride : 0, 0}, {64, box_rows, 1, 1}};
   return make_tmap(out, v);
-}
-
-// [B, T, cols] fp32 row-major (the attention backward's dQ accumulator): rank 3 (cols, T, B), so a box clips at T inside each
-// utterance; box = 32 columns (one 128-byte swizzle row) or 16 columns (64-byte rows, not swizzled) x box_rows rows.  Used as
-// the destination of TMA reductions.
-int make_f32_rows_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int box_cols, int box_rows) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) {
-    set_last_error("cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
-    return -3;
-  }
-  const cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(T), static_cast<cuuint64_t>(B)};
-  const cuuint64_t strides[2] = {static_cast<cuuint64_t>(cols) * 4, static_cast<cuuint64_t>(T) * cols * 4};
-  const cuuint32_t box[3] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows), 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled failed (%d) for the fp32 [%d, %d, %d] map", static_cast<int>(r), B, T, cols);
-    return -3;
-  }
-  return 0;
-}
-
-// [B, T, cols] fp32 seen as [B, T, cols / hd heads, hd] (the attention backward's dQ accumulator at head width 120): box = 32
-// columns of one head (SWIZZLE_128B) x box_rows rows.  As a TMA reduction destination the box clips at the head's last column
-// and at T, so the columns of the next head are never written.
-int make_f32_head_tmap(CUtensorMap* out, const float* ptr, int T, int B, int cols, int hd, int box_rows) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) {
-    set_last_error("cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
-    return -3;
-  }
-  const cuuint64_t dims[4] = {static_cast<cuuint64_t>(hd), static_cast<cuuint64_t>(cols / hd), static_cast<cuuint64_t>(T),
-                              static_cast<cuuint64_t>(B)};
-  const cuuint64_t strides[3] = {static_cast<cuuint64_t>(hd) * 4, static_cast<cuuint64_t>(cols) * 4,
-                                 static_cast<cuuint64_t>(T) * cols * 4};
-  const cuuint32_t box[4] = {32, 1, static_cast<cuuint32_t>(box_rows), 1};
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled failed (%d) for the fp32 head map [%d, %d, %d / %d, %d]", static_cast<int>(r), B, T,
-                   cols, hd, hd);
-    return -3;
-  }
-  return 0;
 }
 
 // ------------------------------------------------------------------ launch

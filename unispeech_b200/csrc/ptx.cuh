@@ -95,14 +95,7 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
 }
 
 // TMA element-wise fp32 add of one shared-memory box into global memory (bulk async-group completion; the data type comes
-// from the rank-3 tensor map); coordinates beyond the tensor bounds are clipped
-__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2) {
-  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-// the same for a rank-4 map (the attention backward's head-shaped dQ map at head width 120)
+// from the rank-4 tensor map); coordinates beyond the tensor bounds are clipped
 __device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2, int c3) {
   asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(m)),
