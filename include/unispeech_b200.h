@@ -475,6 +475,19 @@ int b200s_mix_apply(const float* src, long long bs, int B, int L, const void* pl
 int b200s_row_normalize(float* x, long long bs, int B, int L, const int* valid_len, double* stats, const void* plan,
                         b200s_stream stream);
 
+/* ============================ MFCC features of HuBERT's first iteration (csrc/mfcc.cu) ============================ */
+/* torchaudio.compliance.kaldi.mfcc(wav, sample_frequency=16000, use_energy=False) with every other argument at its default,
+ * then compute_deltas twice (win_length 5, replicate padding): 13 cepstra, 13 deltas, 13 delta-deltas per 10 ms frame, fp32.
+ * wav: fp32 [B, L] (batch stride wav_bs >= L).  n_samples: int32 [B] device, valid samples per utterance, clamped to [0, L];
+ * utterance b has Tm_b = 1 + (n - 400) / 160 frames when n >= 400, else none; frame t covers samples [160 t, 160 t + 400).
+ * Deltas clamp frame indices to the utterance's own [0, Tm_b - 1] in each pass.  feats: fp32 [B, Tm, 39] (batch stride
+ * feats_bs, rows of 39).  rows_bf16: bf16 [B, Tm, 64] (batch stride rows_bs, a multiple of 8; 16-byte aligned) or NULL --
+ * columns 0..38 = feats rounded to bf16, 39..63 = 0: the operand b200s_kmeans_assign multiplies.  Frames t >= Tm_b are written
+ * as zeros in both outputs.  Tm must equal the frame count of L (Tm = 0, L < 400: nothing is launched).  Two launches, no
+ * floating-point atomics: results are bit-identical from call to call and do not depend on the other utterances. */
+int b200s_mfcc(const float* wav, long long wav_bs, int L, const int* n_samples, int B, int Tm, float* feats, long long feats_bs,
+               void* rows_bf16, long long rows_bs, b200s_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -428,6 +428,12 @@ def kmeanspp_init(x, x_rs, n, D, K, seed, d2, centers, inertia=None):
           L.ptr(centers), L.ptr(inertia), _s())
 
 
+# ------------------------------------------------------------------------------------------------- MFCC features
+def mfcc(wav, wav_bs, n_len, n_samples, B, Tm, feats, feats_bs, rows=None, rows_bs=0):
+    _call("b200s_mfcc", L.ptr(wav), L.ll(wav_bs), i32(n_len), L.ptr(n_samples), i32(B), i32(Tm), L.ptr(feats), L.ll(feats_bs),
+          L.ptr(rows), L.ll(rows_bs), _s(), nbytes=4.0 * B * n_len + B * Tm * (156.0 + (128.0 if rows is not None else 0.0)))
+
+
 # ------------------------------------------------------------------------------------------------- on-device data path
 def span_mask(valid_len, B, T, mask_prob, mask_length, min_masks, key, mask, counts):
     _call("b200s_span_mask", L.ptr(valid_len), i32(B), i32(T), f32(mask_prob), i32(mask_length), i32(min_masks), u32(key[0]),

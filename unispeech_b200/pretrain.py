@@ -213,6 +213,19 @@ class WavLMForPretraining(WavLM):
         inds = (torch.arange(T).float() * self.feat2tar_ratio).long()
         return [t[:, inds.to(t.device)] for t in target_list]
 
+    def label_frames(self, L: int, target_list: List[torch.Tensor]) -> int:
+        """Frames the model runs on for waveforms of L samples: the conv frame count T, or int(targ_tsz / feat2tar_ratio) when the
+        shortest label sequence does not cover T frames (the feature trimming of wavlm.py:440-451 / fairseq HubertModel: at
+        label_rate 100 the 100 Hz labels of an utterance are one short whenever (L - 400) mod 320 < 160)."""
+        from .engine import ConvGeom
+        T = ConvGeom(self.conv_cfg, L).T[-1]
+        targ_tsz = min(t.size(1) for t in target_list)
+        if self.feat2tar_ratio * T > targ_tsz:
+            T = int(targ_tsz / self.feat2tar_ratio)
+            if T <= 0:
+                raise ValueError(f"labels of {targ_tsz} frames leave no feature frame at feat2tar_ratio {self.feat2tar_ratio}")
+        return T
+
     def remove_pretraining_modules(self):
         self.final_proj = None
         self.label_embs_concat = None
@@ -294,9 +307,18 @@ class WavLMForPretraining(WavLM):
     def forward(self, source, target_list=None, padding_mask=None, mask=True, features_only=False, output_layer=None,
                 mask_indices=None, mask_channel_indices=None):
         """fairseq WavLMModel.forward.  With `features_only=False` the result carries everything the criterion needs
-        (`x`, `padding_mask`, `mask_indices`, the frame-aligned `target_list`, `features_pen`); logits are never materialised."""
-        self.extract_features(source, padding_mask=padding_mask, mask=mask, output_layer=output_layer, mask_indices=mask_indices,
-                              mask_channel_indices=mask_channel_indices)
+        (`x`, `padding_mask`, `mask_indices`, the frame-aligned `target_list`, `features_pen`); logits are never materialised.
+        Labels shorter than the conv frames trim the features first (`label_frames`): everything after the conv stack, the
+        feature penalty included, runs on the kept frames, and the trimmed frames get a zero gradient."""
+        from .engine import ConvGeom
+        if target_list is not None and not features_only:
+            T = self.label_frames(source.shape[1], target_list)
+            self._frame_limit = T if T < ConvGeom(self.conv_cfg, source.shape[1]).T[-1] else None
+        try:
+            self.extract_features(source, padding_mask=padding_mask, mask=mask, output_layer=output_layer,
+                                  mask_indices=mask_indices, mask_channel_indices=mask_channel_indices)
+        finally:
+            self._frame_limit = None
         res = self._last
         out = {"x": res["x"], "padding_mask": res["padding_mask"], "features": res["features"],
                "layer_results": res["layer_results"]}

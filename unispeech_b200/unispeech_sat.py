@@ -213,7 +213,8 @@ class UniSpeechSATForPretraining(WavLMForPretraining):
             # everything the loss head needs from the host is known before the encoder runs: draw it now (see _draw_instances)
             from .engine import ConvGeom
             B = source.shape[0]
-            T = ConvGeom(self.conv_cfg, source.shape[1]).T[-1]
+            L = source.shape[1]
+            T = ConvGeom(self.conv_cfg, L).T[-1] if target_list is None else self.label_frames(L, target_list)
             pm_h = self.forward_padding_mask(T, padding_mask) if padding_mask is not None else torch.zeros(B, T, dtype=torch.bool)
             if mask_indices is None and mask_channel_indices is None:
                 # the channel draw follows the span draw immediately, as in the reference's apply_mask

@@ -105,17 +105,20 @@ class _ConvFn(torch.autograd.Function):
     """Conv stack + GradMultiply (WavLM/WavLM.py:333-336, WavLM/modules.py:60-69) + the feature penalty of the pre-training
     models (`features.float().pow(2).mean()` taken AFTER GradMultiply, src/fairseq/models/wavlm/wavlm.py:477-484): the penalty is
     an output of this Function, so its gradient and the gradient arriving from the projection reach the extractor together and
-    BOTH are scaled by `feature_grad_mult` in one pass (`b200s_grad_multiply`)."""
+    BOTH are scaled by `feature_grad_mult` in one pass (`b200s_grad_multiply`).  `frames` (< the conv frame count, or None):
+    only the first `frames` frames feed the model (label-driven trimming, pretrain.py), so the penalty is their mean and the
+    gradient of every later frame is zero."""
 
     @staticmethod
-    def forward(ctx, anchor, eng: Engine, wav, want_pen):
+    def forward(ctx, anchor, eng: Engine, wav, want_pen, frames=None):
         from . import ops
         ctx.fwd_stream = torch.cuda.current_stream()
         save = bool(ctx.needs_input_grad[0])
         st = eng.conv_forward(wav, save)
         feats = st["a"][-1]
         B, Tp, C = feats.shape
-        T = st["geo"].T[-1]
+        ctx.T_conv = st["geo"].T[-1]
+        T = ctx.T_conv if frames is None else frames
         pen = None
         if want_pen:
             acc = torch.zeros(1, dtype=torch.float64, device=feats.device)
@@ -134,6 +137,8 @@ class _ConvFn(torch.autograd.Function):
         if dfeat is None:  # only the penalty was used
             dfeat = torch.zeros_like(feats)
         g = dfeat if (dfeat.dtype == BF and dfeat.is_contiguous()) else dfeat.to(BF).contiguous()
+        if T < ctx.T_conv:
+            g[:, T:ctx.T_conv].zero_()  # trimmed frames: nothing downstream read them
         mult = float(ctx.eng.cfg.feature_grad_mult)
         if mult != 1.0 or dpen is not None:
             pg = dpen.float().contiguous() if dpen is not None else None
@@ -141,7 +146,7 @@ class _ConvFn(torch.autograd.Function):
         ctx.eng.conv_backward(ctx.st, g)
         ctx.st = ctx.feats = None
         ctx.eng.backward_stage_done("conv")
-        return None, None, None, None
+        return None, None, None, None, None
 
 
 class _ProjFn(torch.autograd.Function):
@@ -568,11 +573,12 @@ class WavLM(nn.Module):
         from . import ops
         ops.memset_zero(self.grad_buffer())
 
-    def _extractor(self, source, valid_last=None):
+    def _extractor(self, source, valid_last=None, frames=None):
         """`valid_last` (int32 [B], host or device): frames of the extractor output up to every utterance's last valid one.  The
         conv stack then skips the padding beyond them (engine.conv_valid_rows) -- not when the feature penalty is wanted (the
         reference takes `features.pow(2).mean()` over the padded frames too, so they must hold the reference's values), and
-        not when the caller asks for the conv features themselves (`ret_conv`: extract_features passes no `valid_last` then)."""
+        not when the caller asks for the conv features themselves (`ret_conv`: extract_features passes no `valid_last` then).
+        `frames`: see _ConvFn."""
         eng = self._begin(source.device)
         wav = source.float().contiguous()
         w0 = self.feature_extractor.conv_layers[0][0].weight
@@ -580,10 +586,10 @@ class WavLM(nn.Module):
         eng.conv_valid_last = None if want_pen else valid_last
         try:
             if self.feature_grad_mult > 0:
-                feats, st, pen = _ConvFn.apply(w0, eng, wav, want_pen)
+                feats, st, pen = _ConvFn.apply(w0, eng, wav, want_pen, frames)
             else:
                 with torch.no_grad():
-                    feats, st, pen = _ConvFn.apply(w0, eng, wav, want_pen)
+                    feats, st, pen = _ConvFn.apply(w0, eng, wav, want_pen, frames)
         finally:
             eng.conv_valid_last = None
         self._last_pen = pen
@@ -630,7 +636,10 @@ class WavLM(nn.Module):
         CUDA graph; the reference's sampler is host numpy RNG).  With `mask=True` both are sampled when neither is given;
         once either is given, the other one given as None means no mask of that kind."""
         from .engine import ConvGeom
-        T = ConvGeom(self.conv_cfg, source.shape[1]).T[-1]
+        T_conv = ConvGeom(self.conv_cfg, source.shape[1]).T[-1]
+        # pre-training with labels shorter than the conv frames (WavLMForPretraining.forward): the model runs on the first
+        # `_frame_limit` frames -- frame mask, span / channel masks, projection and encoder all see that many
+        T = T_conv if getattr(self, "_frame_limit", None) is None else self._frame_limit
         B = source.shape[0]
         # `padding_mask` may live on the host (as it does in the reference's collater): the frame mask and the span sampler
         # then run on the host without a device sync, and only the small uint8 masks are uploaded.
@@ -661,8 +670,8 @@ class WavLM(nn.Module):
         valid_last = None
         if fpm is not None and getattr(fpm, "_b200_valid", None) is not None:
             valid_last = fpm._b200_valid_host if fpm_host is not None else fpm._b200_valid
-        feats, T2 = self._extractor(source, None if ret_conv else valid_last)
-        assert T2 == T
+        feats, T2 = self._extractor(source, None if ret_conv else valid_last, None if T == T_conv else T)
+        assert T2 == T_conv
         self._last_conv = feats  # conv features [B, Tp, C] (valid rows T): `features_pen` of the pre-training criterion reads them
         eng = self._engine
         mask_u8 = mask_indices.to(device=source.device, dtype=torch.uint8).contiguous() if mask_indices is not None else None
