@@ -58,7 +58,7 @@ def test_no_channel_draw_without_channel_prob():
 
 
 @pytest.mark.parametrize("padded", [False, True])
-def test_sat_early_draw_keeps_the_reference_order(monkeypatch, padded):
+def test_sat_early_draws_reach_the_extraction_call_in_the_reference_order(monkeypatch, padded):
     """UniSpeech-SAT draws its masks before the encoder runs (for the instance-sampling helper thread): the channel draw must
     follow the span draw there, and both must reach the encoder."""
     from unispeech_b200.pretrain import WavLMForPretraining
@@ -77,7 +77,7 @@ def test_sat_early_draw_keeps_the_reference_order(monkeypatch, padded):
         seen.update(kw)
         raise _Stop
 
-    monkeypatch.setattr(WavLMForPretraining, "forward", fake_forward)
+    monkeypatch.setattr(WavLMForPretraining, "_forward", fake_forward)
     B, L = 2, 16000
     T, D = O.num_frames(L, cfg), cfg.encoder_embed_dim
     pm = _padding(B, L, [L, 11000]) if padded else None

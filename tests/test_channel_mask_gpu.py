@@ -229,7 +229,7 @@ def test_model_with_channel_mask_vs_oracle(cuda_device, name):
 
 # ------------------------------------------------------------------------------------------------------------------ wrappers
 @pytest.mark.parametrize("kind", ["hubert", "wav2vec"])
-def test_finetuning_wrapper_draws_and_applies_channel_mask(cuda_device, kind):
+def test_finetuning_wrapper_samples_and_applies_channel_mask(cuda_device, kind):
     """Training mode with apply_mask=True, mask_channel_prob 0.5 / length 64 (the published ASR recipes): the masks drawn from a
     seeded numpy state are the reference's two compute_mask_indices calls in its order, the output equals extract_features with
     those masks injected, and a CTC loss on `proj` back-propagates finite gradients."""
@@ -256,6 +256,9 @@ def test_finetuning_wrapper_draws_and_applies_channel_mask(cuda_device, kind):
     B, L = 2, 16000
     wav, pmask = O.deterministic_waveform(B, L, seed=6, lengths=[16000, 12000])
     T, D = O.num_frames(L, cfg), cfg.encoder_embed_dim
+    drawn = []   # the masks the model sampled for the forward pass
+    sample_masks = m.sample_masks
+    m.sample_masks = lambda *a: drawn.append(sample_masks(*a)) or drawn[-1]
     np.random.seed(123)
     out = enc(wav.to(dev), pmask)
     np.random.seed(123)
@@ -263,8 +266,9 @@ def test_finetuning_wrapper_draws_and_applies_channel_mask(cuda_device, kind):
     mi = compute_mask_indices((B, T), fpm, cfg.mask_prob, cfg.mask_length, "static", 0, min_masks=2, no_overlap=False,
                               min_space=1)
     ci = compute_mask_indices((B, D), None, 0.5, 64, "static", 0, no_overlap=False, min_space=1)
-    assert torch.equal(m._last["mask_indices"].cpu(), torch.from_numpy(mi))
-    assert torch.equal(m._last["mask_channel_indices"].cpu(), torch.from_numpy(ci))
+    assert len(drawn) == 1
+    assert torch.equal(drawn[0][0].cpu(), torch.from_numpy(mi))
+    assert torch.equal(drawn[0][1].cpu(), torch.from_numpy(ci))
     y = out["encoder_out"]                                        # T x B x V
     with torch.no_grad():
         x_inj, _ = m.extract_features(wav.to(dev), padding_mask=pmask, mask=True, mask_indices=torch.from_numpy(mi),

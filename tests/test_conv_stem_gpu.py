@@ -441,11 +441,7 @@ def test_conv_stack(cuda_device, monkeypatch, name, ragged):
     else:
         lasts = [T6] * B
     V = [receptive_rows(l, convs, T) for l in lasts]  # V[b][layer]
-    eng.conv_valid_last = torch.tensor(lasts, dtype=torch.int32) if ragged else None
-    try:
-        st = eng.conv_forward(wav, True)
-    finally:
-        eng.conv_valid_last = None
+    st = eng.conv_forward(wav, True, torch.tensor(lasts, dtype=torch.int32) if ragged else None)
     torch.cuda.synchronize()
     Wb = {i: m.feature_extractor.conv_layers[i][0].weight.detach().to(BF).double() for i in range(1, n)}  # the GEMM operands
     norms = {i: (m.feature_extractor.conv_layers[i][2][1] if ln else None) for i in range(n)}

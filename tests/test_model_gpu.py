@@ -147,6 +147,51 @@ def test_layer_hooks_and_module_tree(cuda_device):
     assert torch.equal(seen["enc"], x)
 
 
+def test_layer_called_alone_after_an_interrupted_call_computes_every_row(cuda_device):
+    """The ragged lengths of a batch belong to that call: after a forward hook raises inside the layer loop, a layer called on
+    its own with a same-size batch of longer utterances must compute what a model that never saw the first batch computes."""
+    cfg = O.tiny_config(pre_ln=True)
+    m, fresh = build(cfg, cuda_device), build(cfg, cuda_device)
+    B, L = 2, 16000
+    T, D = O.num_frames(L, cfg), cfg.encoder_embed_dim
+    wav, pmask = O.deterministic_waveform(B, L, seed=2, lengths=[L, 6000])
+
+    class _Stop(Exception):
+        pass
+
+    def fail(mod, inp, out):
+        raise _Stop
+
+    hook = m.encoder.layers[1].register_forward_hook(fail)
+    with torch.no_grad(), pytest.raises(_Stop):
+        m.extract_features(wav.to(cuda_device), padding_mask=pmask.to(cuda_device))
+    hook.remove()
+    x = torch.randn(T, B, D, generator=torch.Generator().manual_seed(5)).to(cuda_device)
+    pad = torch.zeros(B, T, dtype=torch.bool, device=cuda_device)
+    pad[1, T - 3:] = True
+    with torch.no_grad():
+        fresh.extract_features(wav.to(cuda_device))   # prepares the layer operands
+        want, _, _ = fresh.encoder.layers[0](x, self_attn_padding_mask=pad)
+        got, _, _ = m.encoder.layers[0](x, self_attn_padding_mask=pad)
+    assert torch.equal(got, want), (got.float() - want.float()).abs().amax((0, 2))
+
+
+def test_extract_features_keeps_no_reference_to_its_outputs(cuda_device):
+    """Once the caller drops what extract_features returned, nothing in the model keeps it alive."""
+    import gc
+    import weakref
+    cfg = O.tiny_config(pre_ln=True)
+    m = build(cfg, cuda_device)
+    wav, pmask = O.deterministic_waveform(2, 16000, seed=3, lengths=[16000, 9000])
+    with torch.no_grad():
+        (x, layer_results), fpm = m.extract_features(wav.to(cuda_device), padding_mask=pmask.to(cuda_device),
+                                                     output_layer=cfg.encoder_layers, ret_layer_results=True)
+    refs = [weakref.ref(x), weakref.ref(layer_results[1][0])]
+    del x, layer_results, fpm
+    gc.collect()
+    assert [r() is None for r in refs] == [True, True]
+
+
 def test_state_dict_keys_match_reference_layout():
     from unispeech_b200.wavlm import WavLM, WavLMConfig
     for cfg in (O.tiny_config(pre_ln=False), O.tiny_config(pre_ln=True)):

@@ -33,7 +33,8 @@ def run(backward, churn):
         m._engine.prepared_version = None
     (x, lr), _ = m.extract_features(wav, padding_mask=None, mask=True, mask_indices=mask, ret_layer_results=True,
                                     output_layer=cfg.encoder_layers)
-    feats = m._last_conv[:, :T].detach().clone()
+    with torch.no_grad():
+        feats = m.feature_extractor(wav).transpose(1, 2).clone()
     outs = [feats] + [h.detach().clone() for h, _ in lr]
     if backward:
         x.float().sum().backward()

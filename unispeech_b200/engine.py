@@ -180,9 +180,7 @@ class Engine:
         self.flat: Optional[FlatGrads] = None
         self._params = None
         self.drop: Optional[DR.DropState] = None  # set per forward pass by WavLM._begin (training-mode dropout)
-        self.conv_valid_last = None  # ragged batch: int32 [B] valid frames of the extractor output (set per call by WavLM._extractor)
         self.grad_sync = None  # parallel.OverlappedGradSync: told when a stage of the backward pass has produced its gradients
-        self.ragged_valid = None  # int32 [B] valid frames per utterance of the current forward (ragged batch), else None
 
     def backward_stage_done(self, stage):
         if self.grad_sync is not None:
@@ -290,7 +288,7 @@ class Engine:
         return self.flat.view(p)
 
     # ---- row-wise GEMMs of the layer stack: flat over all B*T rows, or -- for a ragged batch -- per utterance with the padded
-    # tail of every utterance skipped (`rag`: int32 [B] valid frames on the device, see WavLM.extract_features)
+    # tail of every utterance skipped (`rag`: int32 [B] valid frames on the device, see WavLM._extract)
     @staticmethod
     def _mm(a, K, w, N, out, rag, T, B, **epi):
         if rag is None:
@@ -336,8 +334,9 @@ class Engine:
         return None
 
     # ------------------------------------------------------------------------------------------------ conv stack
-    def conv_forward(self, wav: torch.Tensor, save: bool):
-        """ConvFeatureExtractionModel.forward (WavLM/WavLM.py:485-504) -> channels-last features [B, Tp, C] (valid rows T)."""
+    def conv_forward(self, wav: torch.Tensor, save: bool, valid_last=None):
+        """ConvFeatureExtractionModel.forward (WavLM/WavLM.py:485-504) -> channels-last features [B, Tp, C] (valid rows T).
+        `valid_last` (int32 [B], host or device, or None): frames of the output up to every utterance's last valid one."""
         m, cfg = self.m, self.cfg
         convs = m.conv_cfg
         B, L_ = wav.shape
@@ -349,8 +348,8 @@ class Engine:
         # ragged batch: per layer, the rows any valid output frame depends on; the conv GEMMs zero-fill whole tiles beyond them
         # (layer 0 and the LayerNorms still walk every row: finite values, never read by a valid frame)
         cv = None
-        if self.conv_valid_last is not None:
-            cv = conv_valid_rows(self.conv_valid_last, convs, geo.T).to(dev, non_blocking=True)
+        if valid_last is not None:
+            cv = conv_valid_rows(valid_last, convs, geo.T).to(dev, non_blocking=True)
         st["cv"] = cv
         vrow = (lambda i: cv[i]) if cv is not None else (lambda i: None)
         cbias = [blk[0].bias for blk in m.feature_extractor.conv_layers]  # conv_bias=True: fp32 [C] per layer, else None
@@ -612,9 +611,9 @@ class Engine:
         return dxm
 
     # ------------------------------------------------------------------------------------------------ transformer layer
-    def layer_forward(self, idx: int, x: torch.Tensor, pad_u8, tab, save: bool):
+    def layer_forward(self, idx: int, x: torch.Tensor, pad_u8, tab, save: bool, rag=None):
         """TransformerSentenceEncoderLayer.forward (WavLM/WavLM.py:677-742) + MultiheadAttention fast path
-        (WavLM/modules.py:457-564) on x: bf16 [B,T,D]."""
+        (WavLM/modules.py:457-564) on x: bf16 [B,T,D].  `rag`: int32 [B] valid frames (ragged batch, with `pad_u8`) or None."""
         m, cfg = self.m, self.cfg
         lyr = m.encoder.layers[idx]
         a = lyr.self_attn
@@ -631,7 +630,6 @@ class Engine:
         p_a = d.p_attn if d is not None else 0.0
         p_act = d.p_act if d is not None else 0.0
         st = dict(x=x, drop=d)
-        rag = self.ragged_valid if pad_u8 is not None else None   # int32 [B] valid frames (ragged batch) or None
         want_gate = tab is not None and cfg.gru_rel_pos
         gate = self._take_gate(x, idx) if (want_gate and not pre_ln) else None
         if pre_ln:

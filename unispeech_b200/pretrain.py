@@ -310,26 +310,23 @@ class WavLMForPretraining(WavLM):
         (`x`, `padding_mask`, `mask_indices`, the frame-aligned `target_list`, `features_pen`); logits are never materialised.
         Labels shorter than the conv frames trim the features first (`label_frames`): everything after the conv stack, the
         feature penalty included, runs on the kept frames, and the trimmed frames get a zero gradient."""
-        from .engine import ConvGeom
-        if target_list is not None and not features_only:
-            T = self.label_frames(source.shape[1], target_list)
-            self._frame_limit = T if T < ConvGeom(self.conv_cfg, source.shape[1]).T[-1] else None
-        try:
-            self.extract_features(source, padding_mask=padding_mask, mask=mask, output_layer=output_layer,
-                                  mask_indices=mask_indices, mask_channel_indices=mask_channel_indices)
-        finally:
-            self._frame_limit = None
-        res = self._last
+        return self._forward(source, target_list, padding_mask, mask, features_only, output_layer, mask_indices,
+                             mask_channel_indices)[0]
+
+    def _forward(self, source, target_list, padding_mask, mask, features_only, output_layer, mask_indices, mask_channel_indices):
+        """`forward`, and the full result dict of the extraction call it made (for the subclasses' loss heads): (out, res)."""
+        frames = self.label_frames(source.shape[1], target_list) if target_list is not None and not features_only else None
+        res = self._extract(source, padding_mask, mask, False, output_layer, mask_indices, mask_channel_indices, frames)
         out = {"x": res["x"], "padding_mask": res["padding_mask"], "features": res["features"],
                "layer_results": res["layer_results"]}
         if features_only:
-            return out
+            return out, res
         T = res["x"].shape[1]
         out["mask_indices"] = res["mask_indices"]
-        out["padding_mask_host"] = res.get("padding_mask_host")  # host copy of the frame mask when the caller's mask was on the host
+        out["padding_mask_host"] = res["padding_mask_host"]  # host copy of the frame mask when the caller's mask was on the host
         out["target_list"] = self.forward_targets(T, target_list) if target_list is not None else None
-        out["features_pen"] = self._last_pen  # mean(features^2) after GradMultiply, wavlm.py:477-484 (kernel, inside _ConvFn)
-        return out
+        out["features_pen"] = res["features_pen"]  # mean(features^2) after GradMultiply, wavlm.py:477-484 (kernel, inside _ConvFn)
+        return out, res
 
     def criterion(self, net_output: Dict, pred_masked_weight: float = 1.0, pred_nomask_weight: float = 0.0,
                   loss_weights: Optional[List[float]] = None):

@@ -225,14 +225,13 @@ class UniSpeechSATForPretraining(WavLMForPretraining):
                 gen = torch.Generator()
                 gen.set_state(torch.get_rng_state())
                 fut = _draw_pool().submit(self._draw_instances, mask_indices.bool(), pm_h, gen, source.device)
-        out = super().forward(source, target_list=target_list, padding_mask=padding_mask, mask=mask, features_only=features_only,
-                              output_layer=output_layer, mask_indices=mask_indices, mask_channel_indices=mask_channel_indices)
+        out, res = self._forward(source, target_list=target_list, padding_mask=padding_mask, mask=mask, features_only=features_only,
+                                 output_layer=output_layer, mask_indices=mask_indices, mask_channel_indices=mask_channel_indices)
         if fut is not None:
             pre = fut.result()
             torch.set_rng_state(gen.get_state())
         if features_only or not self.utterance_contrastive_loss:
             return out
-        res = self._last
         spk_x = res["spk_x"]                      # [B, T, D]: output of layer `utterance_contrastive_layer` (normalised for pre-LN)
         B, T, D = spk_x.shape
         dev = spk_x.device

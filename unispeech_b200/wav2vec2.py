@@ -175,9 +175,8 @@ class Wav2Vec2Model(WavLM):
         if float(getattr(self.cfg, "dropout_features", 0.0)) > 0 and self.training and not features_only:
             raise NotImplementedError("dropout_features > 0 on the quantizer input is not implemented")
         # (`layer` is the 0-based index of the reference's TransformerEncoder.extract_features; extract_features here is 1-based)
-        self.extract_features(source, padding_mask=padding_mask, mask=mask, output_layer=None if layer is None else layer + 1,
-                              mask_indices=mask_indices, mask_channel_indices=mask_channel_indices)
-        res = self._last
+        res = self._extract(source, padding_mask, mask, False, None if layer is None else layer + 1, mask_indices,
+                            mask_channel_indices)
         if features_only:
             return {"x": res["x"], "padding_mask": res["padding_mask"], "features": res["unmasked_features"],
                     "layer_results": res["layer_results"]}
@@ -204,7 +203,7 @@ class Wav2Vec2Model(WavLM):
         outs = _W2vNceFn.apply(x2d, f2d, self.final_proj.weight, self, up(rows_h.to(torch.int32)), up(neg_ns), S, N,
                                DR.site_key(seed, _SITE_GUMBEL_W2V), stats)
         out = {"loss_nce": outs[0], "sample_size": S, "correct": stats["correct"], "count": stats["count"],
-               "padding_mask": res["padding_mask"], "features_pen": self._last_pen, "mask_indices": mi}
+               "padding_mask": res["padding_mask"], "features_pen": res["features_pen"], "mask_indices": mi}
         if self.quantizer is not None:
             out.update(prob_perplexity=outs[1], code_perplexity=stats["code_perplexity"], num_vars=stats["num_vars"],
                        temp=stats["temp"], codes=stats["codes"])

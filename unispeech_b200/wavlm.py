@@ -107,14 +107,14 @@ class _ConvFn(torch.autograd.Function):
     an output of this Function, so its gradient and the gradient arriving from the projection reach the extractor together and
     BOTH are scaled by `feature_grad_mult` in one pass (`b200s_grad_multiply`).  `frames` (< the conv frame count, or None):
     only the first `frames` frames feed the model (label-driven trimming, pretrain.py), so the penalty is their mean and the
-    gradient of every later frame is zero."""
+    gradient of every later frame is zero.  `valid_last`: see Engine.conv_forward."""
 
     @staticmethod
-    def forward(ctx, anchor, eng: Engine, wav, want_pen, frames=None):
+    def forward(ctx, anchor, eng: Engine, wav, want_pen, frames=None, valid_last=None):
         from . import ops
         ctx.fwd_stream = torch.cuda.current_stream()
         save = bool(ctx.needs_input_grad[0])
-        st = eng.conv_forward(wav, save)
+        st = eng.conv_forward(wav, save, valid_last)
         feats = st["a"][-1]
         B, Tp, C = feats.shape
         ctx.T_conv = st["geo"].T[-1]
@@ -146,14 +146,15 @@ class _ConvFn(torch.autograd.Function):
         ctx.eng.conv_backward(ctx.st, g)
         ctx.st = ctx.feats = None
         ctx.eng.backward_stage_done("conv")
-        return None, None, None, None, None
+        return None, None, None, None, None, None
 
 
 class _ProjFn(torch.autograd.Function):
     """LayerNorm(features) -> post_extract_proj -> dropout_input -> mask_emb / zero padded frames.  Outputs: the view of the padded
     pos_conv input buffer, `features` (projected, WavLM's ret_conv value) and -- `want_fn`, wav2vec 2.0 -- the LayerNorm output
     `unmasked_features` (src/fairseq/models/wav2vec/wav2vec2.py:578-580) whose gradient (quantizer branch) is added to the
-    projection's in the backward pass."""
+    projection's in the backward pass -- and the stage state, whose `xpad` is the buffer the first output is a view of (the
+    pos_conv stem reads the zero padding around it)."""
 
     @staticmethod
     def forward(ctx, feats, anchor, eng: Engine, T, mask_u8, pad_u8, want_features, want_fn=False, chan_u8=None):
@@ -162,13 +163,12 @@ class _ProjFn(torch.autograd.Function):
         st = eng.project_forward(feats, T, mask_u8, pad_u8, save, want_features, chan_u8)
         ctx.eng, ctx.st, ctx.T, ctx.mask, ctx.pad, ctx.chan = eng, st, T, mask_u8, pad_u8, chan_u8
         half = eng.cfg.conv_pos // 2
-        eng._last_xpad = st["xpad"]  # the padded pos_conv input buffer the returned view lives in
         xv = st["xpad"][:, half:half + T]
-        return xv, st["features"], (st["fn"] if want_fn else None)
+        return xv, st["features"], (st["fn"] if want_fn else None), st
 
     @staticmethod
     @_on_forward_stream
-    def backward(ctx, dxv, _dfeatures, dfn_extra=None):
+    def backward(ctx, dxv, _dfeatures, dfn_extra=None, _unused=None):
         if dfn_extra is not None:
             dfn_extra = dfn_extra if (dfn_extra.dtype == torch.bfloat16 and dfn_extra.is_contiguous()) else \
                 dfn_extra.to(torch.bfloat16).contiguous()
@@ -197,11 +197,11 @@ class _StemFn(torch.autograd.Function):
 
 class _LayerFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, anchor, eng: Engine, idx, pad_u8, bias_state):
+    def forward(ctx, x, anchor, eng: Engine, idx, pad_u8, bias_state, rag):
         ctx.fwd_stream = torch.cuda.current_stream()
         save = bool(ctx.needs_input_grad[0] or ctx.needs_input_grad[1])
         tab = bias_state["tab"] if bias_state is not None else None
-        out, st = eng.layer_forward(idx, x, pad_u8, tab, save)
+        out, st = eng.layer_forward(idx, x, pad_u8, tab, save, rag)
         ctx.eng, ctx.idx, ctx.st, ctx.bias_state = eng, idx, st, bias_state
         if bias_state is not None and save:
             ctx.first = not bias_state["has_first"]
@@ -224,7 +224,7 @@ class _LayerFn(torch.autograd.Function):
             ops.relpos_table_bwd(dtab, bs["lut"], dtab.shape[1], H, eng.g(emb))
         ctx.st = None
         eng.backward_stage_done(("layer", ctx.idx))
-        return dx, None, None, None, None, None
+        return dx, None, None, None, None, None, None
 
 
 class _LNFn(torch.autograd.Function):
@@ -288,7 +288,7 @@ class ConvFeatureExtractionModel(nn.Module):
 
     def forward(self, x):
         """[B, L] waveform -> [B, C, T] (channels-first view of the channels-last kernel output), as the reference returns."""
-        feats, T = self._owner[0]._extractor(x)
+        feats, T, _ = self._owner[0]._extractor(x)
         return feats[:, :T].transpose(1, 2)
 
 
@@ -351,9 +351,12 @@ class TransformerSentenceEncoderLayer(nn.Module):
         self.final_layer_norm = nn.LayerNorm(D)
         self._owner = None  # set by WavLM (list wrapper, so the owner is not registered as a sub-module)
 
-    def forward(self, x, self_attn_mask=None, self_attn_padding_mask=None, need_weights=False, pos_bias=None):
+    def forward(self, x, self_attn_mask=None, self_attn_padding_mask=None, need_weights=False, pos_bias=None,
+                valid_frames=None):
         """x: T x B x C.  `pos_bias` carries the shared relative-position state between layers (the reference passes the
-        materialised [B*H,T,T] bias tensor here; we pass the per-head Toeplitz table instead).  Returns (x, None, pos_bias)."""
+        materialised [B*H,T,T] bias tensor here; we pass the per-head Toeplitz table instead).  `valid_frames` (int32 [B] on
+        the device, with a padding mask only): frames of every utterance up to its last valid one; the row GEMMs and LayerNorms
+        then skip the padded tail and write zeros there.  Returns (x, None, pos_bias)."""
         assert self_attn_mask is None, "streaming / attention masks are not supported"
         model = self._owner[0]
         eng = model._engine_for(x.device)
@@ -361,13 +364,13 @@ class TransformerSentenceEncoderLayer(nn.Module):
         if xb.dtype != BF or not xb.is_contiguous():
             xb = xb.to(BF).contiguous()
         B, T, _ = xb.shape
-        pad_u8 = None
+        pad_u8, rag = None, None
         if self_attn_padding_mask is not None:
             pad_u8 = self_attn_padding_mask if self_attn_padding_mask.dtype == torch.uint8 else self_attn_padding_mask.to(torch.uint8)
-            pad_u8 = pad_u8.contiguous()
+            pad_u8, rag = pad_u8.contiguous(), valid_frames
         if pos_bias is None and model.encoder.relative_position_embedding:
             pos_bias = model.encoder._make_bias_state(T, x.device)
-        out = _LayerFn.apply(xb, self.fc1.weight, eng, self.index, pad_u8, pos_bias)
+        out = _LayerFn.apply(xb, self.fc1.weight, eng, self.index, pad_u8, pos_bias, rag)
         return out.transpose(0, 1), None, pos_bias
 
 
@@ -417,10 +420,11 @@ class TransformerEncoder(nn.Module):
         dtab = torch.zeros(H, 2 * T - 1, dtype=torch.float32, device=device) if torch.is_grad_enabled() else None
         return dict(tab=tab, dtab=dtab, lut=lut, has_first=False)
 
-    def forward(self, x, padding_mask=None, streaming_mask=None, layer=None, extract_layer=None):
+    def forward(self, x, padding_mask=None, streaming_mask=None, layer=None, extract_layer=None, *, _xpad=None, _valid=None):
         """Returns (x, layer_results) like the reference WavLM encoder; with `extract_layer` (UniSpeech-SAT encoder,
-        unispeech_sat.py:1202-1210) a third value: that layer's output, normalised by `layer_norm_for_extract` for pre-LN models."""
-        res = self.extract_features(x, padding_mask, streaming_mask, layer, extract_layer=extract_layer)
+        unispeech_sat.py:1202-1210) a third value: that layer's output, normalised by `layer_norm_for_extract` for pre-LN models.
+        `_xpad` and `_valid` come from WavLM._extract only (see `_encode`)."""
+        res = self._encode(x, padding_mask, streaming_mask, layer, extract_layer, _xpad, _valid)
         x, layer_results = res[0], res[1]
         er = res[2] if extract_layer is not None else None
         if self.layer_norm_first and layer is None:
@@ -439,16 +443,20 @@ class TransformerEncoder(nn.Module):
         also be a list of 1-based layer numbers (fairseq WavLM, src/fairseq/models/wavlm/wavlm.py:730-737: those layers' outputs
         are collected without early exit); `extract_layer` (0-based) adds that layer's output as a third return value
         (UniSpeech-SAT encoder, unispeech_sat.py:1236-1255)."""
+        return self._encode(x, padding_mask, streaming_mask, tgt_layer, extract_layer)
+
+    def _encode(self, x, padding_mask, streaming_mask, tgt_layer, extract_layer, xpad=None, valid=None):
+        """`extract_features` body.  From WavLM._extract, `x` is a view of `xpad`, the zero-padded pos_conv input buffer
+        the projection wrote, and `valid` (int32 [B] or None) the ragged lengths the layers skip the padded tails with."""
         assert streaming_mask is None, "streaming masks are not supported"
         model = self._owner[0]
         eng = model._engine_for(x.device)
         cfg = model.cfg
         B, T, D = x.shape
         half = cfg.conv_pos // 2
-        xpad = getattr(x, "_b200_xpad", None)
         if xpad is None:
-            # external caller (not extract_features): make sure the bf16 operands exist for the current parameters, then stage
-            # into the zero-padded pos_conv buffer and zero padded frames
+            # external caller: make sure the bf16 operands exist for the current parameters, then stage into the zero-padded
+            # pos_conv buffer and zero padded frames
             from . import ops
             eng = model._begin(x.device)
             xpad = torch.zeros(B, T + cfg.conv_pos, D, dtype=BF, device=x.device)
@@ -467,11 +475,10 @@ class TransformerEncoder(nn.Module):
         er = None
         pos_bias = self._make_bias_state(T, x.device) if self.relative_position_embedding else None
         pad_u8 = padding_mask.to(torch.uint8).contiguous() if padding_mask is not None else None
-        eng.ragged_valid = getattr(padding_mask, "_b200_valid", None) if padding_mask is not None else None
         for i, layer in enumerate(self.layers):
             dropout_probability = np.random.random()
             if not self.training or (dropout_probability > self.layerdrop):
-                x, _z, pos_bias = layer(x, self_attn_padding_mask=pad_u8, need_weights=False, pos_bias=pos_bias)
+                x, _z, pos_bias = layer(x, self_attn_padding_mask=pad_u8, need_weights=False, pos_bias=pos_bias, valid_frames=valid)
             if tgt_list is not None:
                 if i + 1 in tgt_list:
                     layer_results.append((x, None))
@@ -482,7 +489,6 @@ class TransformerEncoder(nn.Module):
             if tgt_list is None and i == tgt_layer:
                 r = x
                 break
-        eng.ragged_valid = None  # belongs to this batch only (a layer called on its own later computes every row)
         if r is not None:
             x = r
         if extract_layer is not None:
@@ -521,6 +527,11 @@ class WavLM(nn.Module):
             lyr._owner = owner
         self._engine: Optional[Engine] = None
         self.dropout_seed: Optional[int] = None  # None: draw a fresh seed per forward; an int pins the dropout masks (tests)
+        # what the model's own forward pass needs from extract_features (set by the subclasses, honoured by every caller)
+        self._want_features_pen = False      # pre-training models: the feature penalty (keeps every conv row, see _extractor)
+        self._want_unmasked_features = False  # wav2vec 2.0: the LayerNorm'ed conv features of the quantizer branch
+        self._extract_layer = None           # UniSpeech-SAT: 0-based `utterance_contrastive_layer - 1` (unispeech_sat.py:640-645)
+        self._predict_layers = None          # ILS-HuBERT: 1-based layers whose outputs feed intermediate heads (ils_hubert.py:167-171)
 
     def __deepcopy__(self, memo):
         """`copy.deepcopy(model)` (EMA / teacher copies, checkpoint averaging): the engine holds raw device pointers to THIS model's
@@ -578,22 +589,18 @@ class WavLM(nn.Module):
         conv stack then skips the padding beyond them (engine.conv_valid_rows) -- not when the feature penalty is wanted (the
         reference takes `features.pow(2).mean()` over the padded frames too, so they must hold the reference's values), and
         not when the caller asks for the conv features themselves (`ret_conv`: extract_features passes no `valid_last` then).
-        `frames`: see _ConvFn."""
+        `frames`: see _ConvFn.  Returns (features [B, Tp, C], conv frame count, feature penalty or None)."""
         eng = self._begin(source.device)
         wav = source.float().contiguous()
         w0 = self.feature_extractor.conv_layers[0][0].weight
-        want_pen = bool(getattr(self, "_want_features_pen", False))
-        eng.conv_valid_last = None if want_pen else valid_last
-        try:
-            if self.feature_grad_mult > 0:
-                feats, st, pen = _ConvFn.apply(w0, eng, wav, want_pen, frames)
-            else:
-                with torch.no_grad():
-                    feats, st, pen = _ConvFn.apply(w0, eng, wav, want_pen, frames)
-        finally:
-            eng.conv_valid_last = None
-        self._last_pen = pen
-        return feats, st["geo"].T[-1]
+        want_pen = self._want_features_pen
+        valid_last = None if want_pen else valid_last
+        if self.feature_grad_mult > 0:
+            feats, st, pen = _ConvFn.apply(w0, eng, wav, want_pen, frames, valid_last)
+        else:
+            with torch.no_grad():
+                feats, st, pen = _ConvFn.apply(w0, eng, wav, want_pen, frames, valid_last)
+        return feats, st["geo"].T[-1], pen
 
     # ---- reference API
     def apply_mask(self, B, T, padding_mask):
@@ -635,11 +642,21 @@ class WavLM(nn.Module):
         optional) let a caller inject the masked frames and channels instead of sampling them (used by the parity tests and the
         CUDA graph; the reference's sampler is host numpy RNG).  With `mask=True` both are sampled when neither is given;
         once either is given, the other one given as None means no mask of that kind."""
+        res = self._extract(source, padding_mask, mask, ret_conv, output_layer, mask_indices, mask_channel_indices)
+        feature = res["features"] if ret_conv else res["x"]
+        if ret_layer_results:
+            feature = (feature, res["layer_results"])
+        return feature, res["padding_mask"]
+
+    def _extract(self, source, padding_mask, mask, ret_conv, output_layer, mask_indices, mask_channel_indices, frames=None):
+        """The forward pass behind `extract_features` and the models' `forward`: returns everything one call produced as a dict
+        (`x`, `padding_mask`, `features`, `layer_results`, `mask_indices`, `mask_channel_indices`, `padding_mask_host`, `spk_x`,
+        `unmasked_features`, `features_pen`).  `frames` (pre-training with labels shorter than the conv frames,
+        WavLMForPretraining.forward): the model runs on the first `frames` frames -- frame mask, span / channel masks, projection
+        and encoder all see that many."""
         from .engine import ConvGeom
         T_conv = ConvGeom(self.conv_cfg, source.shape[1]).T[-1]
-        # pre-training with labels shorter than the conv frames (WavLMForPretraining.forward): the model runs on the first
-        # `_frame_limit` frames -- frame mask, span / channel masks, projection and encoder all see that many
-        T = T_conv if getattr(self, "_frame_limit", None) is None else self._frame_limit
+        T = T_conv if frames is None else frames
         B = source.shape[0]
         # `padding_mask` may live on the host (as it does in the reference's collater): the frame mask and the span sampler
         # then run on the host without a device sync, and only the small uint8 masks are uploaded.
@@ -656,51 +673,39 @@ class WavLM(nn.Module):
             raise ValueError(f"mask_channel_indices must be [B, encoder_embed_dim] = [{B}, {self.cfg.encoder_embed_dim}]; "
                              f"got {list(mask_channel_indices.shape)}")
         # ragged batch: frames of every utterance up to its last valid one (host arithmetic when the mask lives on the host; with
-        # a device-only mask two tiny device ops, no synchronisation).  The layer GEMMs skip the padded tail of every utterance.
-        # The tensor travels to the encoder as an attribute of the frame mask, so a stale one can never meet another batch.
+        # a device-only mask two tiny device ops, no synchronisation): `valid_last` for the conv stack, `valid` on the device for
+        # the encoder layers, which skip the padded tail of every utterance.
+        valid = valid_last = None
         if fpm is not None:
             if fpm_host is not None:
                 if bool(fpm_host.any()):
                     last = ((~fpm_host).to(torch.int32) * torch.arange(1, T + 1, dtype=torch.int32)).amax(1)
-                    fpm._b200_valid_host = last.to(torch.int32).contiguous()
-                    fpm._b200_valid = fpm._b200_valid_host.to(source.device, non_blocking=True)
+                    valid_last = last.to(torch.int32).contiguous()
+                    valid = valid_last.to(source.device, non_blocking=True)
             else:
-                fpm._b200_valid = ((~fpm).to(torch.int32) * torch.arange(1, T + 1, dtype=torch.int32, device=fpm.device)) \
+                valid = valid_last = ((~fpm).to(torch.int32) * torch.arange(1, T + 1, dtype=torch.int32, device=fpm.device)) \
                     .amax(1).to(torch.int32).contiguous()
-        valid_last = None
-        if fpm is not None and getattr(fpm, "_b200_valid", None) is not None:
-            valid_last = fpm._b200_valid_host if fpm_host is not None else fpm._b200_valid
-        feats, T2 = self._extractor(source, None if ret_conv else valid_last, None if T == T_conv else T)
+            fpm._b200_valid = valid  # for KMeans.predict on the returned mask (nothing in the model reads it)
+        feats, T2, pen = self._extractor(source, None if ret_conv else valid_last, None if T == T_conv else T)
         assert T2 == T_conv
-        self._last_conv = feats  # conv features [B, Tp, C] (valid rows T): `features_pen` of the pre-training criterion reads them
         eng = self._engine
         mask_u8 = mask_indices.to(device=source.device, dtype=torch.uint8).contiguous() if mask_indices is not None else None
         chan_u8 = mask_channel_indices.to(device=source.device, dtype=torch.uint8).contiguous() \
             if mask_channel_indices is not None else None
         pad_u8 = fpm.to(torch.uint8).contiguous() if fpm is not None else None
-        want_fn = bool(getattr(self, "_want_unmasked_features", False))
-        xv, features, unmasked = _ProjFn.apply(feats, self.post_extract_proj.weight, eng, T, mask_u8, pad_u8, ret_conv, want_fn,
-                                               chan_u8)
-        xv._b200_xpad = eng._last_xpad
-        el = getattr(self, "_extract_layer", None)  # UniSpeech-SAT: 0-based `utterance_contrastive_layer - 1` (unispeech_sat.py:640-645)
-        pl = getattr(self, "_predict_layers", None)  # ILS-HuBERT: 1-based layers whose outputs feed intermediate heads (ils_hubert.py:167-171)
+        xv, features, unmasked, proj_st = _ProjFn.apply(feats, self.post_extract_proj.weight, eng, T, mask_u8, pad_u8, ret_conv,
+                                                        self._want_unmasked_features, chan_u8)
+        el, pl = self._extract_layer, self._predict_layers
         lay = (list(pl) if (pl is not None and output_layer is None) else None) if output_layer is None else output_layer - 1
-        enc = self.encoder(xv, padding_mask=fpm, layer=lay, extract_layer=el)
-        x, layer_results = enc[0], enc[1]
-        res = {"x": x, "padding_mask": fpm, "features": features, "layer_results": layer_results,
-               "mask_indices": mask_indices, "mask_channel_indices": mask_channel_indices, "padding_mask_host": fpm_host,
-               "spk_x": enc[2] if el is not None else None, "unmasked_features": unmasked}
-        self._last = res
-        feature = res["features"] if ret_conv else res["x"]
-        if ret_layer_results:
-            feature = (feature, res["layer_results"])
-        return feature, res["padding_mask"]
+        enc = self.encoder(xv, padding_mask=fpm, layer=lay, extract_layer=el, _xpad=proj_st["xpad"], _valid=valid)
+        return {"x": enc[0], "padding_mask": fpm, "features": features, "layer_results": enc[1],
+                "mask_indices": mask_indices, "mask_channel_indices": mask_channel_indices, "padding_mask_host": fpm_host,
+                "spk_x": enc[2] if el is not None else None, "unmasked_features": unmasked, "features_pen": pen}
 
     def forward(self, source, target_list=None, padding_mask=None, mask=True, features_only=False, output_layer=None):
         """fairseq-style entry (src/fairseq/models/wavlm/wavlm.py:465-523, encoder part): returns the result dict.
         The masked-prediction heads (final_proj / label embeddings) are outside the hot path (SURVEY.md section 8f)."""
-        self.extract_features(source, padding_mask=padding_mask, mask=mask, output_layer=output_layer)
-        res = self._last
+        res = self._extract(source, padding_mask, mask, False, output_layer, None, None)
         out = {"x": res["x"], "padding_mask": res["padding_mask"], "features": res["features"],
                "layer_results": res["layer_results"]}
         if not features_only:
