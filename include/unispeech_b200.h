@@ -86,6 +86,28 @@ int b200s_gemm_wgrad_ragged(const void* y, long long y_bs, long long y_rs, const
                             int rows, int batches, int N, int K, float* dw, long long dw_ld, const int* valid,
                             b200s_stream stream);
 
+/* ---- FP8 (e4m3) inference path of the encoder projections (csrc/fp8.cu, csrc/fp8.cuh) ----------------------------------
+ * Quantisation rule (activations per row, weights per output channel), amax = max |x| of the row in fp32:
+ *   q = e4m3_satfinite(x * (448 / amax)),  s = amax / 448  (IEEE divisions);  amax == 0 gives q = 0, s = 0.
+ * A bf16 input is quantised from its bf16 value.  `valid` (int32 [batches], device) may be NULL (every row counts).
+ *
+ * out[b, r, n] = epilogue( a_scale[b*rows + r] * w_scale[n] * sum_k a8[b, r, k] w8[n, k] ): e4m3 K-major operands (A rows at
+ * a8 + b*a_bs + r*a_rs bytes, W [N, K] contiguous), fp32 accumulation, bf16 out.  The epilogue takes `bias`, `gelu` (the value,
+ * no out_pre) and `res1`, applied after the scales; anything else is an error.  Ragged batches as b200s_gemm_rows_ragged: an M
+ * tile at or past valid[b] is written as zeros.  K % 128 == 0, N % 8 == 0, 16-byte-aligned rows. */
+int b200s_gemm_rows_fp8(const void* a8, const float* a_scale, long long a_bs, long long a_rs, int rows, int batches, int K,
+                        const void* w8, const float* w_scale, int N, void* out, long long out_bs, long long out_ld,
+                        const b200s_epilogue* epi, const int* valid, b200s_stream stream);
+/* bf16 rows [batches, rows, D] (element strides x_bs, x_rs) -> e4m3 rows (byte strides q_bs, q_rs) and scale[b*rows + r]: the
+ * GEMM inputs that no LayerNorm produces (attention output, GELU output).  Rows at or past valid[b] are not read; they are
+ * written as zeros with s = 0.  D % 8 == 0, D <= 8192. */
+int b200s_quantize_rows_fp8(const void* x, long long x_bs, long long x_rs, int rows, int batches, int D, void* q, long long q_bs,
+                            long long q_rs, float* scale, const int* valid, b200s_stream stream);
+/* Every e4m3 weight of the encoder in one launch.  descs: device array of n_descs records
+ *   { const float* src; void* dst; float* scale; int N; int K; }   (32 bytes, K % 8 == 0)
+ * dst[n, k] = e4m3 of the fp32 master src[n, k] with scale[n] per output channel; max_rows = the largest N. */
+int b200s_prep_linear_fp8_batched(const void* descs, int n_descs, int max_rows, b200s_stream stream);
+
 /* Grouped positional convolution as an implicit GEMM (TransformerEncoder.pos_conv, WavLM/WavLM.py:514-527,577-579;
  * SamePad WavLM/modules.py:72-83), also used for its input gradient with flipped/transposed taps:
  *   out[b,t,g*Cg+n] = epilogue( sum_{j<taps} sum_{c<Cg} xpad[b, t+j, g*Cg+c] * wp[g*Cgp+n, j*Cgp+c] )
@@ -162,6 +184,16 @@ int b200s_layer_norm_gate_fwd(const void* x, long long x_bs, long long x_rs, con
                               void* y, long long y_bs, long long y_rs, float* mean, float* rstd, int T, int B, int D,
                               const float* grep_w, const float* grep_b, const float* grep_a, int H, float* gate,
                               b200s_stream stream);
+
+/* LayerNorm forward with an e4m3 output for the fp8 GEMMs: q / scale (b200s_quantize_rows_fp8 layout and rule) are taken from
+ * the bf16-rounded normalised row, so they equal the quantisation of the bf16 y.  y (bf16), mean and rstd are optional (NULL);
+ * y, when written, is bit-identical to b200s_layer_norm_fwd.  gate != NULL also writes the gru_rel_pos gate of the attention
+ * that consumes the row (b200s_layer_norm_gate_fwd semantics; D = H * 64 in 256..1280).  Rows at or past valid[b] (valid may be
+ * NULL): zeros, s = 0, mean = rstd = 0, gate = 1.  D as b200s_layer_norm_fwd. */
+int b200s_layer_norm_fwd_fp8(const void* x, long long x_bs, long long x_rs, const float* gamma, const float* beta, void* y,
+                             long long y_bs, long long y_rs, float* mean, float* rstd, void* q, long long q_bs, long long q_rs,
+                             float* scale, int rows_per_batch, int batches, int D, const float* grep_w, const float* grep_b,
+                             const float* grep_a, int H, float* gate, const int* valid, b200s_stream stream);
 
 /* dx = LN-backward(dy) [+ dres];  dgamma, dbeta (+=);  colsum (+=) = column sums of dx (bias gradient of x's producer). */
 int b200s_layer_norm_bwd(const void* dy, long long dy_bs, long long dy_rs, const void* x, long long x_bs,

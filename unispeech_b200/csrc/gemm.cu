@@ -57,7 +57,7 @@ struct ViewSpec {
   CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B;
 };
 
-// bf16 or fp32, zero OOB fill; bf16 maps (MMA operands) promote 256-byte L2 lines, fp32 maps (reduction destinations) none.
+// bf16, fp32 or bytes (fp8), zero OOB fill; bf16 and byte maps (MMA operands) promote 256-byte L2 lines, fp32 maps (reduction destinations) none.
 // Returns 0 on success.
 static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
   EncodeTiledFn fn = get_encode_fn();
@@ -66,7 +66,7 @@ static int make_tmap(CUtensorMap* out, const ViewSpec& v) {
     return -3;
   }
   const bool f32 = v.dtype == CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  const long long esize = f32 ? 4 : 2;
+  const long long esize = f32 ? 4 : v.dtype == CU_TENSOR_MAP_DATA_TYPE_UINT8 ? 1 : 2;
   cuuint64_t dims[4];
   cuuint64_t strides[3];
   cuuint32_t box[4];
@@ -113,6 +113,15 @@ int make_head_tmap(CUtensorMap* out, const void* ptr, CUtensorMapDataType dtype,
 int make_rows_tmap(CUtensorMap* out, const void* ptr, long long cols, long long rows, long long batches, long long row_stride,
                    long long batch_stride, int box_rows) {
   ViewSpec v{ptr, {cols, rows, batches, 1}, {row_stride, batches > 1 ? batch_stride : 0, 0}, {64, box_rows, 1, 1}};
+  return make_tmap(out, v);
+}
+
+// [batches, rows, K] e4m3 bytes with arbitrary row / batch strides (bytes): box = one 128-byte K block x box_rows rows, 128B
+// swizzle (the fp8 row GEMM's operands)
+int make_fp8_rows_tmap(CUtensorMap* out, const void* ptr, long long K, long long rows, long long batches, long long row_stride,
+                       long long batch_stride, int box_rows) {
+  ViewSpec v{ptr, {K, rows, batches, 1}, {row_stride, batches > 1 ? batch_stride : 0, 0}, {128, box_rows, 1, 1},
+             CU_TENSOR_MAP_DATA_TYPE_UINT8};
   return make_tmap(out, v);
 }
 

@@ -8,6 +8,7 @@
 #include "../../include/unispeech_b200.h"
 #include "common.h"
 #include "dropout.cuh"
+#include "fp8.cuh"
 #include "ptx.cuh"
 
 namespace b200 {
@@ -204,6 +205,145 @@ __global__ void __launch_bounds__(256, 32 * VEC * NCH > 1280 ? 2 : 4) ln_fwd_ker
           const float yb = __bfloat162float(__float2bfloat16_rn(v[i * 8 + j]));  // what the attention kernel will read
           sa = fmaf(yb, wa[j], sa);
           sb = fmaf(yb, wb[j], sb);
+        }
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) {
+          sa += __shfl_xor_sync(0xffffffffu, sa, o);
+          sb += __shfl_xor_sync(0xffffffffu, sb, o);
+        }
+        if ((lane & 7) == 0) {
+          const int h = i * 4 + (lane >> 3);
+          const float g1 = 1.0f / (1.0f + __expf(-(sa + gba)));
+          const float g2 = 1.0f / (1.0f + __expf(-(sb + gbb)));
+          ga.gate[(bidx * ga.H + h) * ga.T + t] = g1 * (g2 * ga.grep_a[h] - 1.0f) + 2.0f;
+        }
+      }
+    }
+  }
+}
+
+// LayerNorm forward with an e4m3 output (fp8 inference path, fp8.cuh): ln_fwd_kernel's arithmetic (so y, when written, is
+// bit-identical to b200s_layer_norm_fwd's, and the gate is a function of y as in the gate-fused kernels), then the row's amax over the bf16-ROUNDED values, which the warp already holds whole, and
+// q = e4m3(y_bf16 * 448 / amax), scale = amax / 448.  y, mean and rstd are optional.  (From D = 512 the row, the amax and the
+// gate weights do not fit the 64 registers of four resident blocks without spilling: two blocks.)
+struct Fp8Rows {
+  uint8_t* q;
+  long long bs, rs;  // bytes
+  float* scale;      // [rows]
+};
+template <int VEC>
+__device__ __forceinline__ void store_fp8_vec(uint8_t* p, const float* v, float rinv) {
+  if constexpr (VEC == 8) *reinterpret_cast<uint2*>(p) = make_uint2(fp8x4(v, rinv), fp8x4(v + 4, rinv));
+  else if constexpr (VEC == 4) *reinterpret_cast<uint32_t*>(p) = fp8x4(v, rinv);
+  else *reinterpret_cast<uint16_t*>(p) = static_cast<uint16_t>(fp8x2(v[0], v[1], rinv));
+}
+template <int VEC, int NCH, bool GATE>
+__global__ void __launch_bounds__(256, 32 * VEC * NCH >= 512 ? 2 : 4) ln_fwd_fp8_kernel(const __nv_bfloat16* __restrict__ x, RowView xv,
+                                                     const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                     __nv_bfloat16* __restrict__ y, RowView yv,
+                                                     float* __restrict__ mean_out, float* __restrict__ rstd_out,
+                                                     long long rows, float eps, GateArgs ga, Fp8Rows f8, const int* __restrict__ valid) {
+  pdl_grid_sync();
+  constexpr int D = 32 * VEC * NCH;
+  constexpr int N = NCH * VEC;
+  __shared__ __align__(16) float gs[D], bs[D];
+  for (int c = threadIdx.x; c < D; c += blockDim.x) {
+    gs[c] = gamma[c];
+    bs[c] = beta[c];
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const long long warp_global = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const long long nwarps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  float wa[GATE ? 8 : 1], wb[GATE ? 8 : 1], gba = 0.f, gbb = 0.f;
+  if constexpr (GATE) {
+    static_assert(VEC == 8, "fused gate needs 8 columns per lane");
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = (lane & 7) * 8 + j;
+      wa[j] = ga.grep_w[c] + ga.grep_w[64 + c] + ga.grep_w[128 + c] + ga.grep_w[192 + c];
+      wb[j] = ga.grep_w[256 + c] + ga.grep_w[320 + c] + ga.grep_w[384 + c] + ga.grep_w[448 + c];
+    }
+    gba = ga.grep_b[0] + ga.grep_b[1] + ga.grep_b[2] + ga.grep_b[3];
+    gbb = ga.grep_b[4] + ga.grep_b[5] + ga.grep_b[6] + ga.grep_b[7];
+  }
+  for (long long r = warp_global; r < rows; r += nwarps) {
+    float v[N];
+    unsigned rb, rt;
+    xv.split(r, rb, rt);
+    uint8_t* qr = f8.q + rb * f8.bs + rt * f8.rs;
+    if (valid != nullptr && static_cast<int>(rt) >= valid[rb]) {  // ragged batch: a padded frame is written as zeros, nothing read
+#pragma unroll
+      for (int i = 0; i < N; ++i) v[i] = 0.f;
+#pragma unroll
+      for (int i = 0; i < NCH; ++i) {
+        if (y != nullptr) VecIO<VEC>::store(y + yv.at(rb, rt) + (i * 32 + lane) * VEC, v + i * VEC);
+        store_fp8_vec<VEC>(qr + (i * 32 + lane) * VEC, v + i * VEC, 0.f);
+      }
+      if (lane == 0) {
+        f8.scale[r] = 0.f;
+        if (mean_out) mean_out[r] = 0.f;
+        if (rstd_out) rstd_out[r] = 0.f;
+      }
+      if constexpr (GATE) {
+        if (lane < ga.H) ga.gate[(static_cast<long long>(rb) * ga.H + lane) * ga.T + rt] = 1.0f;
+      }
+      continue;
+    }
+    const __nv_bfloat16* xr = x + xv.off(r);
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) VecIO<VEC>::load(xr + (i * 32 + lane) * VEC, v + i * VEC);
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < N; ++i) s += v[i];
+    const float sum = warp_sum(s);
+    const float mean = sum * (1.0f / D);
+    // x - mean exactly as ln_fwd_kernel's compiled code forms it (so y is bit-identical to b200s_layer_norm_fwd): one FMA with
+    // the row sum (the mean is not rounded first), except at D = 1920, where it subtracts the rounded mean.  That form is nvcc's
+    // contraction choice for ln_fwd_kernel's `v[i] - mean`, not its source: re-check it (test_layer_norm_fp8) with a new toolchain.
+    constexpr bool kFmaMean = D != 1920;
+#pragma unroll
+    for (int i = 0; i < N; ++i) v[i] = kFmaMean ? fmaf(sum, -(1.0f / D), v[i]) : v[i] - mean;
+    float qv = 0.f;
+#pragma unroll
+    for (int i = 0; i < N; ++i) qv += v[i] * v[i];
+    const float rstd = rsqrtf(warp_sum(qv) * (1.0f / D) + eps);
+    float amax = 0.f;
+#pragma unroll
+    for (int ch = 0; ch < NCH; ++ch) {
+      float gg[VEC], bb[VEC];
+      smem_load_vec<VEC>(gs + (ch * 32 + lane) * VEC, gg);
+      smem_load_vec<VEC>(bs + (ch * 32 + lane) * VEC, bb);
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) {
+        const float o = __bfloat162float(__float2bfloat16_rn(v[ch * VEC + j] * rstd * gg[j] + bb[j]));
+        v[ch * VEC + j] = o;
+        amax = fmaxf(amax, fabsf(o));
+      }
+    }
+    if (y != nullptr) {
+      __nv_bfloat16* yr = y + yv.off(r);
+#pragma unroll
+      for (int i = 0; i < NCH; ++i) VecIO<VEC>::store(yr + (i * 32 + lane) * VEC, v + i * VEC);
+    }
+    amax = warp_max(amax);
+    const float rinv = fp8_row_rinv(amax);
+#pragma unroll
+    for (int i = 0; i < NCH; ++i) store_fp8_vec<VEC>(qr + (i * 32 + lane) * VEC, v + i * VEC, rinv);
+    if (lane == 0) {
+      f8.scale[r] = fp8_row_scale(amax);
+      if (mean_out) mean_out[r] = mean;
+      if (rstd_out) rstd_out[r] = rstd;
+    }
+    if constexpr (GATE) {
+      const long long bidx = r / ga.T, t = r % ga.T;
+#pragma unroll
+      for (int i = 0; i < NCH; ++i) {
+        float sa = 0.f, sb = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          sa = fmaf(v[i * 8 + j], wa[j], sa);
+          sb = fmaf(v[i * 8 + j], wb[j], sb);
         }
 #pragma unroll
         for (int o = 1; o < 8; o <<= 1) {
@@ -1455,6 +1595,47 @@ int b200s_relpos_table_fwd(const float* emb, const int* lut, int n, int H, float
 int b200s_relpos_table_bwd(const float* dtab, const int* lut, int n, int H, float* demb, b200s_stream stream) {
   B200_CHECK_ARG(dtab && lut && demb, "relpos_table_bwd: null pointer");
   B200_CHECK_CUDA(launch_pdl(relpos_table_bwd_kernel, dim3(ceil_div(n * H, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), dtab, lut, n, H, demb));
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
+}  // extern "C"
+
+extern "C" {
+
+// LayerNorm forward with an e4m3 output (and optionally bf16 y, statistics, the fused gate): the fp8 inference path.  The
+// warp-per-row kernel at every width, gate included (D = H * 64 in 256..1280).
+int b200s_layer_norm_fwd_fp8(const void* x, long long x_bs, long long x_rs, const float* gamma, const float* beta, void* y,
+                             long long y_bs, long long y_rs, float* mean, float* rstd, void* q, long long q_bs, long long q_rs,
+                             float* scale, int rows_per_batch, int batches, int D, const float* grep_w, const float* grep_b,
+                             const float* grep_a, int H, float* gate, const int* valid, b200s_stream stream) {
+  B200_CHECK_ARG(x && gamma && beta && q && scale, "layer_norm_fwd_fp8: null pointer");
+  B200_CHECK_ARG(!gate || (grep_w && grep_b && grep_a), "layer_norm_fwd_fp8: the gate needs grep_w, grep_b and grep_a");
+  B200_CHECK_ARG(!gate || (D == H * 64 && D >= 256 && D <= 1280), "layer_norm_fwd_fp8: the fused gate needs D = H*64 in 256..1280");
+  B200_CHECK_ARG(q_rs % 8 == 0 && q_bs % 8 == 0 && (reinterpret_cast<uintptr_t>(q) & 7) == 0,
+                 "layer_norm_fwd_fp8: e4m3 rows must be 8-byte aligned");
+  const long long rows = static_cast<long long>(rows_per_batch) * batches;
+  if (rows == 0) return 0;
+  RowView xv{x_bs, x_rs, rows_per_batch}, yv{y_bs, y_rs, rows_per_batch};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const GateArgs ga{grep_w, grep_b, grep_a, gate, H, rows_per_batch};
+  const Fp8Rows f8{static_cast<uint8_t*>(q), q_bs, q_rs, scale};
+  int rc = dispatch_width(D, [&](auto vec, auto nch) {
+    constexpr int V = decltype(vec)::value, NC = decltype(nch)::value;
+    if constexpr (V == 8) {
+      if (gate) {
+        B200_CHECK_CUDA(launch_pdl(ln_fwd_fp8_kernel<V, NC, true>, dim3(ln_fwd_grid(rows)), dim3(256), 0, st,
+                                   static_cast<const __nv_bfloat16*>(x), xv, gamma, beta, static_cast<__nv_bfloat16*>(y), yv, mean,
+                                   rstd, rows, 1e-5f, ga, f8, valid));
+        return 0;
+      }
+    }
+    B200_CHECK_CUDA(launch_pdl(ln_fwd_fp8_kernel<V, NC, false>, dim3(ln_fwd_grid(rows)), dim3(256), 0, st,
+                               static_cast<const __nv_bfloat16*>(x), xv, gamma, beta, static_cast<__nv_bfloat16*>(y), yv, mean,
+                               rstd, rows, 1e-5f, ga, f8, valid));
+    return 0;
+  });
+  if (rc) return rc;
   B200_CHECK_LAUNCH();
   return 0;
 }

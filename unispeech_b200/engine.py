@@ -180,6 +180,8 @@ class Engine:
         self.flat: Optional[FlatGrads] = None
         self._params = None
         self.drop: Optional[DR.DropState] = None  # set per forward pass by WavLM._begin (training-mode dropout)
+        self.lw8 = None  # e4m3 encoder weights + channel scales: allocated by the first fp8 call (prepare_fp8)
+        self.fp8_version = None
         self.grad_sync = None  # parallel.OverlappedGradSync: told when a stage of the backward pass has produced its gradients
 
     def backward_stage_done(self, stage):
@@ -274,6 +276,36 @@ class Engine:
                                    "move the model to its device before the first call")
         ops.prep_linear_batched(self.prep_descs, self.prep_n, self.prep_tiles)  # every nn.Linear operand, one launch
         self.prepared_version = ver
+
+    def prepare_fp8(self):
+        """fp32 masters -> e4m3 encoder projection weights with one scale per output channel (fused QKV, out_proj, fc1, fc2 of
+        every layer; one launch).  Allocated on the first call, so a model never run in fp8 holds no fp8 copy; re-derived when a
+        parameter changed, by the same version rule as `prepare()`."""
+        ver = self._param_version()
+        if ver == self.fp8_version:
+            return
+        m, cfg, dev = self.m, self.cfg, self.dev
+        D, Fd = cfg.encoder_embed_dim, cfg.encoder_ffn_embed_dim
+        if self.lw8 is None:
+            import struct
+            u8 = lambda *s: torch.empty(*s, dtype=torch.uint8, device=dev)
+            f = lambda n: torch.empty(n, dtype=torch.float32, device=dev)
+            self.lw8, recs = [], []
+            for lyr, w in zip(m.encoder.layers, self.lw):
+                w8 = dict(qkv=u8(3 * D, D), sqkv=f(3 * D), o=u8(D, D), so=f(D), w1=u8(Fd, D), s1=f(Fd), w2=u8(D, Fd), s2=f(D))
+                for src, (q, sc) in ((w["wqkv_master"], ("qkv", "sqkv")), (lyr.self_attn.out_proj.weight.data, ("o", "so")),
+                                     (lyr.fc1.weight.data, ("w1", "s1")), (lyr.fc2.weight.data, ("w2", "s2"))):
+                    recs.append(struct.pack("<QQQii", src.data_ptr(), w8[q].data_ptr(), w8[sc].data_ptr(), src.shape[0],
+                                            src.shape[1]))
+                self.lw8.append(w8)
+            self.prep8_descs = torch.frombuffer(bytearray(b"".join(recs)), dtype=torch.uint8).to(dev)
+            self.prep8_n, self.prep8_rows = len(recs), max(3 * D, Fd)
+        for kw, fw in self.prep_ptrs:  # the descriptor table holds raw master pointers: they must not have moved
+            if kw.data_ptr() != fw.data_ptr() + 4 * D * D:
+                raise RuntimeError("model parameters were re-allocated after the first GPU forward (e.g. .to()/.cuda()); "
+                                   "move the model to its device before the first call")
+        ops.prep_linear_fp8_batched(self.prep8_descs, self.prep8_n, self.prep8_rows)
+        self.fp8_version = ver
 
     def lut(self, T: int) -> torch.Tensor:
         if T not in self.lut_cache:
@@ -701,6 +733,92 @@ class Engine:
             st.update(qkv=qkv, gate=gate, ao=ao, lse=lse, y1=y1, x1=x1, ffn_in=ffn_in, hp=hp, hg=hg, y2=y2, tab=tab, pad=pad_u8,
                       dmask=dmask, rag=rag)
         return out, (st if save else None)
+
+    def layer_forward_fp8(self, idx: int, x: torch.Tensor, pad_u8, tab, rag=None, x8=None, gate=None):
+        """Inference-only `layer_forward` with the four projections (QKV, out_proj, fc1, fc2) as e4m3 GEMMs (`prepare_fp8`
+        operands): no saved state, no dropout; attention runs on the bf16 QKV output as in bf16.  `x8` = (q, scale): x already in
+        e4m3 (post-LN models: the previous layer's final LayerNorm wrote it), else x is quantised here; `gate`: the gate of this
+        layer's attention if that LayerNorm wrote it too.  Returns (out, (q, scale) of out or None, gate for layer idx + 1 or None):
+        post-LN models hand their e4m3 output and the next gate on to the next layer."""
+        m, cfg = self.m, self.cfg
+        lyr = m.encoder.layers[idx]
+        a = lyr.self_attn
+        w8 = self.lw8[idx]
+        B, T, D = x.shape
+        M = B * T
+        Fd, H = cfg.encoder_ffn_embed_dim, cfg.encoder_attention_heads
+        dev = x.device
+        e = lambda *s: torch.empty(*s, dtype=BF, device=dev)
+        u8 = lambda *s: torch.empty(*s, dtype=torch.uint8, device=dev)
+        f = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        pre_ln = cfg.layer_norm_first
+        want_gate = tab is not None and cfg.gru_rel_pos
+        fuse_gate = want_gate and D == H * 64 and 256 <= D <= 1280  # the LayerNorm kernel's fused gate (8 columns per lane)
+
+        def mm(a8, sa, K, wq, ws, N, out, **epi):
+            ops.gemm_rows_fp8(a8, sa, T * K, K, T, B, K, wq, ws, N, out, T * N, N,
+                              L.make_epilogue(**epi) if epi else None, valid=rag)
+
+        def quant(src, K):
+            q, sc = u8(B, T, K), f(M)
+            ops.quantize_rows_fp8(src, T * K, K, T, B, K, q, T * K, K, sc, valid=rag)
+            return q, sc
+
+        def ln8(src, ln, y=None, gate_out=None, attn=None):  # gate_out: the gate of `attn`, which consumes the output
+            q, sc = u8(B, T, D), f(M)
+            if gate_out is not None:
+                ops.layer_norm_fwd_fp8(src, T * D, D, ln.weight, ln.bias, y, T * D, D, None, None, q, T * D, D, sc, T, B, D,
+                                       attn.grep_linear.weight, attn.grep_linear.bias, attn.grep_a, H, gate_out, valid=rag)
+            else:
+                ops.layer_norm_fwd_fp8(src, T * D, D, ln.weight, ln.bias, y, T * D, D, None, None, q, T * D, D, sc, T, B, D,
+                                       valid=rag)
+            return q, sc
+
+        if pre_ln:
+            ln = lyr.self_attn_layer_norm
+            if want_gate and fuse_gate:
+                gate = f(B, H, T)
+                xq = ln8(x, ln, gate_out=gate, attn=a)
+            elif want_gate:  # the gate is computed from the bf16 LayerNorm output
+                xn = e(B, T, D)
+                xq = ln8(x, ln, y=xn)
+                gate = f(B, H, T)
+                ops.gate_fwd(xn, T * D, D, T, B, H, a.grep_linear.weight, a.grep_linear.bias, a.grep_a, gate)
+            else:
+                xq = ln8(x, ln)
+        else:
+            xq = x8 if x8 is not None else quant(x, D)
+            if want_gate and gate is None:  # no gate left behind by the producer of x (first layer, direct call)
+                gate = f(B, H, T)
+                ops.gate_fwd(x, T * D, D, T, B, H, a.grep_linear.weight, a.grep_linear.bias, a.grep_a, gate)
+        if not want_gate:
+            gate = None
+        qkv = e(B, T, 3 * D)
+        mm(*xq, D, w8["qkv"], w8["sqkv"], 3 * D, qkv, bias=self.lw[idx]["bqkv"])
+        ao, lse = e(B, T, D), f(B, H, T)
+        ops.attn_fwd(qkv, gate, tab, pad_u8, ao, lse, B, T, H, self.head_dim ** -0.5, head_dim=self.head_dim)
+        y1 = e(B, T, D)
+        mm(*quant(ao, D), D, w8["o"], w8["so"], D, y1, bias=a.out_proj.bias, res1=x, res1_ld=D, res1_bs=T * D)
+        if pre_ln:
+            x1 = y1
+            ffn_q = ln8(x1, lyr.final_layer_norm)
+        else:
+            x1 = e(B, T, D)
+            ffn_q = ln8(y1, lyr.self_attn_layer_norm, y=x1)
+        hg = e(B, T, Fd)
+        mm(*ffn_q, D, w8["w1"], w8["s1"], Fd, hg, bias=lyr.fc1.bias, gelu=2)
+        y2 = e(B, T, D)
+        mm(*quant(hg, Fd), Fd, w8["w2"], w8["s2"], D, y2, bias=lyr.fc2.bias, res1=x1, res1_ld=D, res1_bs=T * D)
+        if pre_ln:
+            return y2, None, None
+        out = e(B, T, D)
+        next_gate = None
+        if want_gate and fuse_gate and idx + 1 < len(m.encoder.layers):  # `out` is the next layer's input: leave its gate behind
+            next_gate = f(B, H, T)
+            out_q = ln8(y2, lyr.final_layer_norm, y=out, gate_out=next_gate, attn=m.encoder.layers[idx + 1].self_attn)
+        else:
+            out_q = ln8(y2, lyr.final_layer_norm, y=out)
+        return out, out_q, next_gate
 
     def layer_backward(self, idx: int, st, dout: torch.Tensor, dtab):
         m, cfg = self.m, self.cfg

@@ -70,6 +70,25 @@ def gemm_rows(a, a_bs, a_rs, rows, batches, K, w, N, out, out_bs, out_ld, epi: O
           flops=2.0 * rows * batches * K * N)
 
 
+def gemm_rows_fp8(a8, a_scale, a_bs, a_rs, rows, batches, K, w8, w_scale, N, out, out_bs, out_ld,
+                  epi: Optional[L.Epilogue] = None, valid=None):
+    """e4m3 row GEMM with per-row (`a_scale`, [batches * rows]) and per-channel (`w_scale`, [N]) scales; strides of `a8` in bytes.
+    `valid` (int32 [batches] on the device): ragged batch -- M tiles beyond an utterance's valid frames are zero-filled."""
+    _call("b200s_gemm_rows_fp8", L.ptr(a8), L.ptr(a_scale), L.ll(a_bs), L.ll(a_rs), i32(rows), i32(batches), i32(K), L.ptr(w8),
+          L.ptr(w_scale), i32(N), L.ptr(out), L.ll(out_bs), L.ll(out_ld), C.addressof(epi) if epi is not None else None,
+          L.ptr(valid), _s(), flops=2.0 * rows * batches * K * N)
+
+
+def quantize_rows_fp8(x, x_bs, x_rs, rows, batches, D, q, q_bs, q_rs, scale, valid=None):
+    """bf16 rows -> e4m3 rows (byte strides q_bs, q_rs) + one scale per row; rows at or past valid[b] become zeros, s = 0."""
+    _call("b200s_quantize_rows_fp8", L.ptr(x), L.ll(x_bs), L.ll(x_rs), i32(rows), i32(batches), i32(D), L.ptr(q), L.ll(q_bs),
+          L.ll(q_rs), L.ptr(scale), L.ptr(valid), _s(), nbytes=3.0 * rows * batches * D)
+
+
+def prep_linear_fp8_batched(descs, n_descs, max_rows):
+    _call("b200s_prep_linear_fp8_batched", L.ptr(descs), i32(n_descs), i32(max_rows), _s())
+
+
 def gemm_wgrad(y, y_bs, y_rs, x, x_bs, x_rs, rows, batches, N, K, dw, dw_ld, valid=None):
     """`valid` (int32 [batches] on the device): ragged batch -- row blocks beyond an utterance's valid frames are skipped."""
     if valid is not None:
@@ -120,6 +139,16 @@ def layer_norm_gate_fwd(x, x_bs, x_rs, gamma, beta, y, y_bs, y_rs, mean, rstd, T
         _call("b200s_layer_norm_gate_fwd_ragged", L.ptr(x), L.ll(x_bs), L.ll(x_rs), L.ptr(gamma), L.ptr(beta), L.ptr(y),
               L.ll(y_bs), L.ll(y_rs), L.ptr(mean), L.ptr(rstd), i32(T), i32(B), i32(D), L.ptr(grep_w), L.ptr(grep_b),
               L.ptr(grep_a), i32(H), L.ptr(gate), L.ptr(valid), _s(), nbytes=nb)
+
+
+def layer_norm_fwd_fp8(x, x_bs, x_rs, gamma, beta, y, y_bs, y_rs, mean, rstd, q, q_bs, q_rs, scale, rows_per_batch, batches, D,
+                       grep_w=None, grep_b=None, grep_a=None, H=0, gate=None, valid=None):
+    """LayerNorm with an e4m3 output (q, byte strides, one scale per row); `y`, `mean`, `rstd` may be None; `gate` (fp32
+    [B, H, T]) also writes the gru_rel_pos gate of the consuming attention."""
+    _call("b200s_layer_norm_fwd_fp8", L.ptr(x), L.ll(x_bs), L.ll(x_rs), L.ptr(gamma), L.ptr(beta), L.ptr(y), L.ll(y_bs),
+          L.ll(y_rs), L.ptr(mean), L.ptr(rstd), L.ptr(q), L.ll(q_bs), L.ll(q_rs), L.ptr(scale), i32(rows_per_batch), i32(batches),
+          i32(D), L.ptr(grep_w), L.ptr(grep_b), L.ptr(grep_a), i32(H), L.ptr(gate), L.ptr(valid), _s(),
+          nbytes=3.0 * rows_per_batch * batches * D)
 
 
 def layer_norm_bwd(dy, dy_bs, dy_rs, x, x_bs, x_rs, mean, rstd, gamma, beta, dres, dres_bs, dres_rs, dx, dx_bs, dx_rs,

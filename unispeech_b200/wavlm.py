@@ -91,6 +91,20 @@ def _check_supported(cfg):
 # ----------------------------------------------------------------------------------------------------------------
 # autograd glue: each Function runs the kernels of one stage and stashes what its backward needs
 # ----------------------------------------------------------------------------------------------------------------
+def _check_fp8_call(model, params=None):
+    """The fp8 path is inference only (no backward): raised before anything touches the device."""
+    if model.training:
+        raise RuntimeError("fp8=True is an inference path: call model.eval() first")
+    if torch.is_grad_enabled() and any(p.requires_grad for p in (params if params is not None else model.parameters())):
+        raise RuntimeError("fp8=True is an inference path without a backward: run it under torch.no_grad() / "
+                           "torch.inference_mode(), or with parameters that do not require grad")
+
+
+def _fp8_tag(t):
+    """What identifies a layer output for the fp8 hand-off: its memory (views share it) and its version counter."""
+    return (t.data_ptr(), tuple(t.shape), t.stride(), t._version)
+
+
 def _on_forward_stream(bwd):
     """Run a Function's backward on the stream its forward ran on (explicitly: the kernels are launched through ctypes on
     `torch.cuda.current_stream()`, and the autograd worker thread must not fall back to the legacy default stream -- this is
@@ -352,11 +366,13 @@ class TransformerSentenceEncoderLayer(nn.Module):
         self._owner = None  # set by WavLM (list wrapper, so the owner is not registered as a sub-module)
 
     def forward(self, x, self_attn_mask=None, self_attn_padding_mask=None, need_weights=False, pos_bias=None,
-                valid_frames=None):
+                valid_frames=None, fp8=False):
         """x: T x B x C.  `pos_bias` carries the shared relative-position state between layers (the reference passes the
         materialised [B*H,T,T] bias tensor here; we pass the per-head Toeplitz table instead).  `valid_frames` (int32 [B] on
         the device, with a padding mask only): frames of every utterance up to its last valid one; the row GEMMs and LayerNorms
-        then skip the padded tail and write zeros there.  Returns (x, None, pos_bias)."""
+        then skip the padded tail and write zeros there.  `fp8` (inference only, see WavLM.extract_features): the projections
+        run as e4m3 GEMMs, and `pos_bias` (then always a dict) also carries this layer's e4m3 output to the next layer.
+        Returns (x, None, pos_bias)."""
         assert self_attn_mask is None, "streaming / attention masks are not supported"
         model = self._owner[0]
         eng = model._engine_for(x.device)
@@ -370,7 +386,30 @@ class TransformerSentenceEncoderLayer(nn.Module):
             pad_u8, rag = pad_u8.contiguous(), valid_frames
         if pos_bias is None and model.encoder.relative_position_embedding:
             pos_bias = model.encoder._make_bias_state(T, x.device)
+        if fp8:
+            return self._forward_fp8(eng, xb, pad_u8, pos_bias, rag)
         out = _LayerFn.apply(xb, self.fc1.weight, eng, self.index, pad_u8, pos_bias, rag)
+        return out.transpose(0, 1), None, pos_bias
+
+    def _forward_fp8(self, eng, xb, pad_u8, pos_bias, rag):
+        """The fp8 layer call.  The previous layer's e4m3 copy of its output (and the gate it computed for this layer) travel in
+        `pos_bias["fp8_next"]`, tagged with the output's storage (address, shape, strides) and version counter: they are used only
+        if `xb` views that same memory, unmodified -- `xb` is a new view of it (the layers pass T x B x C transposes), so identity
+        cannot be the test.  A forward hook that replaced the output or modified it in place (the version counter is shared by all
+        views) makes this layer quantise its input itself."""
+        if pos_bias is None:
+            pos_bias = {"tab": None}
+        if not pos_bias.get("fp8_ready"):  # a direct layer call: check it, and make sure the e4m3 weights match the masters
+            _check_fp8_call(self._owner[0])
+            eng.prepare_fp8()
+        x8 = gate = None
+        nxt = pos_bias.pop("fp8_next", None)
+        if nxt is not None and nxt[0] == _fp8_tag(xb):
+            x8, gate = nxt[1], nxt[2]
+        with torch.no_grad():
+            out, out8, next_gate = eng.layer_forward_fp8(self.index, xb, pad_u8, pos_bias.get("tab"), rag, x8, gate)
+        if out8 is not None:
+            pos_bias["fp8_next"] = (_fp8_tag(out), out8, next_gate, out)  # (out held: its memory cannot be reused meanwhile)
         return out.transpose(0, 1), None, pos_bias
 
 
@@ -420,11 +459,12 @@ class TransformerEncoder(nn.Module):
         dtab = torch.zeros(H, 2 * T - 1, dtype=torch.float32, device=device) if torch.is_grad_enabled() else None
         return dict(tab=tab, dtab=dtab, lut=lut, has_first=False)
 
-    def forward(self, x, padding_mask=None, streaming_mask=None, layer=None, extract_layer=None, *, _xpad=None, _valid=None):
+    def forward(self, x, padding_mask=None, streaming_mask=None, layer=None, extract_layer=None, *, _xpad=None, _valid=None,
+                fp8=False):
         """Returns (x, layer_results) like the reference WavLM encoder; with `extract_layer` (UniSpeech-SAT encoder,
         unispeech_sat.py:1202-1210) a third value: that layer's output, normalised by `layer_norm_for_extract` for pre-LN models.
         `_xpad` and `_valid` come from WavLM._extract only (see `_encode`)."""
-        res = self._encode(x, padding_mask, streaming_mask, layer, extract_layer, _xpad, _valid)
+        res = self._encode(x, padding_mask, streaming_mask, layer, extract_layer, _xpad, _valid, fp8)
         x, layer_results = res[0], res[1]
         er = res[2] if extract_layer is not None else None
         if self.layer_norm_first and layer is None:
@@ -445,7 +485,7 @@ class TransformerEncoder(nn.Module):
         (UniSpeech-SAT encoder, unispeech_sat.py:1236-1255)."""
         return self._encode(x, padding_mask, streaming_mask, tgt_layer, extract_layer)
 
-    def _encode(self, x, padding_mask, streaming_mask, tgt_layer, extract_layer, xpad=None, valid=None):
+    def _encode(self, x, padding_mask, streaming_mask, tgt_layer, extract_layer, xpad=None, valid=None, fp8=False):
         """`extract_features` body.  From WavLM._extract, `x` is a view of `xpad`, the zero-padded pos_conv input buffer
         the projection wrote, and `valid` (int32 [B] or None) the ragged lengths the layers skip the padded tails with."""
         assert streaming_mask is None, "streaming masks are not supported"
@@ -474,11 +514,17 @@ class TransformerEncoder(nn.Module):
         r = None
         er = None
         pos_bias = self._make_bias_state(T, x.device) if self.relative_position_embedding else None
+        if fp8:
+            _check_fp8_call(model, eng._params)
+            eng.prepare_fp8()
+            pos_bias = dict(pos_bias or {"tab": None}, fp8_ready=True)
+        lkw = dict(fp8=True) if fp8 else {}
         pad_u8 = padding_mask.to(torch.uint8).contiguous() if padding_mask is not None else None
         for i, layer in enumerate(self.layers):
             dropout_probability = np.random.random()
             if not self.training or (dropout_probability > self.layerdrop):
-                x, _z, pos_bias = layer(x, self_attn_padding_mask=pad_u8, need_weights=False, pos_bias=pos_bias, valid_frames=valid)
+                x, _z, pos_bias = layer(x, self_attn_padding_mask=pad_u8, need_weights=False, pos_bias=pos_bias, valid_frames=valid,
+                                        **lkw)
             if tgt_list is not None:
                 if i + 1 in tgt_list:
                     layer_results.append((x, None))
@@ -637,18 +683,27 @@ class WavLM(nn.Module):
         return padding_mask.all(-1)
 
     def extract_features(self, source, padding_mask=None, mask=False, ret_conv=False, output_layer=None,
-                         ret_layer_results=False, mask_indices=None, mask_channel_indices=None):
+                         ret_layer_results=False, mask_indices=None, mask_channel_indices=None, *, fp8=False):
         """Same contract as the reference.  `mask_indices` (bool [B,T], optional) and `mask_channel_indices` (bool [B,D],
         optional) let a caller inject the masked frames and channels instead of sampling them (used by the parity tests and the
         CUDA graph; the reference's sampler is host numpy RNG).  With `mask=True` both are sampled when neither is given;
-        once either is given, the other one given as None means no mask of that kind."""
-        res = self._extract(source, padding_mask, mask, ret_conv, output_layer, mask_indices, mask_channel_indices)
+        once either is given, the other one given as None means no mask of that kind.
+        `fp8=True` (inference: eval mode, no gradient): the encoder layers' QKV, out_proj, fc1 and fc2 projections run as e4m3
+        GEMMs with per-row activation and per-channel weight scales (the conv stack, post_extract_proj, pos_conv, attention and the
+        LayerNorms stay bf16 / fp32).  RuntimeError in training mode, with gradients enabled on a model that requires them, or
+        with `mask=True`."""
+        if fp8:
+            _check_fp8_call(self)
+            if mask:
+                raise RuntimeError("extract_features(fp8=True) is an inference path: mask=True is not supported")
+        res = self._extract(source, padding_mask, mask, ret_conv, output_layer, mask_indices, mask_channel_indices, fp8=fp8)
         feature = res["features"] if ret_conv else res["x"]
         if ret_layer_results:
             feature = (feature, res["layer_results"])
         return feature, res["padding_mask"]
 
-    def _extract(self, source, padding_mask, mask, ret_conv, output_layer, mask_indices, mask_channel_indices, frames=None):
+    def _extract(self, source, padding_mask, mask, ret_conv, output_layer, mask_indices, mask_channel_indices, frames=None,
+                 fp8=False):
         """The forward pass behind `extract_features` and the models' `forward`: returns everything one call produced as a dict
         (`x`, `padding_mask`, `features`, `layer_results`, `mask_indices`, `mask_channel_indices`, `padding_mask_host`, `spk_x`,
         `unmasked_features`, `features_pen`).  `frames` (pre-training with labels shorter than the conv frames,
@@ -697,7 +752,7 @@ class WavLM(nn.Module):
                                                         self._want_unmasked_features, chan_u8)
         el, pl = self._extract_layer, self._predict_layers
         lay = (list(pl) if (pl is not None and output_layer is None) else None) if output_layer is None else output_layer - 1
-        enc = self.encoder(xv, padding_mask=fpm, layer=lay, extract_layer=el, _xpad=proj_st["xpad"], _valid=valid)
+        enc = self.encoder(xv, padding_mask=fpm, layer=lay, extract_layer=el, _xpad=proj_st["xpad"], _valid=valid, fp8=fp8)
         return {"x": enc[0], "padding_mask": fpm, "features": features, "layer_results": enc[1],
                 "mask_indices": mask_indices, "mask_channel_indices": mask_channel_indices, "padding_mask_host": fpm_host,
                 "spk_x": enc[2] if el is not None else None, "unmasked_features": unmasked, "features_pen": pen}
