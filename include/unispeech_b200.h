@@ -454,6 +454,31 @@ int b200s_ctc_beta_grad(const void* logits, long long frame_stride, long long ba
                         const float* nll, const float* upstream, void* grad, long long grad_frame_stride,
                         long long grad_batch_stride, int Vpad, b200s_stream stream);
 
+/* ============================ CTC forced alignment (csrc/ctc_align.cu) ============================ */
+/* The most probable CTC path of each utterance's known transcript (torchaudio.functional.forced_align, batched): Viterbi over
+ * the extended sequence l' = (blank, l_1, blank, ..., l_S, blank) with lp[t,c] = float(logit[t,c]) - lse[t] in fp32, lse from
+ * b200s_ctc_stats.  Logits, input_len, targets and target_len are addressed as in the CTC loss entry points above (frames
+ * t >= input_len[b] are never read).
+ * Tie rule (torchaudio's CPU implementation, reproduced bit for bit): at each (frame, position) the predecessor is skip (s-2)
+ * if skip > advance && skip > stay, else advance (s-1) if advance > stay && advance > skip, else stay (s) -- strict
+ * comparisons, so exact ties go to stay, and advance == skip > stay takes stay.  The path ends at the final blank if its alpha
+ * is strictly larger than the last label's, else at the last label.
+ * Outputs: labels int32 [B, T] (class per frame on the path), frame_scores fp32 [B, T] (lp at that class), score fp32 [B]
+ * (alpha at the end position: the sum of frame_scores up to fp32 reassociation).  Frames t >= input_len[b] get (-1, 0).  An
+ * INFEASIBLE utterance (input_len < S + number of equal adjacent labels, target_len outside [0, Smax], a label outside [0, V)
+ * or equal to blank) gets labels -1 and frame_scores 0 on every frame and score -inf; the others are unaffected.  S = 0 aligns
+ * every valid frame to blank (score 0 when input_len = 0).
+ * workspace: caller-allocated 2-bit backpointers, b200s_ctc_align_workspace_bytes(B, T, Smax) =
+ *   B * T * ceil((2 * Smax + 1) / 16) * 4 bytes (one 32-bit word per 16 positions per frame).
+ * Limits, checked before any launch: 1 <= V <= 1024, 0 <= blank < V, 0 <= Smax <= B200S_CTC_ALIGN_MAX_TARGET, workspace_bytes
+ * at least the size above.  Two launches (Viterbi, backtrack), no floating-point atomics: results are bit-identical from call
+ * to call and do not depend on the other utterances of the batch. */
+#define B200S_CTC_ALIGN_MAX_TARGET 8191
+long long b200s_ctc_align_workspace_bytes(int B, int T, int Smax); /* -1 for bad sizes */
+int b200s_ctc_align(const void* logits, long long frame_stride, long long batch_stride, const float* lse, const int* input_len,
+                    const int* targets, int Smax, const int* target_len, int B, int T, int V, int blank, void* workspace,
+                    long long workspace_bytes, int* labels, float* frame_scores, float* score, b200s_stream stream);
+
 /* ============================ k-means pseudo-labels (csrc/kmeans.cu) ============================ */
 /* Nearest-centroid labels, Lloyd updates and k-means++ seeding over bf16 features (the label stage of HuBERT-style pre-training).
  * Centres: fp32 master [K, D]; the bf16 copy the assignment multiplies, [Kp, D] with Kp = K rounded up to a multiple of 256 (rows

@@ -8,6 +8,10 @@ src/fairseq/models/wav2vec/wav2vec2_asr.py `Wav2VecCtc`).
     fine-tuning wrappers return over their [B*T, Vp] buffer is consumed, and its gradient produced, without a copy.  The loss stays
     on the device; nothing synchronises, so a fixed-shape fine-tuning step captures in a CUDA graph.
   * `CtcCriterion`: `forward(model, sample) -> (loss, sample_size, logging_output)` with the reference's contract (below).
+  * `forced_align(logits_tbv, input_len, targets, target_len, blank)`: the most probable CTC path of each utterance's known
+    transcript (csrc/ctc_align.cu), bit for bit what `torchaudio.functional.forced_align` returns for each utterance on
+    lp = logits - logsumexp(logits) in fp32, but batched, on the bf16 logits themselves and for transcripts of up to
+    `MAX_ALIGN_TARGET` labels.  `token_spans` turns its paths into per-token frame spans (`torchaudio.functional.merge_tokens`).
   * `HubertCtc` / `Wav2VecCtc`: `w2v_encoder` = `HubertEncoder` / `Wav2VecEncoder`, `forward(**net_input)`, `get_logits`,
     `get_normalized_probs`, `set_num_updates`; `state_dict` keys `w2v_encoder.w2v_model.*`, `w2v_encoder.proj.*`.
 
@@ -18,7 +22,7 @@ unspecified without it); `zero_infinity` additionally replaces its +inf by 0 in 
 """
 from __future__ import annotations
 
-from typing import List, Optional
+from typing import List, NamedTuple, Optional
 
 import torch
 import torch.nn as nn
@@ -31,6 +35,7 @@ from .wavlm import _on_forward_stream
 
 MAX_TARGET = 511   # B200S_CTC_MAX_TARGET: one thread per position of the extended label sequence, 2 * 511 + 1 <= 1024
 MAX_CLASSES = 1024
+MAX_ALIGN_TARGET = 8191   # B200S_CTC_ALIGN_MAX_TARGET: up to 32 positions of the extended label sequence per thread, 512 threads
 
 
 class _CtcFn(torch.autograd.Function):
@@ -137,6 +142,70 @@ def greedy_collapse(argmax: torch.Tensor, input_len, blank: int = 0) -> List[Lis
             prev = c
         hyps.append(out)
     return hyps
+
+
+def forced_align(logits_tbv: torch.Tensor, input_len: torch.Tensor, targets: torch.Tensor, target_len: torch.Tensor,
+                 blank: int = 0):
+    """CTC forced alignment of bf16 logits T x B x V (log-softmax included) to padded `targets` [B, Smax] with lengths
+    `target_len` [B] over `input_len` [B] valid frames -- the same inputs as `ctc_loss`.
+
+    Returns (labels int32 [B, T], frame_scores fp32 [B, T], score fp32 [B]), all on the logits' device: the class of each frame
+    on the most probable path through (blank, l_1, blank, ..., l_S, blank), lp = logit - logsumexp(logit) (fp32) at that class,
+    and the path's log-probability.  Per utterance these are bit-identical to `torchaudio.functional.forced_align` (CPU) on the
+    same fp32 lp, ties included.  Frames past input_len get (-1, 0).  An infeasible utterance (input too short for its target
+    with one blank between equal neighbours, target_len outside [0, Smax], a label outside [0, V) or equal to blank) gets -1 on
+    every frame and score -inf instead of an error, so nothing is read back: the call captures in a CUDA graph.  Limits:
+    Smax <= MAX_ALIGN_TARGET, V <= MAX_CLASSES.  The backpointer workspace, B * T * ceil((2 Smax + 1) / 16) * 4 bytes, comes
+    from the caching allocator."""
+    if not logits_tbv.is_cuda or logits_tbv.dtype != BF or logits_tbv.dim() != 3:
+        raise ValueError("forced_align: logits must be a CUDA bf16 tensor T x B x V (there is no CPU or fp32 path)")
+    if logits_tbv.stride(2) != 1:
+        raise ValueError("forced_align: the class dimension of the logits must have unit stride")
+    if targets.dim() != 2 or targets.shape[0] != logits_tbv.shape[1]:
+        raise ValueError(f"forced_align: targets must be [B, Smax] padded, got {tuple(targets.shape)}")
+    dev = logits_tbv.device
+    T, B, V = logits_tbv.shape
+    fs, bs = logits_tbv.stride(0), logits_tbv.stride(1)
+    Smax = targets.shape[1]
+    input_len, targets, target_len = _i32(input_len, dev), _i32(targets, dev), _i32(target_len, dev)
+    lse = torch.empty(B, T, dtype=torch.float32, device=dev)
+    labels = torch.empty(B, T, dtype=torch.int32, device=dev)
+    frame_scores = torch.empty(B, T, dtype=torch.float32, device=dev)
+    score = torch.empty(B, dtype=torch.float32, device=dev)
+    ws = ops.ctc_align_workspace_bytes(B, T, Smax)   # -1 past the limits: the call below then reports which one
+    workspace = torch.empty(max(ws, 1), dtype=torch.uint8, device=dev)
+    ops.ctc_stats(logits_tbv, fs, bs, input_len, B, T, V, lse, None)
+    ops.ctc_align(logits_tbv, fs, bs, lse, input_len, targets, Smax, target_len, B, T, V, int(blank), workspace, labels,
+                  frame_scores, score)
+    return labels, frame_scores, score
+
+
+class TokenSpan(NamedTuple):
+    """One token of an aligned path: frames [start, end) (end exclusive), score = mean frame score over them."""
+    token: int
+    start: int
+    end: int
+    score: float
+
+
+def token_spans(labels: torch.Tensor, frame_scores: torch.Tensor, input_len, blank: int = 0) -> List[List[TokenSpan]]:
+    """Per-token spans of `forced_align` paths (host side), with `torchaudio.functional.merge_tokens` semantics on each
+    utterance's first input_len[b] frames: runs of equal classes are merged, blank runs dropped, and each span's score is the
+    mean of its frame scores.  An infeasible utterance (labels -1) has no spans.  Frames are the model's output frames: 320
+    samples (20 ms) apart at 16 kHz, so frame f starts at f * 320 / 16000 seconds."""
+    labels, frame_scores = labels.cpu(), frame_scores.cpu()
+    out = []
+    for b, n in enumerate(int(v) for v in input_len):
+        n = min(max(n, 0), labels.shape[1])
+        tok, sc = labels[b, :n], frame_scores[b, :n]
+        if n == 0 or bool((tok < 0).any()):
+            out.append([])
+            continue
+        edge = torch.tensor([-1], dtype=tok.dtype)
+        cuts = torch.nonzero(torch.diff(tok, prepend=edge, append=edge) != 0).flatten().tolist()
+        toks = tok.tolist()
+        out.append([TokenSpan(toks[s], s, e, sc[s:e].mean().item()) for s, e in zip(cuts[:-1], cuts[1:]) if toks[s] != blank])
+    return out
 
 
 class CtcCriterion(nn.Module):

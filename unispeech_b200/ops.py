@@ -430,6 +430,18 @@ def ctc_beta_grad(logits, frame_stride, batch_stride, lse, input_len, targets, S
           L.ptr(upstream), L.ptr(grad), L.ll(grad_frame_stride), L.ll(grad_batch_stride), i32(Vpad), _s())
 
 
+
+# ------------------------------------------------------------------------------------------------- CTC forced alignment
+def ctc_align_workspace_bytes(B, T, Smax) -> int:
+    return int(L.load().b200s_ctc_align_workspace_bytes(i32(B), i32(T), i32(Smax)))
+
+
+def ctc_align(logits, frame_stride, batch_stride, lse, input_len, targets, Smax, target_len, B, T, V, blank, workspace, labels,
+              frame_scores, score):
+    _call("b200s_ctc_align", L.ptr(logits), L.ll(frame_stride), L.ll(batch_stride), L.ptr(lse), L.ptr(input_len), L.ptr(targets),
+          i32(Smax), L.ptr(target_len), i32(B), i32(T), i32(V), i32(blank), L.ptr(workspace), L.ll(workspace.numel()),
+          L.ptr(labels), L.ptr(frame_scores), L.ptr(score), _s())
+
 # ------------------------------------------------------------------------------------------------- k-means pseudo-labels
 def kmeans_assign(x, x_bs, x_rs, rows, batches, D, valid, centers_bf16, cnorm, K, labels, score=None, prev_labels=None,
                   changed=None):
