@@ -479,6 +479,60 @@ int b200s_ctc_align(const void* logits, long long frame_stride, long long batch_
                     const int* targets, int Smax, const int* target_len, int B, int T, int V, int blank, void* workspace,
                     long long workspace_bytes, int* labels, float* frame_scores, float* score, b200s_stream stream);
 
+/* ============================ CTC beam-search decoding (csrc/ctc_decode.cu) ============================ */
+/* CTC prefix beam search (Hannun et al. 2014) with optional word n-gram LM scoring, batched over utterances; the definition is
+ * oracle/decode_oracle.py.  Logits and input_len are addressed as in b200s_ctc_align (frames t >= input_len[b] are never read),
+ * lp[t,c] = float(logit[t,c]) - lse[t] in fp32, lse from b200s_ctc_stats.  lae(a, b) = max + log1p(exp(-|a - b|)) in fp32.
+ *
+ * Hash: h' = splitmix64(h ^ (x + 1)) from h = 0 (splitmix64: z += 0x9E3779B97F4A7C15; z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9;
+ * z = (z ^ z >> 27) * 0x94D049BB133111EB; z ^ z >> 31).  A prefix is identified by the hash of its class ids, a spelling by the
+ * hash of its class ids, an n-gram by the hash of its word ids (oldest first).
+ * Beam state: pb, pnb (log-probabilities of the prefix ending in blank / in its last class), lm (LM part), the prefix hash, the
+ * partial word's hash (0 when empty), the last class, the last order - 1 words (starting at <s>).  Start: the empty prefix,
+ * pb = 0, pnb = -inf, lm = 0.  Per frame, with T_K = the beam_token non-blank classes of highest lp (ties to the smaller id):
+ *   stay of every beam:           pb' = lae(pb, pnb) + lp[blank];  pnb' = pnb + lp[last] (-inf for the empty prefix);
+ *   extension of beam j by c in T_K: prefix + c receives (c == last_j ? pb_j : lae(pb_j, pnb_j)) + lp[c] into pnb.
+ *   An extension reaching a prefix that is already a beam is merged into its stay (pnb' = lae(pnb', ext)); stays first, then
+ *   extensions by parent rank, then class id.  Ranking score = lae(pb, pnb) + lm, order by (score desc, prefix hash asc), keep the
+ *   best `beam` after every frame.
+ * LM (word level, KenLM's ARPA semantics): appending word_boundary after a non-empty partial word ends the word:
+ *   lm += lm_weight * ln P(word | context) + word_score (in that fp32 order), and the word joins the context.  ln P = ln 10 * (the
+ *   backoffs, log10, of the longer contexts that matched no n-gram, summed from the longest down, then the log10 p of the
+ *   longest n-gram that exists).  The spelling table maps the class ids of each LM word's spelling to its id, each character
+ *   spelled by the FIRST class whose symbol is that single character (the boundary excluded): a partial word is a known word
+ *   only if its class ids are exactly that spelling, so a later class with a repeated symbol, or a multi-character symbol,
+ *   spells no known word.  A spelling that is not in the spelling table is the word `unk`: it adds unk_score after
+ *   word_score, and its LM term is 0 when has_unk is 0 (the ARPA file has no <unk>).  An empty word (a leading boundary, or
+ *   boundary blank boundary) scores nothing.  After the last frame a non-empty partial word is scored the same way, then
+ *   lm += lm_weight * ln P(</s> | context); score = lae(pb, pnb) + lm.  With order = 0 there is no LM and word_boundary is unused.
+ * Candidate pruning: each beam is extended only by the min(beam_token, beam + 2) classes of T_K with the highest lp and the
+ * boundary class; this can differ from the full candidate set only where exact score ties straddle the beam cutoff.
+ * Outputs: tokens int32 [B, nbest, T] (class ids, blanks removed and repeats collapsed, -1 after the end), lengths int32
+ * [B, nbest], scores fp32 [B, nbest], best first.  Entries past the number of surviving beams have length 0 and score -inf.
+ * workspace: (parent slot | (appended class + 1) << 8) per (b, t, slot), b200s_ctc_decode_workspace_bytes(B, T, beam) =
+ * B * T * beam * 4 bytes.
+ * Limits, checked before any launch: 2 <= V <= 1024, 0 <= blank < V, 1 <= beam <= B200S_CTC_DECODE_MAX_BEAM,
+ * 1 <= nbest <= beam, 1 <= beam_token <= V - 1, 0 <= order <= B200S_CTC_LM_MAX_ORDER, word_boundary in [0, V) and != blank
+ * with an LM, table capacities powers of two, workspace_bytes at least the size above.  Two launches (search, backtrack), no
+ * floating-point atomics: results are bit-identical from call to call and do not depend on the other utterances.
+ *
+ * b200s_ctc_lm_table_build: inserts n entries into an open-addressing table (keys uint64 [capacity], zero-filled by the caller;
+ * vals two uint32 per slot): key = the hash of seqs[i, :] (width ints, ended by the first negative one), value = (v0[i], v1[i]
+ * or 0).  capacity: a power of two above n.  *status |= 1 when a key is 0 or already present (a 64-bit collision: the caller
+ * passes no duplicate sequences), |= 2 when the table is full.  n-gram table: (log10 p, log10 backoff) as fp32 bits; spelling
+ * table: (word id, 0). */
+#define B200S_CTC_DECODE_MAX_BEAM 128
+#define B200S_CTC_LM_MAX_ORDER 5
+long long b200s_ctc_decode_workspace_bytes(int B, int T, int beam); /* -1 for bad sizes */
+int b200s_ctc_lm_table_build(const int* seqs, int n, int width, const uint32_t* v0, const uint32_t* v1, void* keys, void* vals,
+                             long long capacity, int* status, b200s_stream stream);
+int b200s_ctc_decode(const void* logits, long long frame_stride, long long batch_stride, const float* lse, const int* input_len,
+                     int B, int T, int V, int blank, int beam, int nbest, int beam_token, int word_boundary, const void* lm_keys,
+                     const void* lm_vals, long long lm_capacity, const void* spell_keys, const void* spell_vals,
+                     long long spell_capacity, int order, int bos, int eos, int unk, int has_unk, float lm_weight,
+                     float word_score, float unk_score, void* workspace, long long workspace_bytes, int* tokens, int* lengths,
+                     float* scores, b200s_stream stream);
+
 /* ============================ k-means pseudo-labels (csrc/kmeans.cu) ============================ */
 /* Nearest-centroid labels, Lloyd updates and k-means++ seeding over bf16 features (the label stage of HuBERT-style pre-training).
  * Centres: fp32 master [K, D]; the bf16 copy the assignment multiplies, [Kp, D] with Kp = K rounded up to a multiple of 256 (rows

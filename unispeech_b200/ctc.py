@@ -12,6 +12,9 @@ src/fairseq/models/wav2vec/wav2vec2_asr.py `Wav2VecCtc`).
     transcript (csrc/ctc_align.cu), bit for bit what `torchaudio.functional.forced_align` returns for each utterance on
     lp = logits - logsumexp(logits) in fp32, but batched, on the bf16 logits themselves and for transcripts of up to
     `MAX_ALIGN_TARGET` labels.  `token_spans` turns its paths into per-token frame spans (`torchaudio.functional.merge_tokens`).
+  * `ctc_beam_search(logits_tbv, input_len, beam_size, nbest, blank, beam_size_token, lm, lm_weight, word_score, unk_score)`:
+    batched CTC prefix beam search (csrc/ctc_decode.cu) with an optional word n-gram LM (`ngram.NgramLM.from_arpa`) scored at
+    word boundaries, lexicon-free; `hypotheses_to_words` spells the result.
   * `HubertCtc` / `Wav2VecCtc`: `w2v_encoder` = `HubertEncoder` / `Wav2VecEncoder`, `forward(**net_input)`, `get_logits`,
     `get_normalized_probs`, `set_num_updates`; `state_dict` keys `w2v_encoder.w2v_model.*`, `w2v_encoder.proj.*`.
 
@@ -178,6 +181,71 @@ def forced_align(logits_tbv: torch.Tensor, input_len: torch.Tensor, targets: tor
     ops.ctc_align(logits_tbv, fs, bs, lse, input_len, targets, Smax, target_len, B, T, V, int(blank), workspace, labels,
                   frame_scores, score)
     return labels, frame_scores, score
+
+
+class CtcHypotheses(NamedTuple):
+    """`ctc_beam_search` result, best first per utterance: tokens int32 [B, nbest, T] (class ids, no blanks, repeats collapsed,
+    -1 past `lengths`), lengths int32 [B, nbest], scores fp32 [B, nbest] (-inf, length 0 where fewer beams survived)."""
+    tokens: torch.Tensor
+    lengths: torch.Tensor
+    scores: torch.Tensor
+
+
+def ctc_beam_search(logits_tbv: torch.Tensor, input_len: torch.Tensor, beam_size: int = 32, nbest: int = 1, blank: int = 0,
+                    beam_size_token: Optional[int] = None, lm=None, lm_weight: float = 0.0, word_score: float = 0.0,
+                    unk_score: float = 0.0) -> CtcHypotheses:
+    """CTC prefix beam search over bf16 logits T x B x V (log-softmax included) with `input_len` [B] valid frames -- the inputs
+    of `forced_align` -- in one CTA per utterance (csrc/ctc_decode.cu).  The semantics are written out in
+    include/unispeech_b200.h (b200s_ctc_decode): lp = logit - logsumexp(logit) in fp32, prefixes carry
+    (pb, pnb), ranking score = logaddexp(pb, pnb) + LM part, ties to the smaller 64-bit prefix hash, the best `beam_size` kept
+    after every frame; `beam_size_token` (default all) non-blank classes of highest lp are tried per frame.
+    `lm` (`ngram.NgramLM`): at each word boundary (its `word_boundary` class after a non-empty word) the score gains
+    lm_weight * ln P(word | previous words) + word_score; a spelling the LM does not know scores as <unk> + unk_score; at the end
+    the open word and </s> are scored.  Without `lm` the score is acoustic only.
+    Limits: 1 <= beam_size <= 128, nbest <= beam_size, 2 <= V <= MAX_CLASSES.  Nothing synchronises: the call captures in a CUDA
+    graph.  The backpointer workspace, B * T * beam_size * 4 bytes, comes from the caching allocator."""
+    if not logits_tbv.is_cuda or logits_tbv.dtype != BF or logits_tbv.dim() != 3:
+        raise ValueError("ctc_beam_search: logits must be a CUDA bf16 tensor T x B x V (there is no CPU or fp32 path)")
+    if logits_tbv.stride(2) != 1:
+        raise ValueError("ctc_beam_search: the class dimension of the logits must have unit stride")
+    dev = logits_tbv.device
+    T, B, V = logits_tbv.shape
+    fs, bs = logits_tbv.stride(0), logits_tbv.stride(1)
+    input_len = _i32(input_len, dev)
+    beam_token = V - 1 if beam_size_token is None else int(beam_size_token)
+    lse = torch.empty(B, T, dtype=torch.float32, device=dev)
+    tokens = torch.empty(B, max(int(nbest), 1), T, dtype=torch.int32, device=dev)
+    lengths = torch.empty(B, max(int(nbest), 1), dtype=torch.int32, device=dev)
+    scores = torch.empty(B, max(int(nbest), 1), dtype=torch.float32, device=dev)
+    ws = ops.ctc_decode_workspace_bytes(B, T, beam_size)   # -1 past the limits: the call below then reports which one
+    workspace = torch.empty(max(ws, 1), dtype=torch.uint8, device=dev)
+    ops.ctc_stats(logits_tbv, fs, bs, input_len, B, T, V, lse, None)
+    ops.ctc_decode(logits_tbv, fs, bs, lse, input_len, B, T, V, int(blank), int(beam_size), int(nbest), beam_token,
+                   -1 if lm is None else lm.word_boundary, lm, lm_weight, word_score, unk_score, workspace, tokens, lengths, scores)
+    return CtcHypotheses(tokens, lengths, scores)
+
+
+def hypotheses_to_words(hyp: CtcHypotheses, symbols, word_boundary: int) -> List[List[List[str]]]:
+    """Host side: per utterance and n-best entry, the words of the hypothesis (its symbols joined, split at `word_boundary`,
+    empty words dropped)."""
+    tokens, lengths = hyp.tokens.cpu().tolist(), hyp.lengths.cpu().tolist()
+    out = []
+    for tb, lb in zip(tokens, lengths):
+        per = []
+        for row, n in zip(tb, lb):
+            words, cur = [], []
+            for c in row[:n]:
+                if c == word_boundary:
+                    if cur:
+                        words.append("".join(cur))
+                    cur = []
+                else:
+                    cur.append(symbols[c])
+            if cur:
+                words.append("".join(cur))
+            per.append(words)
+        out.append(per)
+    return out
 
 
 class TokenSpan(NamedTuple):

@@ -442,6 +442,31 @@ def ctc_align(logits, frame_stride, batch_stride, lse, input_len, targets, Smax,
           i32(Smax), L.ptr(target_len), i32(B), i32(T), i32(V), i32(blank), L.ptr(workspace), L.ll(workspace.numel()),
           L.ptr(labels), L.ptr(frame_scores), L.ptr(score), _s())
 
+
+# ------------------------------------------------------------------------------------------------- CTC beam-search decoding
+def ctc_decode_workspace_bytes(B, T, beam) -> int:
+    return int(L.load().b200s_ctc_decode_workspace_bytes(i32(B), i32(T), i32(beam)))
+
+
+def ctc_lm_table_build(seqs, n, width, v0, v1, keys, vals, status):
+    _call("b200s_ctc_lm_table_build", L.ptr(seqs), i32(n), i32(width), L.ptr(v0), L.ptr(v1), L.ptr(keys), L.ptr(vals),
+          L.ll(keys.numel()), L.ptr(status), _s())
+
+
+def ctc_decode(logits, frame_stride, batch_stride, lse, input_len, B, T, V, blank, beam, nbest, beam_token, word_boundary, lm,
+               lm_weight, word_score, unk_score, workspace, tokens, lengths, scores):
+    """`lm`: an `ngram.NgramLM` (its device tables and word ids) or None."""
+    if lm is None:
+        tables, (order, bos, eos, unk, has_unk) = (None, None, 0, None, None, 0), (0, 0, 0, 0, 0)
+    else:
+        tables = (lm.ngram_keys, lm.ngram_vals, lm.ngram_keys.numel(), lm.spell_keys, lm.spell_vals, lm.spell_keys.numel())
+        order, bos, eos, unk, has_unk = lm.order, lm.bos, lm.eos, lm.unk, int(lm.has_unk)
+    _call("b200s_ctc_decode", L.ptr(logits), L.ll(frame_stride), L.ll(batch_stride), L.ptr(lse), L.ptr(input_len), i32(B), i32(T),
+          i32(V), i32(blank), i32(beam), i32(nbest), i32(beam_token), i32(word_boundary), L.ptr(tables[0]), L.ptr(tables[1]),
+          L.ll(tables[2]), L.ptr(tables[3]), L.ptr(tables[4]), L.ll(tables[5]), i32(order), i32(bos), i32(eos), i32(unk),
+          i32(has_unk), f32(lm_weight), f32(word_score), f32(unk_score), L.ptr(workspace), L.ll(workspace.numel()), L.ptr(tokens),
+          L.ptr(lengths), L.ptr(scores), _s())
+
 # ------------------------------------------------------------------------------------------------- k-means pseudo-labels
 def kmeans_assign(x, x_bs, x_rs, rows, batches, D, valid, centers_bf16, cnorm, K, labels, score=None, prev_labels=None,
                   changed=None):
