@@ -708,6 +708,12 @@ class Engine:
         hg = e(B, T, Fd)
         hp = e(B, T, Fd) if save else None
         self._mm(ffn_in, D, w["w1"], Fd, hg, rag, T, B, bias=lyr.fc1.bias, gelu=2, out_pre=hp, pre_ld=Fd)  # hp = gelu'(fc1 output)
+        if rag is not None and pre_ln and save:
+            # a live tile computes its padded rows in full: there hg = gelu(b1) and hp = gelu'(b1).  A pre-LN backward feeds dout
+            # itself to fc2 (dz2 = dout), so zeroed, they keep dout at padded frames out of d fc2.weight (dz2 x hg) and
+            # d fc1.bias (column sum of dz2 W2^T * hp).  (Post-LN: the ragged final LayerNorm backward zeroes dz2 there.)
+            ops.frame_mask_fwd(hg, T * Fd, Fd, T, B, Fd, None, pad_u8, None)
+            ops.frame_mask_fwd(hp, T * Fd, Fd, T, B, Fd, None, pad_u8, None)
         if p_act > 0:  # dropout2 after the activation (WavLM/WavLM.py:711,736); the same mask folded into the stored
             # derivative makes the backward epilogue (dy * hp) the gradient through activation AND dropout
             k_act = d.key(DR.layer_site(idx, DR.L_ACTIVATION))
