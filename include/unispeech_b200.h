@@ -533,6 +533,52 @@ int b200s_ctc_decode(const void* logits, long long frame_stride, long long batch
                      float word_score, float unk_score, void* workspace, long long workspace_bytes, int* tokens, int* lengths,
                      float* scores, b200s_stream stream);
 
+/* ============================ Lexicon-constrained CTC beam search (csrc/ctc_decode_lex.cu) ============================ */
+/* b200s_ctc_decode with every word held to a lexicon (flashlight's LexiconDecoder), and the LM look-ahead of partial words in the
+ * ranking; the definition is oracle/lexicon_oracle.py.  Everything of b200s_ctc_decode above holds (lp, lae, prefix hash, stays,
+ * merges and their order, ranking ties, the backoff LM term, fp32 order of operations, outputs, workspace, limits), with these
+ * changes.
+ * Lexicon: each word has one or more spellings, sequences of non-blank classes other than word_boundary; the first word in file
+ * order keeps a spelling that several words share.  The spellings form a trie whose root (node 0) is the empty partial word.
+ * Beam state: the trie node of the partial word in place of its hash (the node is a function of the prefix).
+ * Extension of beam j by c in T_K:
+ *   c != word_boundary: allowed only if node_j has a child by c, which becomes the beam's node (also for the repeat extension
+ *   from pb; the stay pnb + lp[last] keeps the node);
+ *   c == word_boundary at the root: the empty word, allowed, scores nothing;
+ *   c == word_boundary at a node that ends word w: lm += lm_weight * ln P(w | ctx) + word_score (+ unk_score when w is not in
+ *   the LM, whose LM term is then <unk>'s, or 0 without <unk>), the node returns to the root and w (or <unk>) joins the
+ *   context.  Without an LM (order = 0) only word_score is added;
+ *   c == word_boundary at a node that ends no word: not allowed.
+ * Every allowed extension of every beam by every class of T_K is a candidate, with the stays (no min(beam_token, beam + 2)
+ * pruning).  Merges: an extension reaching an existing beam's prefix is merged into that beam's stay, as in b200s_ctc_decode.
+ * Look-ahead: smear[n] fp32 per node, 0 at the root (trie_smear null: 0 everywhere).  Ranking score =
+ * lae(pb, pnb) + (lm + lm_weight * smear[node]), each operation rounded to fp32 in that order; lm holds completed words only.
+ * unispeech_b200.lexicon computes smear[n] = max over the words w ending at n or below it of ln P(w | <s>) (w as <unk>, or 0
+ * without <unk>, when not in the LM), with ln_prob's order (log10 terms summed in fp32, then * ln 10); 0 without an LM.
+ * End of utterance: at a node that ends a word, that word is scored as at a boundary, then lm += lm_weight * ln P(</s> | ctx);
+ * at the root only </s>; at a node that ends no word the hypothesis is dropped.  The n-best are the survivors by (score desc,
+ * hash asc); entries past them have length 0 and score -inf.
+ * Trie arrays (device, nodes in BFS order, the children of a node contiguous and in class order):
+ *   trie_mask uint32 [nodes, ceil(V / 32)]  bit c of node n: n has a child by class c;
+ *   trie_first_child int32 [nodes]          index of n's first child; its child by c is first_child + (mask bits below c);
+ *   trie_word int32 [nodes]                 -1: n ends no word, -2: a word the LM does not know, else the LM word id (any
+ *                                           value >= 0 without an LM);
+ *   trie_smear fp32 [nodes] or null.
+ * b200s_ctc_trie_bytes(nodes, V) = nodes * (4 * ceil(V / 32) + 12).  The kernel trusts the arrays' contents
+ * (unispeech_b200.lexicon builds and checks them); null arrays and a node count outside [1, B200S_CTC_TRIE_MAX_NODES] are
+ * rejected before any launch, with the checks of b200s_ctc_decode (word_boundary is required).  Candidates per frame:
+ * at most beam * (beam_token + 1) <= 128 * 1024, enumerated by index and not stored, so no further limit applies.  Dynamic
+ * shared memory: beam * ceil(V / 32) * 10 bytes. */
+#define B200S_CTC_TRIE_MAX_NODES (1 << 30)
+long long b200s_ctc_trie_bytes(long long nodes, int V); /* -1 for bad sizes */
+int b200s_ctc_decode_lexicon(const void* logits, long long frame_stride, long long batch_stride, const float* lse,
+                             const int* input_len, int B, int T, int V, int blank, int beam, int nbest, int beam_token,
+                             int word_boundary, const void* lm_keys, const void* lm_vals, long long lm_capacity, int order, int bos,
+                             int eos, int unk, int has_unk, float lm_weight, float word_score, float unk_score,
+                             const uint32_t* trie_mask, const int* trie_first_child, const int* trie_word,
+                             const float* trie_smear, long long trie_nodes, void* workspace, long long workspace_bytes,
+                             int* tokens, int* lengths, float* scores, b200s_stream stream);
+
 /* ============================ k-means pseudo-labels (csrc/kmeans.cu) ============================ */
 /* Nearest-centroid labels, Lloyd updates and k-means++ seeding over bf16 features (the label stage of HuBERT-style pre-training).
  * Centres: fp32 master [K, D]; the bf16 copy the assignment multiplies, [Kp, D] with Kp = K rounded up to a multiple of 256 (rows

@@ -14,7 +14,8 @@ src/fairseq/models/wav2vec/wav2vec2_asr.py `Wav2VecCtc`).
     `MAX_ALIGN_TARGET` labels.  `token_spans` turns its paths into per-token frame spans (`torchaudio.functional.merge_tokens`).
   * `ctc_beam_search(logits_tbv, input_len, beam_size, nbest, blank, beam_size_token, lm, lm_weight, word_score, unk_score)`:
     batched CTC prefix beam search (csrc/ctc_decode.cu) with an optional word n-gram LM (`ngram.NgramLM.from_arpa`) scored at
-    word boundaries, lexicon-free; `hypotheses_to_words` spells the result.
+    word boundaries, lexicon-free, or with `lexicon` (`lexicon.Lexicon.from_file`) held to a word lexicon with LM look-ahead
+    (csrc/ctc_decode_lex.cu); `hypotheses_to_words` spells the result.
   * `HubertCtc` / `Wav2VecCtc`: `w2v_encoder` = `HubertEncoder` / `Wav2VecEncoder`, `forward(**net_input)`, `get_logits`,
     `get_normalized_probs`, `set_num_updates`; `state_dict` keys `w2v_encoder.w2v_model.*`, `w2v_encoder.proj.*`.
 
@@ -193,7 +194,7 @@ class CtcHypotheses(NamedTuple):
 
 def ctc_beam_search(logits_tbv: torch.Tensor, input_len: torch.Tensor, beam_size: int = 32, nbest: int = 1, blank: int = 0,
                     beam_size_token: Optional[int] = None, lm=None, lm_weight: float = 0.0, word_score: float = 0.0,
-                    unk_score: float = 0.0) -> CtcHypotheses:
+                    unk_score: float = 0.0, lexicon=None) -> CtcHypotheses:
     """CTC prefix beam search over bf16 logits T x B x V (log-softmax included) with `input_len` [B] valid frames -- the inputs
     of `forced_align` -- in one CTA per utterance (csrc/ctc_decode.cu).  The semantics are written out in
     include/unispeech_b200.h (b200s_ctc_decode): lp = logit - logsumexp(logit) in fp32, prefixes carry
@@ -202,6 +203,11 @@ def ctc_beam_search(logits_tbv: torch.Tensor, input_len: torch.Tensor, beam_size
     `lm` (`ngram.NgramLM`): at each word boundary (its `word_boundary` class after a non-empty word) the score gains
     lm_weight * ln P(word | previous words) + word_score; a spelling the LM does not know scores as <unk> + unk_score; at the end
     the open word and </s> are scored.  Without `lm` the score is acoustic only.
+    `lexicon` (`lexicon.Lexicon`, built for this `lm` or for none, csrc/ctc_decode_lex.cu): every word must be a lexicon word
+    (flashlight's LexiconDecoder).  An extension must follow an edge of the lexicon's trie, a boundary may only end a lexicon
+    word (scored as above, or by word_score alone without `lm`), a hypothesis that ends inside a word is dropped, and every
+    allowed extension of every beam by the `beam_size_token` classes is tried.  With smearing="max" the ranking adds
+    lm_weight * the best ln P(w | <s>) of the words the partial word can still become.
     Limits: 1 <= beam_size <= 128, nbest <= beam_size, 2 <= V <= MAX_CLASSES.  Nothing synchronises: the call captures in a CUDA
     graph.  The backpointer workspace, B * T * beam_size * 4 bytes, comes from the caching allocator."""
     if not logits_tbv.is_cuda or logits_tbv.dtype != BF or logits_tbv.dim() != 3:
@@ -217,9 +223,16 @@ def ctc_beam_search(logits_tbv: torch.Tensor, input_len: torch.Tensor, beam_size
     tokens = torch.empty(B, max(int(nbest), 1), T, dtype=torch.int32, device=dev)
     lengths = torch.empty(B, max(int(nbest), 1), dtype=torch.int32, device=dev)
     scores = torch.empty(B, max(int(nbest), 1), dtype=torch.float32, device=dev)
+    if lexicon is not None:
+        lexicon.check(V, lm, dev, int(blank))
     ws = ops.ctc_decode_workspace_bytes(B, T, beam_size)   # -1 past the limits: the call below then reports which one
     workspace = torch.empty(max(ws, 1), dtype=torch.uint8, device=dev)
     ops.ctc_stats(logits_tbv, fs, bs, input_len, B, T, V, lse, None)
+    if lexicon is not None:
+        ops.ctc_decode_lexicon(logits_tbv, fs, bs, lse, input_len, B, T, V, int(blank), int(beam_size), int(nbest), beam_token,
+                               lexicon.word_boundary, lm, lm_weight, word_score, unk_score, lexicon, workspace, tokens, lengths,
+                               scores)
+        return CtcHypotheses(tokens, lengths, scores)
     ops.ctc_decode(logits_tbv, fs, bs, lse, input_len, B, T, V, int(blank), int(beam_size), int(nbest), beam_token,
                    -1 if lm is None else lm.word_boundary, lm, lm_weight, word_score, unk_score, workspace, tokens, lengths, scores)
     return CtcHypotheses(tokens, lengths, scores)

@@ -5,6 +5,7 @@ kernel (csrc/ctc_decode.cu, `b200s_ctc_lm_table_build`).
   * spelling table: key = hash of a word's class ids -> word id.  Each character of a word maps to the class whose symbol is
     that character; words with a character no single-character symbol spells are left out (`dropped` counts them).
 
+`NgramLM.start_ln` (host, fp32 per word id) holds ln P(w | <s>), from which `lexicon.Lexicon` builds its look-ahead.
 Word ids are the order of the unigram section.  <s> and </s> must be unigrams; <unk> is optional (without it an unknown spelling
 has no LM term, only `unk_score`).  Limits: order <= 5, fewer than 2^24 words.  A malformed file raises ValueError.
 """
@@ -171,4 +172,23 @@ class NgramLM:
         if st:
             raise ValueError(f"{path}: the 64-bit hash of two different n-grams or spellings collided (status {st}); "
                              "the tables cannot hold this LM")
-        return cls(order, words, word_ids, ng_keys, ng_vals, sp_keys, sp_vals, ("<unk>",) in grams[0], dropped, word_boundary)
+        lm = cls(order, words, word_ids, ng_keys, ng_vals, sp_keys, sp_vals, ("<unk>",) in grams[0], dropped, word_boundary)
+        lm.start_ln = start_log_probs(order, grams, words)
+        return lm
+
+
+def start_log_probs(order: int, grams, words: Sequence[str]) -> np.ndarray:
+    """fp32 [len(words)]: ln P(w | <s>) of every word id, in the device's `ln_prob` order (log10 backoff of <s> when the bigram
+    (<s>, w) is missing, then the log10 p, summed in fp32 from 0, then * ln 10 in fp32).  The look-ahead of a lexicon's trie
+    (`lexicon.Lexicon`) is built from these."""
+    f32 = np.float32
+    p1 = np.asarray([grams[0][(w,)][0] for w in words], dtype=f32)
+    if order > 1:
+        acc = (f32(0.0) + f32(grams[0][("<s>",)][1])) + p1
+        ids = {w: i for i, w in enumerate(words)}
+        for (a, w), (p, _) in grams[1].items():
+            if a == "<s>":
+                acc[ids[w]] = f32(0.0) + f32(p)
+    else:
+        acc = f32(0.0) + p1
+    return (acc.astype(f32) * f32(2.302585092994046)).astype(f32)

@@ -467,6 +467,23 @@ def ctc_decode(logits, frame_stride, batch_stride, lse, input_len, B, T, V, blan
           i32(has_unk), f32(lm_weight), f32(word_score), f32(unk_score), L.ptr(workspace), L.ll(workspace.numel()), L.ptr(tokens),
           L.ptr(lengths), L.ptr(scores), _s())
 
+def ctc_decode_lexicon(logits, frame_stride, batch_stride, lse, input_len, B, T, V, blank, beam, nbest, beam_token, word_boundary,
+                       lm, lm_weight, word_score, unk_score, lexicon, workspace, tokens, lengths, scores):
+    """`lm`: an `ngram.NgramLM` or None; `lexicon`: a `lexicon.Lexicon` (its trie arrays; the look-ahead only with
+    smearing="max" and an LM)."""
+    if lm is None:
+        keys, vals, cap, order, bos, eos, unk, has_unk = None, None, 0, 0, 0, 0, 0, 0
+    else:
+        keys, vals, cap = lm.ngram_keys, lm.ngram_vals, lm.ngram_keys.numel()
+        order, bos, eos, unk, has_unk = lm.order, lm.bos, lm.eos, lm.unk, int(lm.has_unk)
+    smear = lexicon.smear if lm is not None and lexicon.smearing == "max" else None
+    _call("b200s_ctc_decode_lexicon", L.ptr(logits), L.ll(frame_stride), L.ll(batch_stride), L.ptr(lse), L.ptr(input_len), i32(B),
+          i32(T), i32(V), i32(blank), i32(beam), i32(nbest), i32(beam_token), i32(word_boundary), L.ptr(keys), L.ptr(vals),
+          L.ll(cap), i32(order), i32(bos), i32(eos), i32(unk), i32(has_unk), f32(lm_weight), f32(word_score), f32(unk_score),
+          L.ptr(lexicon.mask), L.ptr(lexicon.first_child), L.ptr(lexicon.word), L.ptr(smear), L.ll(lexicon.nodes),
+          L.ptr(workspace), L.ll(workspace.numel()), L.ptr(tokens), L.ptr(lengths), L.ptr(scores), _s())
+
+
 # ------------------------------------------------------------------------------------------------- k-means pseudo-labels
 def kmeans_assign(x, x_bs, x_rs, rows, batches, D, valid, centers_bf16, cnorm, K, labels, score=None, prev_labels=None,
                   changed=None):
